@@ -1,13 +1,14 @@
 """Headline benchmark (driver contract): shallow-water steps/s on a 4096x4096 grid.
 
 BASELINE.json metric: "allreduce bus GB/s vs message size and shallow_water.py steps/sec
-(whole box, device-timed, max over ranks) at 1/2/4/8 B200".  ``value`` is the shallow-water
+(whole box, device-timed, max over ranks) at 1/2/4/8 GPUs".  ``value`` is the shallow-water
 throughput (defined for every N, including N=1); the allreduce bus-bandwidth sweep (N>1)
 is reported in the extra key ``allreduce_busbw_gbs``.
 
     python bench.py --gpus N --steps K --warmup W            # N=1 directly
     python -m torch.distributed.run --nproc-per-node N ... bench.py --gpus N ...   # N>1
     python bench.py --impl reference                          # reference arm
+    python bench.py --dump-outputs DIR                        # + the final state as DIR/*.npy
 
 * device-timed with CUDA events on the launching stream, barrier + synchronize on both
   sides, max over ranks; W untimed warm-up steps, exactly K timed steps;
@@ -17,7 +18,12 @@ is reported in the extra key ``allreduce_busbw_gbs``.
 * ``e2e``: the same K steps through the public API, in chunks of ``e2e_chunk_steps`` model
   steps (the reference's ``do_multistep(state, 100)`` call granularity); every chunk copies
   the model state host->device from pinned memory and reads the surface-height snapshot back
-  device->host, timed by the wall clock between barriers.
+  device->host, timed by the wall clock between barriers;
+* ``--dump-outputs DIR``: the model state (h, u, v, dh, du, dv) after the last timed step, as
+  float32 ``DIR/<field>.npy`` (``<field>_rank<r>.npy`` per rank when N > 1).  Each rank writes the
+  same fixed, seeded sample of DUMP_SAMPLES // N cells of its local block for every field (all cells
+  when the block is smaller), so the files of two builds run with the same arguments compare value
+  by value, and all files together hold at most 6 x 4 x DUMP_SAMPLES bytes = 24 MiB at any N.
 """
 
 from __future__ import annotations
@@ -35,6 +41,7 @@ sys.path.insert(0, REPO)
 GRID = 4096
 # published reference numbers (BASELINE.md): 3600x1800 grid on Tesla P100, derived steps/s
 BASELINE_STEPS_PER_S = {1: 80.0, 2: 129.0}
+DUMP_SAMPLES = 1 << 20          # cells per field over all ranks: 6 fields x 4 MiB in total
 
 
 def reference_arm() -> int:
@@ -63,6 +70,8 @@ def main() -> int:
     ap.add_argument("--impl", default="ours", choices=["ours", "reference"])
     ap.add_argument("--grid", type=int, default=GRID)
     ap.add_argument("--no-sweep", action="store_true", help="skip the allreduce sweep extras")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the model state after the last timed step as DIR/<field>.npy")
     ns = ap.parse_args()
     if ns.impl == "reference":
         return reference_arm()
@@ -154,7 +163,7 @@ def main() -> int:
         # device timeline -- the rest was the host getting from `start.record()` to `cudaGraphLaunch`
         # while eight `nvidia-smi` clock queries started next to it; the clocks are now read through
         # in-process NVML, and the end-to-end number below accounts for launch latency separately).
-        torch.cuda._sleep(int(4e7))                 # ~20 ms at 1.9 GHz: also covers a descheduled rank process
+        torch.cuda._sleep(int(4e7))                 # ~20 ms at 2 GHz: also covers a descheduled rank process
         # device-side barrier on the stream right before the start event: the ranks' timed windows
         # open together on the GPUs, whatever skew the host-side barrier left between the processes
         m.barrier(comm=comm)
@@ -162,6 +171,7 @@ def main() -> int:
         gpu_launches = run_steps(K)
         end.record()
         torch.cuda.synchronize()
+        final_state = [t.clone() for t in model.state] if ns.dump_outputs else None
         if start.elapsed_time(end) < 400:           # keep the GPU under load long enough to sample
             t_end = time.time() + 0.5
             while time.time() < t_end:
@@ -172,6 +182,9 @@ def main() -> int:
     steps_per_s = K / (ms * 1e-3)
     nproc_y, nproc_x, ny_local, nx_local, pipeline = (model.nproc_y, model.nproc_x, model.ny_local, model.nx_local,
                                                       model.pipeline)
+    if final_state is not None:
+        dump_outputs(ns.dump_outputs, model.state._fields, final_state, rank, size)
+        del final_state
     finite = bool(torch.isfinite(model.h).all().item())
     mass = model.total_mass().item()
     checks["finite"] = finite
@@ -275,7 +288,8 @@ def main() -> int:
                 "seq_len": None,
                 "parallelism": f"2-D domain decomposition {nproc_y}x{nproc_x}",
                 "l2": ("L2 flushed before the timed region; per-rank state "
-                       f"{13 * ny_local * nx_local * 4 / 2**20:.0f} MiB vs 126 MiB L2"),
+                       f"{13 * ny_local * nx_local * 4 / 2**20:.0f} MiB vs "
+                       f"{torch.cuda.get_device_properties(dev).L2_cache_size / 2**20:.0f} MiB L2"),
                 "graph_chunk_steps": C,
                 "kernel_path": pipeline,
                 "baseline_note": ("vs_baseline divides by the reference's published P100 numbers for "
@@ -302,6 +316,26 @@ def main() -> int:
         print(json.dumps(out))
     m.flush()
     return 0
+
+
+def dump_outputs(out_dir, names, state, rank, size):
+    """float32 ``out_dir/<name>.npy`` per state field: a seeded sample of DUMP_SAMPLES // size flat
+    indices of this rank's block, the same in every run and for every field, in ascending order."""
+    import numpy as np
+    import torch
+
+    os.makedirs(out_dir, exist_ok=True)
+    numel = state[0].numel()
+    idx = None
+    per_rank = DUMP_SAMPLES // size
+    if numel > per_rank:
+        gen = torch.Generator().manual_seed(20240601)
+        idx = torch.randperm(numel, generator=gen)[:per_rank].sort().values.to(state[0].device)
+    for name, t in zip(names, state):
+        flat = t.reshape(-1)
+        vals = (flat if idx is None else flat[idx]).float().cpu().numpy()
+        suffix = f"_rank{rank}" if size > 1 else ""
+        np.save(os.path.join(out_dir, f"{name}{suffix}.npy"), vals)
 
 
 def correctness_checks(m, MPI, comm, dev):

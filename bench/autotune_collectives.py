@@ -1,7 +1,7 @@
 """Measure the transport crossovers of the GPU collectives for THIS job's world size on THIS box and write
 a tuning file (mpi4jax_b200/_src/tuning.py explains the keys and how the file is picked up).
 
-    python -m mpi4jax_b200.run -n 8 bench/autotune_collectives.py --out mpi4jax_b200/_src/tuning_tables/NVIDIA_B200.json
+    python -m mpi4jax_b200.run -n 8 bench/autotune_collectives.py --out mpi4jax_b200/_src/tuning_tables/NVIDIA_H100_80GB_HBM3.json
 
 For every message size (1 KiB .. 64 MiB, powers of two) the allreduce is timed with each forced transport
 (`algorithm="ll" | "oneshot" | "twoshot" | "nvls"`), bcast with the multicast path forced on and off; device

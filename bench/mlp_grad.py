@@ -6,7 +6,7 @@ gradient correctness), data-parallel and tensor-parallel, eager and under ``mpi4
   both collectives, update.  The reference's counterpart is ``jax.grad`` of a jitted loss that
   calls ``mpi4jax.allreduce`` / ``bcast`` (README.rst:59-96, tests/collective_ops/test_allreduce.py:141-223).
 * tp: first layer column-sharded, second layer row-sharded; in bf16 the row-parallel GEMM and its
-  allreduce are ONE tcgen05 + multimem kernel (csrc/b2_gemm.cu).
+  allreduce are ONE wgmma + multimem kernel (csrc/b2_gemm.cu).
 
 Device-timed (CUDA events on the launching stream, barrier + synchronize before, max over ranks).
 

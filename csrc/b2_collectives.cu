@@ -115,11 +115,10 @@ __device__ __forceinline__ void move_stage(const B2MoveArgs& a, char* mine, cons
 }
 
 // Pull chunk [off, off + len) from the peers' staging into the output AND stage chunk [noff, noff + nlen)
-// of this rank's input, in ONE loop: the NVLink loads (~3 us round trip) and the local HBM loads of a
+// of this rank's input, in ONE loop: the NVLink loads (microseconds of round trip) and the local HBM loads of a
 // thread are in flight together, U vectors each -- a CTA is one per SM (co-residency, pick_chunks), so
-// what it cannot overlap inside a thread it cannot overlap at all.  Measured before (2 GPUs, 256 MiB,
-// profiles/r2_bw_probe_n2.log): 460 GB/s for every collective, proportional to the CTA count, next to
-// 625 GB/s for the p2p ring on 64 CTAs -- latency-bound phases in a row, not the link.
+// what it cannot overlap inside a thread it cannot overlap at all: latency-bound phases in a row, not the
+// link, would otherwise bound the bandwidth.
 template <int NS, int NI, int U, bool SPLIT>
 __device__ __noinline__ void move_pull_and_stage(const B2DevComm& c, const B2MoveArgs& a, const size_t par,
                                                  char* mine, const char* in, char* out, const size_t off,
@@ -566,7 +565,7 @@ static size_t round_up(size_t x, size_t m) { return (x + m - 1) / m * m; }
 // so the block-paired barriers cannot wait for a CTA that has not been scheduled yet (if other work
 // owns the SMs the launch starts late, it does not deadlock: tests/test_coresidency.py).  The 64-register
 // kernels (NVLS allreduce, multicast bcast, reduce-to-root) fit twice per SM -- and their bandwidth
-// is proportional to the CTA count up to the link limit (profiles/r2_bw_probe_*.log).
+// grows with the CTA count up to the link limit.
 #include <map>
 static int coresident_blocks(const B2Comm* c, const void* kernel) {
   static std::map<const void*, int> per_sm;

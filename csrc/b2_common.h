@@ -17,7 +17,7 @@
 #include <cstdint>
 
 #define B2_ABI_VERSION 10   // bump whenever a struct shared with Python or a C signature changes
-#define B2_MAX_RANKS 16          // ranks per NVLink domain we support (8 on HGX B200)
+#define B2_MAX_RANKS 16          // ranks per NVLink domain we support (8 on HGX H100)
 #define B2_MAX_BLOCKS 1024       // max CTAs per collective launch (flag rows)
 #define B2_P2P_NSLOT 8           // ring slots per directed pair
 #define B2_P2P_MAX_LANES 64      // CTAs cooperating on one p2p message

@@ -1,15 +1,15 @@
 // mpi4jax_b200 -- tile order of the persistent GEMM kernels (csrc/b2_gemm.cu).
 //
 // tile index -> (m_blk, n_blk).  Group 0: row-major over the tile grid.  B2_GEMM_RASTER_GROUP = G > 0: tiles are visited in bands of G
-// M-blocks, column by column inside a band, so that the ~148 tiles in flight cover G rows x ~148/G
-// columns of the tile grid: A row-panels are reused ~148/G times and B column-panels G times from
-// L2 instead of (148 / num_n) rows x all columns (B larger than L2 at 8192^3).  Every rank uses
+// M-blocks, column by column inside a band, so that the ~132 tiles in flight (one per H100 SM) cover G rows
+// x ~132/G columns of the tile grid: A row-panels are reused ~132/G times and B column-panels G times from
+// L2 instead of (132 / num_n) rows x all columns (B larger than L2 at 8192^3).  Every rank uses
 // the same order (the fused all-reduce pairs tile t of all ranks).
 #pragma once
 
 #ifndef B2_GEMM_RASTER_GROUP
-#define B2_GEMM_RASTER_GROUP 2     // measured (profiles/r2_gemm_raster_sweep_1gpu.log): never slower than row-major,
-#endif                               // +6 % at 2048x4096x4096, +12 % at 16384x8192x4096
+#define B2_GEMM_RASTER_GROUP 2
+#endif
 
 
 #ifdef __CUDACC__

@@ -1,7 +1,7 @@
 // mpi4jax_b200 -- kernel launch helper with programmatic dependent launch (PDL).
 //
 // The shallow-water step is 7 short kernels (4 stencils + 3 halo exchanges); at 8 GPUs each is
-// 4-9 us, so the ~2 us launch/drain gap between stream-ordered kernels is a measurable part of
+// short enough that the launch/drain gap between stream-ordered kernels is a visible part of
 // the step.  With PDL the next kernel's CTAs are scheduled while the previous kernel drains and
 // block in `griddepcontrol.wait` until its memory is visible: same semantics, shorter gaps.
 // Works in eager mode and inside CUDA-graph capture (programmatic edges).  Every kernel launched

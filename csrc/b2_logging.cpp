@@ -32,7 +32,7 @@ extern "C" void b2_set_error(const char* fmt, ...) {
   va_end(ap);
 }
 extern "C" const char* b2_last_error(void) { return g_last_error; }
-extern "C" const char* b2_version(void) { return "mpi4jax_b200-native 0.1 (sm_100a)"; }
+extern "C" const char* b2_version(void) { return "mpi4jax_b200-native 0.1 (sm_90a)"; }
 extern "C" void b2_set_logging(int enable) { g_logging = enable ? 1 : 0; }
 extern "C" int b2_get_logging(void) { return g_logging; }
 extern "C" void b2_set_print_callback(b2_print_fn fn) { g_print = fn; }

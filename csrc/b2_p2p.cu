@@ -72,6 +72,7 @@ struct B2P2PArgs {
   int recv_lanes;      // 0 = no recv role
   B2StatusRecord* status;
   int opcode;
+  int anysource_scan;  // communicator option "p2p_anysource_scan" (see p2p_scan)
 };
 
 // ---- flag-in-data transport of small messages ---------------------------------------------------
@@ -238,15 +239,11 @@ __device__ unsigned p2p_match(const B2DevComm& c, const B2P2PArgs& a, int src, u
   }
 }
 
-// B2_P2P_ANYSOURCE_SCAN=1: an ANY_SOURCE receive with a tag looks as deep into every source's
-// window as a receive from a named source does (p2p_scan), instead of at the oldest pending message
-// of each source only.  Default 0 = the code that ran on hardware; the scanning variant is mirrored
-// by the model in tests/_p2p_sim.py (Inbox) and waits for its first GPU run.
-#ifndef B2_P2P_ANYSOURCE_SCAN
-#define B2_P2P_ANYSOURCE_SCAN 0
-#endif
-
-#if B2_P2P_ANYSOURCE_SCAN
+// Communicator option "p2p_anysource_scan" = 1: an ANY_SOURCE receive with a tag looks as deep into
+// every source's window as a receive from a named source does (p2p_scan), instead of at the oldest
+// pending message of each source only (the default).  The scanning variant is mirrored by the model
+// in tests/_p2p_sim.py (Inbox).
+//
 // Non-blocking single pass of the scan in p2p_match: does source `src` hold a message that a
 // receive with tag a.recv_tag may take right now?  (A streamed message that is not at the head is
 // "not available" here -- another source may match -- whereas p2p_match treats it as an error.)
@@ -275,7 +272,6 @@ __device__ bool p2p_scan(const B2DevComm& c, const B2P2PArgs& a, int src) {
   }
   return false;
 }
-#endif
 
 __device__ void p2p_recv_role(const B2DevComm& c, const B2P2PArgs& a, int lane) {
   __shared__ int s_src, s_tag;
@@ -293,21 +289,21 @@ __device__ void p2p_recv_role(const B2DevComm& c, const B2P2PArgs& a, int lane) 
         unsigned spins = 0;
         int probe = 0;
         while (src < 0) {
-#if B2_P2P_ANYSOURCE_SCAN
-          if (p2p_scan(c, a, probe)) {
-            src = probe;
-            break;
+          if (a.anysource_scan) {
+            if (p2p_scan(c, a, probe)) {
+              src = probe;
+              break;
+            }
+          } else {
+            const unsigned want = b2_ld_volatile(c.p2p_recv_seq + probe);
+            const unsigned* h =
+                hdr_base + (((size_t)probe * B2_P2P_NSLOT + want % B2_P2P_NSLOT) * B2_P2P_MAX_LANES) * 4;
+            if (b2_ld_acquire_sys(h) == want + 1u &&
+                (a.recv_tag < 0 || (int)b2_ld_volatile(h + 1) == a.recv_tag)) {
+              src = probe;
+              break;
+            }
           }
-#else
-          const unsigned want = b2_ld_volatile(c.p2p_recv_seq + probe);
-          const unsigned* h =
-              hdr_base + (((size_t)probe * B2_P2P_NSLOT + want % B2_P2P_NSLOT) * B2_P2P_MAX_LANES) * 4;
-          if (b2_ld_acquire_sys(h) == want + 1u &&
-              (a.recv_tag < 0 || (int)b2_ld_volatile(h + 1) == a.recv_tag)) {
-            src = probe;
-            break;
-          }
-#endif
           probe = (probe + 1) % c.size;
           if ((++spins & 0xfffu) == 0) {
             unsigned long long now = b2_gtime();
@@ -455,6 +451,7 @@ static int launch_p2p(B2Comm* c, B2P2PArgs& a, const char* name, cudaStream_t st
     b2_set_error("%s: invalid source rank %d (communicator size %d)", name, a.source, P);
     return B2_ERR_BAD_ARG;
   }
+  a.anysource_scan = c->p2p_anysource_scan;
   b2_k_p2p<<<a.send_lanes + a.recv_lanes, B2_THREADS, 0, stream>>>(c->dev, a);
   b2_count_launch(c);
   cudaError_t err = cudaGetLastError();

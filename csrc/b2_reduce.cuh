@@ -2,7 +2,7 @@
 //
 // Replaces the reference's MPI_Allreduce / MPI_Reduce / MPI_Scan call sites
 // (mpi4jax/_src/xla_bridge/mpi_ops_common.h:236-249, 310-338 and their CUDA
-// callers mpi_xla_bridge_cuda.cpp:167-209, 523-632) with hand-written sm_100a
+// callers mpi_xla_bridge_cuda.cpp:167-209, 523-632) with hand-written sm_90a
 // kernels in which the reduction operator and the dtype up/down-cast are FUSED
 // into the NVLink transfer: no MPI call, no host sync, no staging through host
 // memory, no separate elementwise kernel.

@@ -4,7 +4,7 @@
 // cudaGetDriverEntryPoint so that the shared library has no link-time
 // dependency on libcuda.so (it must import on GPU-less build hosts).
 //
-// Parity: this file is the B200 counterpart of what the reference delegates to
+// Parity: this file is the H100 counterpart of what the reference delegates to
 // the MPI library + mpi4py handles (mpi4jax/_src/utils.py:60-97) and to
 // mpi_xla_bridge_cuda.cpp's cudaMemcpy staging (:55-67, :185-206): here the
 // "communicator" is a set of peer-mapped HBM segments, flags and counters.
@@ -425,15 +425,15 @@ extern "C" B2Comm* b2_comm_create(int device, int rank, int nranks, B2Seg* ctl, 
   void* edev = nullptr;
   cudaHostGetDevicePointer(&edev, (void*)eh, 0);
   d.err = (B2ErrorRecord*)edev;
-  // measured on 8 x B200 (profiles/r1_collectives_sweep_8gpu_v1.json): LL wins up to its 64 KiB
-  // buffer limit (7-12 us vs 13+), in-switch reduction wins from there on, one-shot beats
-  // two-shot up to ~512 KiB when multicast is unavailable
+  // LL up to its 64 KiB buffer limit, in-switch reduction from there on, one-shot before two-shot
+  // up to 512 KiB when multicast is unavailable (per world size: mpi4jax_b200/_src/tuning.py)
   c->ll_max = 64 * 1024;
   c->oneshot_max = 512 * 1024;
   c->nvls_min = 64 * 1024 + 1;
   c->bcast_mc_min = 256 * 1024;
   c->nvls_pipeline = 1;
   c->gemm_raster = -1;
+  c->p2p_anysource_scan = 0;
   c->trace = nullptr;
   c->trace_cap = 0;
   // one 512-thread CTA of the collective kernels (<= 128 registers per thread) fits per SM: grids are
@@ -469,6 +469,7 @@ extern "C" int b2_comm_set_option(B2Comm* c, const char* key, long long value) {
   if (strcmp(key, "bcast_mc_min") == 0) c->bcast_mc_min = (size_t)value;
   else if (strcmp(key, "nvls_pipeline") == 0) c->nvls_pipeline = value != 0;
   else if (strcmp(key, "gemm_raster") == 0) c->gemm_raster = (int)value;
+  else if (strcmp(key, "p2p_anysource_scan") == 0) c->p2p_anysource_scan = value != 0;
   else if (strcmp(key, "trace_ptr") == 0) c->trace = (unsigned long long*)(uintptr_t)value;
   else if (strcmp(key, "trace_cap") == 0) c->trace_cap = (int)value;
   else { b2_set_error("unknown communicator option '%s'", key); return B2_ERR_BAD_ARG; }
@@ -482,6 +483,7 @@ extern "C" long long b2_comm_get_option(B2Comm* c, const char* key) {
   if (strcmp(key, "bcast_mc_min") == 0) return (long long)c->bcast_mc_min;
   if (strcmp(key, "nvls_pipeline") == 0) return c->nvls_pipeline ? 1 : 0;
   if (strcmp(key, "gemm_raster") == 0) return c->gemm_raster < 0 ? 0 : c->gemm_raster;
+  if (strcmp(key, "p2p_anysource_scan") == 0) return c->p2p_anysource_scan;
   b2_set_error("unknown communicator option '%s'", key);
   return -1;
 }
@@ -522,7 +524,7 @@ extern "C" int b2_comm_destroy(B2Comm* c) {
 
 // ---------------------------------------------------------------------------
 // TMA descriptor for a row-major (rows x cols) bf16 matrix, box = box_rows x box_cols,
-// 128-byte swizzle (what the tcgen05 K-major SWIZZLE_128B shared-memory descriptor expects)
+// 128-byte swizzle (what the wgmma K-major SWIZZLE_128B shared-memory descriptor expects)
 // ---------------------------------------------------------------------------
 extern "C" int b2_tensor_map_2d_bf16(CUtensorMap* out, const void* ptr, unsigned long long rows,
                                      unsigned long long cols, unsigned box_rows, unsigned box_cols) {

@@ -10,7 +10,7 @@
 // B2Comm  : a communicator: rank/size, control segment (flags, p2p rings, LL
 //           buffers, halo buffers), growable staging segment, local counters.
 //
-// This is the B200-native counterpart of the reference's native bridge layer
+// This is the H100-native counterpart of the reference's native bridge layer
 // (mpi4jax/_src/xla_bridge/mpi_xla_bridge_cuda.cpp + mpi_ops_common.h); the
 // reference hands device pointers to a CUDA-aware MPI, we own the transport.
 #pragma once
@@ -55,6 +55,7 @@ struct B2Comm {
   size_t bcast_mc_min;          // bcast: root multimem.st from this size on
   int nvls_pipeline;            // software-pipelined NVLS allreduce (default on)
   int gemm_raster;              // tile order of the persistent GEMM: -1 = compile-time default, 0 = row-major, G = bands
+  int p2p_anysource_scan;       // ANY_SOURCE + tag receives scan every source's window (default off, b2_p2p.cu)
   unsigned long long* trace;    // device buffer for the phase timeline of CTA 0 (scripts/allreduce_phases.py)
   int trace_cap;
   int max_blocks;
@@ -158,7 +159,7 @@ int b2_sendrecv(B2Comm* c, const void* sendbuf, size_t send_bytes, int dest, int
                 void* recvbuf, size_t recv_bytes, int source, int recvtag, B2StatusRecord* status,
                 cudaStream_t stream);
 
-// --- tensor-parallel linear: tcgen05 GEMM + in-switch allreduce in one kernel (b2_gemm.cu) ---
+// --- tensor-parallel linear: wgmma GEMM + in-switch allreduce in one kernel (b2_gemm.cu) ---
 int b2_gemm_allreduce(B2Comm* c, const void* A, const void* B, void* out, int M, int N, int K,
                       cudaStream_t stream);
 

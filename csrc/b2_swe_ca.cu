@@ -13,7 +13,7 @@
 // what Fb(t) wrote next to the frame).  Only h is double-buffered (its stencil is read while h' is written);
 // u', v' travel through their own arrays between the tendency and the friction kernels, so u'', v''
 // and the tendencies are updated in place: nine arrays are live per step -- at 8 GPUs (2 M cells per
-// rank) 75 MB, which stays in the 126 MB L2.  The NVLink round of X is
+// rank) 75 MB, more than the 50 MB L2 of an H100, so fewer passes means less HBM traffic.  The NVLink round of X is
 // hidden behind the bulk kernels.  Under CUDA-graph capture (mpi4jax_b200.jit) the event fork /
 // join becomes graph edges.  16 array passes per step instead of 32, one exchange instead of three.
 #include <cstdio>
@@ -49,7 +49,7 @@ __device__ __forceinline__ void ca_stamp_end(const CAStamp& s) {
 // ---- frame kernels -------------------------------------------------------------------------------
 // The frame is a few thousand cells and sits on the step's critical path: latency, not throughput.
 // A thread per cell would evaluate 14 flux quantities (kernel A) or 3 friction stencils (kernel D) one
-// after the other -- ~4000 dependent-issue instructions, measured 18 us.  Instead a CTA takes 32 cells
+// after the other -- ~4000 dependent-issue instructions on the critical path.  Instead a CTA takes 32 cells
 // and one WARP per kind of quantity: warp w evaluates the fluxes of kind w (fe / fn / q / ke; u'' of
 // the cell / its west / its south neighbour in kernel D) for the 32 cells -- no divergence inside a
 // warp --, the values meet in shared memory, warp 0 finishes the cells.

@@ -3,10 +3,9 @@
 //
 // The reference's step (examples/shallow_water.py:270-403) alternates local stencils with halo
 // exchanges four times: fluxes -> exchange(fe, fn, q, ke) -> tendencies -> exchange(h', u', v')
-// -> friction-u -> exchange(fe2, fn2) -> friction-v.  At 8 GPUs a rank owns 2048 x 1024 cells
-// that live in L2; a step is ~20 us of arithmetic and every exchange costs one NVLink round
-// (~9 us), so the exchanges -- not the bandwidth -- bound the step.  Here the tendency phase's
-// result (h', u', v') is exchanged ONCE, three cells deep, and everything the other two exchanges
+// -> friction-u -> exchange(fe2, fn2) -> friction-v.  At 8 GPUs a rank owns 2048 x 1024 cells; with
+// so little arithmetic per step, the NVLink round trip of every exchange -- not the bandwidth --
+// bounds the step.  Here the tendency phase's result (h', u', v') is exchanged ONCE, three cells deep, and everything the other two exchanges
 // used to deliver is recomputed from it on a thin frame around the block:
 //
 //   frame kernel A   h', u', v' on the cells within 3 of the block edge (u', v' two cells further: the
@@ -181,8 +180,7 @@ __device__ __forceinline__ float ca_flux_plain(const CACtx& c, int j, int i, int
   }
 }
 // the rare path is a real call: inlined, its ~250 instructions per flux would sit in every one of the
-// fourteen slots and the kernel would spend its time fetching instructions (measured: 4096 SASS
-// instructions, "no instruction" the top stall)
+// fourteen slots and the kernel would spend its time fetching instructions
 static __device__ __noinline__ float ca_flux_generic(const CACtx& c, int j, int i, int kind) {
   switch (kind) {
     case 0: return ca_fe(c, j, i);

@@ -1,7 +1,7 @@
 """mpi4jax_b200 demo application -- Shallow water
 
 The reference's demo (/root/reference/examples/shallow_water.py), a non-linear shallow-water
-solver adapted from https://github.com/dionhaefner/shallow-water, on the B200-native stack.
+solver adapted from https://github.com/dionhaefner/shallow-water, on the H100-native stack.
 
 Usage examples:
 

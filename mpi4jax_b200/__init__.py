@@ -1,4 +1,4 @@
-"""mpi4jax_b200 -- Blackwell-native communication primitives with the API of mpi4jax.
+"""mpi4jax_b200 -- Hopper-native communication primitives with the API of mpi4jax.
 
 Public namespace (reference: /root/reference/mpi4jax/__init__.py:9-41): the 12 ops and the
 two capability probes, plus what replaces the pieces JAX/mpi4py provided there:

@@ -1,4 +1,4 @@
-"""CUDA backend: drives the native sm_100a core for tensors that live on the GPU.
+"""CUDA backend: drives the native sm_90a core for tensors that live on the GPU.
 
 This is the layer the reference implements in mpi_xla_bridge_cuda.cpp (882 lines of
 host C++ that synchronise the stream and hand pointers to MPI).  Here a communicator
@@ -240,9 +240,10 @@ class NativeComm:
         if len({h for h, _ in devs}) != 1:
             raise MPIError("the GPU transport needs all ranks of a communicator on one NVLink node")
         self.shared_gpu = len(set(devs)) != len(devs)   # several ranks on one GPU (testing only)
-        # p2p ring slot: 16 MiB stripes give 625 GB/s on a 256 MiB sendrecv, 4 MiB ones 380 GB/s (one
-        # header + credit round per 64 KiB lane stripe: profiles/r2_sweep_n8.log vs r2_p2p_n2.log).  The ring
-        # area is P x 8 slots per rank -- 1 GiB at 8 ranks, 0.6 % of a B200's HBM
+        if self.shared_gpu:
+            self.want_mc = False        # a multicast object binds every device once
+        # p2p ring slot: large stripes amortise the header + credit round per 64 KiB lane stripe.  The ring
+        # area is P x 8 slots per rank -- 1 GiB at 8 ranks, 1.25 % of an H100's 80 GB
         slot = env_int("MPI4JAX_B200_P2P_SLOT_BYTES", 16 << 20)
         ll_cap = env_int("MPI4JAX_B200_LL_BYTES", 128 << 10)
         halo_cap = env_int("MPI4JAX_B200_HALO_BYTES", 256 << 10)
@@ -253,7 +254,7 @@ class NativeComm:
                                          slot, ll_cap, halo_cap, timeout)
         if not self.handle:
             raise MPIError(f"native communicator creation failed: {native.last_error()}")
-        # transport thresholds for THIS world size on THIS GPU model (measured table, optionally overridden by
+        # transport thresholds for THIS world size on THIS GPU model (built-in table, optionally overridden by
         # a tuning file: _src/tuning.py); every rank must end up with the same numbers -- the transport
         # choice is made independently on each rank from sizes and thresholds only
         from .. import tuning
@@ -363,7 +364,8 @@ class NativeComm:
         _lib().b2_comm_set_tuning(self.handle, ll_max, oneshot_max, nvls_min, max_blocks)
 
     def set_option(self, key: str, value: int) -> None:
-        """Runtime switches of the native communicator: ``bcast_mc_min`` (bytes), ``nvls_pipeline`` (0/1)."""
+        """Runtime switches of the native communicator: ``bcast_mc_min`` (bytes), ``nvls_pipeline`` (0/1),
+        ``gemm_raster``, ``p2p_anysource_scan`` (0/1)."""
         self._check(_lib().b2_comm_set_option(self.handle, key.encode(), int(value)), "Comm_set_option")
 
     def get_option(self, key: str) -> int:
@@ -588,7 +590,7 @@ class NativeComm:
         self._bind_status(status, rec, out.element_size())
         return out
 
-    # -- tensor-parallel linear: tcgen05 GEMM + in-switch allreduce (csrc/b2_gemm.cu) ----------
+    # -- tensor-parallel linear: wgmma GEMM + in-switch allreduce (csrc/b2_gemm.cu) ------------
     def gemm_allreduce(self, x: torch.Tensor, weight: torch.Tensor) -> torch.Tensor:
         """``allreduce_SUM(x @ weight.T)`` for bf16 ``x (M, K)``, ``weight (N, K)`` in ONE kernel."""
         M, K = x.shape

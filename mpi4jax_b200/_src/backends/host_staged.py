@@ -9,7 +9,7 @@ fallback, never the default on one node:
   needs peer-mapped HBM, i.e. one NVLink domain), with a one-time warning;
 * forced by ``MPI4JAX_B200_TRANSPORT=host`` or the reference's ``MPI4JAX_USE_CUDA_MPI=0``.
 
-Same method surface as ``backends.cuda.NativeComm`` for the 12 ops; the fused / B200-only entry
+Same method surface as ``backends.cuda.NativeComm`` for the 12 ops; the fused / H100-only entry
 points (halo exchange, GEMM+allreduce) raise.  Ops synchronise the stream and block the host, so
 they cannot be captured into CUDA graphs: ``mpi4jax_b200.jit`` runs such functions eagerly.
 """
@@ -112,7 +112,7 @@ class HostStagedComm:
         out = _cpu.sendrecv(self.comm, self._down(sendbuf), host, source, dest, sendtag, recvtag, status)
         return self._up(out, recv_template)
 
-    # -- B200-only entry points ---------------------------------------------------------
+    # -- H100-only entry points ---------------------------------------------------------
     def gemm_allreduce(self, *a, **k):
         self._unsupported("the fused GEMM + allreduce kernel")
 

@@ -2,7 +2,7 @@
 
 The reference takes ``mpi4py`` objects (``MPI.Intracomm``, ``MPI.Op``, ``MPI.Status``)
 and forwards their C handles to its C++ bridge (/root/reference/mpi4jax/_src/utils.py:
-60-153).  Neither mpi4py nor an MPI library exists on the target image, and the B200
+60-153).  Neither mpi4py nor an MPI library exists on the target image, and the H100
 transport is not MPI at all, so this module supplies the small object model user code
 needs (``mpi4jax_b200.MPI``): ``COMM_WORLD``, ``Comm.Get_rank/Get_size/Clone/Split/
 Free/Barrier``, the ten predefined ``Op`` constants, ``Status`` with

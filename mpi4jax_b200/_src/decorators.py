@@ -60,7 +60,7 @@ def env_float(name: str, default: float) -> float:
 
 
 def ensure_cuda_ext(fn=None):
-    """Raise ImportError if the native sm_100a library is unavailable.
+    """Raise ImportError if the native sm_90a library is unavailable.
 
     Usable as a plain call or as a decorator (reference: decorators.py:10-17).
     """
@@ -87,11 +87,11 @@ def ensure_cuda_ext(fn=None):
 
 
 def ensure_xpu_ext(fn=None):
-    """The reference ships an Intel XPU bridge (decorators.py:20-27); B200 has none."""
+    """The reference ships an Intel XPU bridge (decorators.py:20-27); H100 has none."""
 
     def check():
         raise ImportError(
-            "mpi4jax_b200 targets NVIDIA B200 (sm_100a) only; there is no XPU/SYCL extension."
+            "mpi4jax_b200 targets NVIDIA H100 (sm_90a) only; there is no XPU/SYCL extension."
         )
 
     if fn is None:

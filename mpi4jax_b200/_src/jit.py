@@ -2,7 +2,7 @@
 
 The reference's ops are JAX primitives so that they run inside ``jax.jit``; XLA compiles
 the surrounding program and an ordered effect token keeps the custom calls in program
-order (/root/reference/mpi4jax/_src/utils.py:45-53, jax_compat.py:82-100).  The B200
+order (/root/reference/mpi4jax/_src/utils.py:45-53, jax_compat.py:82-100).  The H100
 design replaces the tracing compiler with **CUDA streams and graphs**: every op is a
 kernel on the current stream (stream order == program order, the token is implicit), and
 ``jit`` records the whole function -- stencils, collectives, halo exchanges -- into one

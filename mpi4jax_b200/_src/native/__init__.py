@@ -1,4 +1,4 @@
-"""Bridge registry: loads the native sm_100a library and exposes its C ABI.
+"""Bridge registry: loads the native sm_90a library and exposes its C ABI.
 
 Counterpart of /root/reference/mpi4jax/_src/xla_bridge/__init__.py:1-174, which
 imports the nanobind modules, checks the MPI ABI, fans ``set_logging`` out to every
@@ -37,7 +37,7 @@ from . import codes  # noqa: F401
 _LIB_PATH = Path(__file__).resolve().parents[2] / "_native" / "libb2mpi.so"
 
 HAS_CUDA_EXT = False
-HAS_XPU_EXT = False  # the reference has an Intel XPU bridge; B200 does not
+HAS_XPU_EXT = False  # the reference has an Intel XPU bridge; H100 does not
 CUDA_EXT_ERROR = ""
 lib = None
 
@@ -295,7 +295,7 @@ NATIVE_ABI_INFO = {
     "library": str(_LIB_PATH),
     "loaded": HAS_CUDA_EXT,
     "version": lib.b2_version().decode() if HAS_CUDA_EXT else None,
-    "arch": "sm_100a",
+    "arch": "sm_90a",
     "sizeof_status_record": ctypes.sizeof(B2StatusRecord),
     "sizeof_halo_desc": ctypes.sizeof(B2HaloDesc),
     "python": _abi_expected(),

@@ -1,11 +1,10 @@
-"""In-tree build of the native core (``libb2mpi.so``) for sm_100a.
+"""In-tree build of the native core (``libb2mpi.so``) for sm_90a (H100).
 
 ``python -m mpi4jax_b200._src.native.build`` (or ``__graft_entry__.build()``)
 compiles every translation unit under ``csrc/`` with
-``nvcc -gencode arch=compute_100a,code=sm_100a -lineinfo`` in parallel and links
-them into ``mpi4jax_b200/_native/libb2mpi.so``.  nvcc cross-compiles without a
-GPU, so this also runs on the GPU-less authoring box; the built library travels
-to the GPU box with the repo snapshot (it is git-ignored, not gpurun-ignored).
+``nvcc -gencode arch=compute_90a,code=sm_90a -lineinfo`` in parallel and links
+them into ``mpi4jax_b200/_native/libb2mpi.so`` (git-ignored).  nvcc cross-compiles
+without a GPU, so the library can be built on a machine that has none.
 
 Counterpart of the reference's ``setup.py`` extension build
 (/root/reference/setup.py:81-108, 375-431), which swaps the compiler for
@@ -28,7 +27,7 @@ OUT_DIR = REPO / "mpi4jax_b200" / "_native"
 OBJ_DIR = OUT_DIR / "obj"
 LIB = OUT_DIR / "libb2mpi.so"
 
-ARCH_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a"]
+ARCH_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a"]
 COMMON = ["-O3", "-std=c++17", "-lineinfo", "-Xcompiler", "-fPIC", "-Xcompiler", "-fvisibility=default"]
 # extra nvcc flags, e.g. MPI4JAX_B200_NVCC_FLAGS="-DB2_SWE_EXPLICIT_ROUNDING=1" (part of the cache key)
 COMMON += os.environ.get("MPI4JAX_B200_NVCC_FLAGS", "").split()

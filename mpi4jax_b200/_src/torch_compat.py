@@ -3,7 +3,7 @@
 The reference gates on the JAX version (/root/reference/mpi4jax/_src/jax_compat.py:
 12-48, pinned in _latest_jax_version.txt).  The host framework here is PyTorch
 (streams, CUDA graphs, autograd, ``torch.func``); this module gates on the torch
-version and probes the GPU capabilities the native core needs (sm_100, VMM fd
+version and probes the GPU capabilities the native core needs (sm_90, VMM fd
 handles, multicast).
 """
 
@@ -69,11 +69,11 @@ def device_capabilities(device: int = 0) -> dict:
     """Capabilities relevant to the native transport (all False without a GPU)."""
     import torch
 
-    caps = {"cuda": False, "sm": None, "sm_100": False, "vmm": False, "multicast": False}
+    caps = {"cuda": False, "sm": None, "sm_90": False, "vmm": False, "multicast": False}
     if not torch.cuda.is_available():
         return caps
     major, minor = torch.cuda.get_device_capability(device)
-    caps.update(cuda=True, sm=(major, minor), sm_100=(major == 10))
+    caps.update(cuda=True, sm=(major, minor), sm_90=((major, minor) == (9, 0)))
     try:
         from . import native
 

@@ -10,8 +10,9 @@ The native library picks a transport per call from a handful of byte thresholds
 
 Which transport wins where depends on the number of ranks (at 2 ranks a one-shot pull beats the
 switch at every size: each GPU has to serve P + 1 streams for an in-switch allreduce) and on the box.
-The table below is what was MEASURED on B200 / NVSwitch boxes (the files named next to each entry);
-``bench/autotune_collectives.py`` re-measures the crossovers for the job's world size on the box at hand
+The table below holds the library's defaults for H100 / NVSwitch boxes at every world size; the
+crossovers between its transports have not been measured on H100 yet.
+``bench/autotune_collectives.py`` measures the crossovers for the job's world size on the box at hand
 and writes a JSON file that ``MPI4JAX_B200_TUNING_FILE`` (or ``mpi4jax_b200/_src/tuning_tables/<gpu>.json``)
 makes every later communicator load.  The reference has no counterpart: it hands every call to MPI.
 """
@@ -28,20 +29,16 @@ KEYS = ("ll_max", "oneshot_max", "nvls_min", "bcast_mc_min")
 NATIVE_DEFAULTS = {"ll_max": 64 << 10, "oneshot_max": 512 << 10, "nvls_min": (64 << 10) + 1, "bcast_mc_min": 256 << 10}
 
 # world size -> thresholds (bytes).  A world size that is not listed uses the next smaller entry.
-MEASURED: Dict[str, Dict[int, Dict[str, int]]] = {
-    "NVIDIA B200": {
-        # profiles/r2_sweep_n2_callH.log, r2_allreduce_sym_n2.log: LL 4.2-5.3 us up to its 64 KiB buffer limit,
-        # one-shot pull beyond.  (At two ranks the native selection never takes the switch paths, whatever
-        # nvls_min / bcast_mc_min say: an in-switch allreduce is bounded at P / (P + 1) of a link and loses.)
+DEFAULTS_BY_GPU: Dict[str, Dict[int, Dict[str, int]]] = {
+    "NVIDIA H100 80GB HBM3": {
+        # (at two ranks the native selection never takes the switch paths, whatever nvls_min /
+        # bcast_mc_min say: an in-switch allreduce is bounded at P / (P + 1) of a link and loses)
         2: dict(NATIVE_DEFAULTS),
-        # profiles/r2_sweep_n4.log, r2_allreduce_phases_n4.log
         4: dict(NATIVE_DEFAULTS),
-        # profiles/r2_sweep_n8.log (LL 7.9-12.2 us up to 64 KiB, staged NVLS 19.7 us at 256 KiB and ahead of
-        # one-shot from there on), r1_collectives_sweep_8gpu_v1.json (one-shot vs two-shot without multicast)
         8: dict(NATIVE_DEFAULTS),
     },
 }
-DEFAULT_GPU = "NVIDIA B200"
+DEFAULT_GPU = "NVIDIA H100 80GB HBM3"
 _TABLE_DIR = os.path.join(os.path.dirname(os.path.abspath(__file__)), "tuning_tables")
 
 
@@ -72,9 +69,9 @@ def load_file(path: str) -> Dict[int, Dict[str, int]]:
 
 
 def thresholds(world: int, gpu_name: Optional[str] = None) -> Dict[str, int]:
-    """Thresholds for a communicator of ``world`` ranks on ``gpu_name``: the measured table, overridden
+    """Thresholds for a communicator of ``world`` ranks on ``gpu_name``: the built-in table, overridden
     entry by entry by ``tuning_tables/<gpu name>.json`` and then by ``$MPI4JAX_B200_TUNING_FILE``."""
-    base = _entry_for(MEASURED.get(gpu_name or DEFAULT_GPU, MEASURED[DEFAULT_GPU]), world)
+    base = _entry_for(DEFAULTS_BY_GPU.get(gpu_name or DEFAULT_GPU, DEFAULTS_BY_GPU[DEFAULT_GPU]), world)
     candidates = []
     if gpu_name:
         candidates.append(os.path.join(_TABLE_DIR, gpu_name.replace(" ", "_") + ".json"))

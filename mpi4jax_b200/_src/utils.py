@@ -116,7 +116,7 @@ def backend_of(t: torch.Tensor) -> str:
 
 
 def has_cuda_support() -> bool:
-    """True when the native sm_100a library is loaded (reference: utils.py:159-165)."""
+    """True when the native sm_90a library is loaded (reference: utils.py:159-165)."""
     from . import native
 
     return bool(native.HAS_CUDA_EXT)
@@ -124,7 +124,7 @@ def has_cuda_support() -> bool:
 
 def has_sycl_support() -> bool:
     """Always False: the reference's Intel XPU bridge (utils.py:168-174) is out of scope
-    for a B200-native framework."""
+    for an H100-native framework."""
     return False
 
 

@@ -37,7 +37,7 @@ def collect() -> dict:
         caps = torch_compat.device_capabilities(i)
         props = torch.cuda.get_device_properties(i)
         devices.append({"index": i, "name": props.name, "sm": list(caps["sm"] or ()),
-                        "sm_100": caps["sm_100"], "memory_gib": round(props.total_memory / 2**30, 1),
+                        "sm_90": caps["sm_90"], "memory_gib": round(props.total_memory / 2**30, 1),
                         "sms": props.multi_processor_count, "vmm": caps["vmm"], "multicast": caps["multicast"]})
     info["devices"] = devices
     return info
@@ -59,7 +59,7 @@ def main(argv=None) -> int:
     for d in info["devices"]:
         print(f"  cuda:{d['index']}  {d['name']}  sm_{''.join(map(str, d['sm']))}  {d['sms']} SMs  "
               f"{d['memory_gib']} GiB  vmm={d['vmm']}  multicast(NVLS)={d['multicast']}"
-              + ("" if d["sm_100"] else "   [not a Blackwell sm_100 device: the kernels will not load]"))
+              + ("" if d["sm_90"] else "   [not a Hopper sm_90 device: the kernels will not load]"))
     for k, v in info["env"].items():
         print(f"  {k}={v}")
     return 0

@@ -49,7 +49,7 @@ class ParallelMLP:
         if self.mode == "tp":
             h = torch.tanh(x @ w1_)                           # column-parallel
             if h.is_cuda and h.dtype == torch.bfloat16:
-                # row-parallel GEMM and its allreduce as ONE tcgen05 + multimem.red kernel
+                # row-parallel GEMM and its allreduce as ONE wgmma + multimem.red kernel
                 from ..ops.linear import linear_allreduce
 
                 return linear_allreduce(h, w2_.t(), comm=self.comm)

@@ -7,7 +7,7 @@ Adams-Bashforth time stepping, lateral friction, decomposition ``nproc_y = min(P
 balanced jet (:138-169).  Two execution paths integrate it:
 
 ``backend="native"`` (CUDA tensors)
-    Hand-written sm_100a kernels, enqueued by one native call per ``multistep`` and captured
+    Hand-written sm_90a kernels, enqueued by one native call per ``multistep`` and captured
     into a CUDA graph by :func:`mpi4jax_b200.jit`.  Default schedule: the communication-avoiding
     step (csrc/b2_swe_ca.cu) -- two fused bulk kernels (16 array passes instead of 32) running
     concurrently with a thin frame pipeline that needs ONE three-cell-deep halo exchange per

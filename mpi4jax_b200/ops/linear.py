@@ -3,9 +3,9 @@
 ``linear_allreduce(x, weight)`` = ``allreduce(x @ weight.T, SUM)`` where every rank holds a
 K-shard of both operands -- the tensor-parallel pattern of the reference's matvec tests
 (/root/reference/tests/collective_ops/test_allreduce_matvec.py:41-65).  On CUDA with bf16
-operands and tile-aligned shapes it runs as ONE hand-written sm_100a kernel (tcgen05 MMAs,
-TMA-fed, accumulators in TMEM, every finished tile all-reduced in the NVSwitch with
-``multimem.ld_reduce`` / ``multimem.st`` while the next tile is being multiplied, csrc/b2_gemm.cu);
+operands and tile-aligned shapes it runs as ONE hand-written sm_90a kernel (wgmma MMAs,
+TMA-fed, accumulators in registers, every finished tile all-reduced in the NVSwitch with
+``multimem.ld_reduce`` / ``multimem.st`` while the next tile's operands are loaded, csrc/b2_gemm.cu);
 otherwise it falls back to ``torch.matmul`` + ``allreduce``.
 Differentiable: the adjoint of the allreduce is the identity on the replicated cotangent, so
 ``grad_x = g @ weight`` and ``grad_weight = g.T @ x`` are plain local GEMMs.

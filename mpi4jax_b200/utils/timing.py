@@ -1,4 +1,4 @@
-"""Timing hygiene helpers (B200_PROFILING.md): CUDA events on the launching stream,
+"""Timing hygiene helpers: CUDA events on the launching stream,
 synchronise on both sides, max over ranks, L2 flush between iterations, clock sampling."""
 
 from __future__ import annotations
@@ -30,7 +30,7 @@ _l2_buf: Optional[torch.Tensor] = None
 
 
 def flush_l2(device=None, nbytes: int = 256 << 20) -> None:
-    """Write a buffer larger than the 126 MB L2."""
+    """Write a buffer several times larger than the L2 (50 MB on H100)."""
     global _l2_buf
     if _l2_buf is None or _l2_buf.numel() < nbytes:
         _l2_buf = torch.empty(nbytes, dtype=torch.uint8, device=device or "cuda")

@@ -1,4 +1,4 @@
-"""Fused tcgen05 GEMM+allreduce vs cuBLAS GEMM followed by an allreduce (ours / NCCL)."""
+"""Fused wgmma GEMM+allreduce vs cuBLAS GEMM followed by an allreduce (ours / NCCL)."""
 import os
 import sys
 
@@ -36,7 +36,7 @@ for (M, N, K) in [(4096, 4096, 4096 // size), (8192, 8192, 8192 // size), (8192,
     w = torch.randn(N, K, device=dev).bfloat16()
     flops = 2.0 * M * N * K
     rows = {}
-    rows["fused tcgen05+NVLS (one kernel)"] = timeit(lambda: linear_allreduce(x, w, comm=comm))
+    rows["fused wgmma+NVLS (one kernel)"] = timeit(lambda: linear_allreduce(x, w, comm=comm))
     rows["cublas + our allreduce"] = timeit(lambda: m.allreduce(x @ w.t(), MPI.SUM, comm=comm))
     if nccl is not None:
         def f():

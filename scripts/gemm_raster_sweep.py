@@ -1,4 +1,4 @@
-"""Tile order of the persistent tcgen05 GEMM (csrc/b2_gemm_raster.h): device time per shape for several
+"""Tile order of the persistent wgmma GEMM (csrc/b2_gemm_raster.h): device time per shape for several
 band heights G (communicator option "gemm_raster"; 0 = row-major), next to cuBLAS.  One GPU.
     python scripts/gemm_raster_sweep.py"""
 import os

@@ -1,4 +1,4 @@
-"""Regenerate profiles/sass/*.sass (+ opcode summary) from the built native library."""
+"""Write profiles/sass/*.sass (+ opcode summary) from the built native library (generated locally, not committed)."""
 import collections
 import os
 import re
@@ -19,9 +19,9 @@ WANT = {       # substring of the mangled name (with its length prefix where nam
     "b2_k_allreduce_nvlsILi3": "allreduce_nvls_bf16", "b2_k_allreduce_llIfLi0": "allreduce_ll_f32_sum",
     "b2_k_reduce_chunkedIfLi0": "reduce_chunked_f32_sum",
     "b2_k_reduce_chunkedI13__nv_bfloat16Li0": "reduce_chunked_bf16_sum",
-    "b2_k_gemm": "gemm_allreduce_tcgen05",
+    "b2_k_gemm": "gemm_allreduce_wgmma",
 }
-HEADER = """# SASS listings (cuobjdump -sass libb2mpi.so, sm_100a)
+HEADER = """# SASS listings (cuobjdump -sass libb2mpi.so, sm_90a)
 
 One file per kernel family (typed reduce kernels: the f32/bf16 SUM instances); instruction
 encodings stripped.  What to look for: peer/multicast traffic in the same kernel as the

@@ -1,4 +1,4 @@
-"""Turn .ncu-rep captures into the text summaries committed under profiles/."""
+"""Turn .ncu-rep captures into text summaries under profiles/ (generated locally, not committed)."""
 import csv
 import subprocess
 import sys

@@ -1,4 +1,4 @@
-"""setuptools entry point: builds the native sm_100a core as part of ``build_ext`` / ``pip install``.
+"""setuptools entry point: builds the native sm_90a core as part of ``build_ext`` / ``pip install``.
 
 The reference's ``setup.py`` swaps the C compiler for ``mpicc`` and builds up to three
 nanobind bridges depending on which toolkits it discovers (/root/reference/setup.py:81-108,

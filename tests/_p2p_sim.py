@@ -109,7 +109,7 @@ class Pair:
         return True
 
 
-    # ---- ANY_SOURCE support (B2_P2P_ANYSOURCE_SCAN) ----------------------------------------
+    # ---- ANY_SOURCE support (communicator option p2p_anysource_scan) -----------------------
     def scan(self, recv_tag):
         """Non-blocking variant of match() used by the ANY_SOURCE election: sequence number of the
         message a receive with this tag would take from this source right now, or None.  A streamed

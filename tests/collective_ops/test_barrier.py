@@ -16,10 +16,13 @@ def test_barrier(device):
     """Ranks append lines before/after a barrier to one file; all 'start' lines must precede
     all 'done' lines."""
     rank, size = comm.Get_rank(), comm.Get_size()
-    write_to = os.path.join(tempfile.gettempdir(), f"mpi4jax-b200-barrier-{device.type}.txt")
+    # a fresh file per run, named by rank 0: a fixed name in the shared temp directory could belong
+    # to another user or to a concurrent job
+    write_to = None
     if rank == 0:
-        with open(write_to, "w"):
-            pass
+        fd, write_to = tempfile.mkstemp(prefix=f"mpi4jax-b200-barrier-{device.type}-", suffix=".txt")
+        os.close(fd)
+    write_to = comm.bcast(write_to, root=0)
     comm.Barrier()
     time.sleep(rank * 0.2)
     with open(write_to, "a") as f:
@@ -34,6 +37,9 @@ def test_barrier(device):
     comm.Barrier()
     with open(write_to) as f:
         outputs = f.readlines()
+    comm.Barrier()
+    if rank == 0:
+        os.remove(write_to)
     assert len(outputs) == size * 2
     assert all(o.endswith("start\n") for o in outputs[:size])
     assert all(o.endswith("done\n") for o in outputs[size:])

@@ -7,11 +7,13 @@ import torch
 import mpi4jax_b200 as m
 from mpi4jax_b200 import MPI
 
+from .._peer_job import needs_peers
+
 comm = MPI.COMM_WORLD
 rank = comm.Get_rank()
 size = comm.Get_size()
 
-need2 = pytest.mark.skipif(size < 2, reason="need at least 2 processes to test send/recv")
+need2 = needs_peers("need at least 2 processes to test send/recv")
 
 
 @need2
@@ -56,7 +58,7 @@ def test_send_recv_jit(device):
             send_jit(arr)
 
 
-@pytest.mark.skipif(size < 2 or rank > 1, reason="Runs only on rank 0 and 1")
+@needs_peers("Runs only on rank 0 and 1", max_rank=1)
 def test_send_recv_deadlock(device):
     """Ops must execute in program order (reference: hangs if XLA reorders the custom calls)."""
 
@@ -222,20 +224,29 @@ def test_tags_matched_out_of_order_between_ranks(device):
 
 def test_any_source_with_tag_matches_behind_the_head(device):
     """recv(ANY_SOURCE, tag=T) where T is not the oldest pending message of its source.  The CPU
-    backend always matches it; the GPU election does so when built with -DB2_P2P_ANYSOURCE_SCAN=1
-    (default build: only the oldest pending message of every source is considered)."""
-    import os
+    backend always matches it; the GPU election does so with the communicator option
+    p2p_anysource_scan (default: only the oldest pending message of every source is considered)."""
+    if device.type == "cuda":
+        nc = comm._native_comm()         # the option belongs to this communicator: every op below uses it
+        nc.set_option("p2p_anysource_scan", 1)
+        try:
+            _any_source_behind_the_head(device)
+        finally:
+            m.flush()
+            nc.set_option("p2p_anysource_scan", 0)
+    else:
+        _any_source_behind_the_head(device)
 
-    if device.type == "cuda" and not os.environ.get("MPI4JAX_B200_TEST_ANYSOURCE_SCAN"):
-        pytest.skip("needs a build with -DB2_P2P_ANYSOURCE_SCAN=1 (set MPI4JAX_B200_TEST_ANYSOURCE_SCAN=1)")
+
+def _any_source_behind_the_head(device):
     a = torch.full((6,), 1.0, device=device)
     b = torch.full((6,), 2.0, device=device)
-    m.send(a, rank, tag=1)
-    m.send(b, rank, tag=2)
+    m.send(a, rank, tag=1, comm=comm)
+    m.send(b, rank, tag=2, comm=comm)
     status = MPI.Status()
-    got = m.recv(torch.empty_like(a), source=MPI.ANY_SOURCE, tag=2, status=status)
+    got = m.recv(torch.empty_like(a), source=MPI.ANY_SOURCE, tag=2, status=status, comm=comm)
     assert torch.equal(got, b) and status.Get_source() == rank and status.Get_tag() == 2
-    got = m.recv(torch.empty_like(a), source=MPI.ANY_SOURCE, tag=1, status=status)
+    got = m.recv(torch.empty_like(a), source=MPI.ANY_SOURCE, tag=1, status=status, comm=comm)
     assert torch.equal(got, a) and status.Get_tag() == 1
 
 

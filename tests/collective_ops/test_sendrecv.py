@@ -9,11 +9,13 @@ from torch.func import grad, jacfwd, jacrev, vmap
 import mpi4jax_b200 as m
 from mpi4jax_b200 import MPI
 
+from .._peer_job import needs_peers
+
 comm = MPI.COMM_WORLD
 rank = comm.Get_rank()
 size = comm.Get_size()
 
-pair = pytest.mark.skipif(size < 2 or rank > 1, reason="Runs only on rank 0 and 1")
+pair = needs_peers("Runs only on rank 0 and 1", max_rank=1)
 other = 1 - rank
 
 

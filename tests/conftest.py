@@ -6,7 +6,7 @@ Test strategy (mirrors the reference, SURVEY.md section 4): the same test files 
  * once per rank under ``python -m mpi4jax_b200.run -n 2 -m pytest ...`` (tests/test_multirank.py
    spawns that job, as the reference's CI runs ``mpirun -np 2 pytest .``).
 Every test that takes the ``device`` fixture runs on CPU (gloo backend) and, marked ``gpu``,
-on CUDA (native sm_100a kernels).  ``pytest -m "not gpu"`` needs no GPU.
+on CUDA (native sm_90a kernels).  ``pytest -m "not gpu"`` needs no GPU.
 """
 
 import os
@@ -18,7 +18,7 @@ sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on a B200 box)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (an H100)")
 
 
 def pytest_report_header(config):

@@ -1,4 +1,4 @@
-"""Tensor-parallel linear: tcgen05 GEMM + in-switch allreduce in one kernel (csrc/b2_gemm.cu)
+"""Tensor-parallel linear: wgmma GEMM + in-switch allreduce in one kernel (csrc/b2_gemm.cu)
 against a plain fp32 PyTorch reference of the same op."""
 
 import pytest
@@ -25,7 +25,10 @@ def _reference(x, w):
 
 
 @pytest.mark.gpu
-@pytest.mark.parametrize("shape", [(128, 128, 64), (256, 384, 512), (1024, 512, 2048), (128, 256, 4096)])
+# (2048, 2048, 256): 256 tiles, more than one per CTA on any GPU -- the operand ring and the fused
+# epilogue's batches then carry across tile boundaries
+@pytest.mark.parametrize("shape", [(128, 128, 64), (256, 384, 512), (1024, 512, 2048), (128, 256, 4096),
+                                   (2048, 2048, 256)])
 def test_linear_allreduce_matches_fp32_reference(shape):
     if not torch.cuda.is_available():
         pytest.skip("no CUDA device")

@@ -47,7 +47,7 @@ def test_tile_order_is_a_bijection(tmp_path, group, grid):
         for start in range(0, len(order) - group, group):
             rows = {m // group for m, _ in order[start:start + group]}
             assert len(rows) <= 2
-        # the 148 tiles in flight (one per SM) stay within the bands they started in
-        if num_m * num_n >= 148 and num_m >= group:
-            bands = -(-148 // (group * num_n)) + 1
-            assert len({m for m, _ in order[:148]}) <= group * bands
+        # the 132 tiles in flight (one per H100 SM) stay within the bands they started in
+        if num_m * num_n >= 132 and num_m >= group:
+            bands = -(-132 // (group * num_n)) + 1
+            assert len({m for m, _ in order[:132]}) <= group * bands

@@ -2,7 +2,7 @@ def test_has_cuda_support():
     from mpi4jax_b200 import has_cuda_support
 
     assert isinstance(has_cuda_support(), bool)
-    assert has_cuda_support(), "the native sm_100a library must be built (python __graft_entry__.py)"
+    assert has_cuda_support(), "the native sm_90a library must be built (python __graft_entry__.py)"
 
 
 def test_has_sycl_support():
@@ -17,7 +17,7 @@ def test_native_abi_info():
 
     for key in ("library", "loaded", "version", "arch", "sizeof_status_record", "sizeof_halo_desc"):
         assert key in NATIVE_ABI_INFO
-    assert NATIVE_ABI_INFO["arch"] == "sm_100a"
+    assert NATIVE_ABI_INFO["arch"] == "sm_90a"
     assert NATIVE_ABI_INFO["sizeof_status_record"] == 24
     assert NATIVE_ABI_INFO["loaded"]
     native, python = NATIVE_ABI_INFO["native"], NATIVE_ABI_INFO["python"]

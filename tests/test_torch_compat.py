@@ -43,4 +43,4 @@ def test_device_capabilities_keys():
     from mpi4jax_b200._src.torch_compat import device_capabilities
 
     caps = device_capabilities()
-    assert set(caps) == {"cuda", "sm", "sm_100", "vmm", "multicast"}
+    assert set(caps) == {"cuda", "sm", "sm_90", "vmm", "multicast"}

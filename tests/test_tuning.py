@@ -7,30 +7,32 @@ import pytest
 
 from mpi4jax_b200._src import tuning
 
+H100 = "NVIDIA H100 80GB HBM3"
 
-def test_measured_table_covers_the_world_sizes_it_was_measured_at():
+
+def test_default_table_covers_every_world_size():
     for world in (2, 3, 4, 6, 8, 16):
-        t = tuning.thresholds(world, "NVIDIA B200")
+        t = tuning.thresholds(world, H100)
         assert set(t) == set(tuning.KEYS)
         assert t["ll_max"] <= 64 << 10            # the LL buffers hold 2 x 64 KiB per peer
     # the table compiled into the module is what the native library starts with: a communicator created
     # without a tuning file makes no extra native call
-    assert tuning.thresholds(8, "NVIDIA B200") == tuning.NATIVE_DEFAULTS
-    # world sizes in between use the next smaller measured entry
-    assert tuning.thresholds(6, "NVIDIA B200") == tuning.thresholds(4, "NVIDIA B200")
-    # an unknown GPU model falls back to the B200 numbers
-    assert tuning.thresholds(8, "Some Other GPU") == tuning.thresholds(8, "NVIDIA B200")
+    assert tuning.thresholds(8, H100) == tuning.NATIVE_DEFAULTS
+    # world sizes in between use the next smaller entry of the table
+    assert tuning.thresholds(6, H100) == tuning.thresholds(4, H100)
+    # an unknown GPU model falls back to the H100 numbers
+    assert tuning.thresholds(8, "Some Other GPU") == tuning.thresholds(8, H100)
 
 
 def test_tuning_file_overrides_entry_by_entry(tmp_path, monkeypatch):
     path = tmp_path / "box.json"
-    path.write_text(json.dumps({"gpu": "NVIDIA B200", "table": {"4": {"nvls_min": 1 << 20}, "8": {"ll_max": 32 << 10}}}))
+    path.write_text(json.dumps({"gpu": H100, "table": {"4": {"nvls_min": 1 << 20}, "8": {"ll_max": 32 << 10}}}))
     monkeypatch.setenv("MPI4JAX_B200_TUNING_FILE", str(path))
-    base4 = dict(tuning._entry_for(tuning.MEASURED["NVIDIA B200"], 4))
-    got4 = tuning.thresholds(4, "NVIDIA B200")
+    base4 = dict(tuning._entry_for(tuning.DEFAULTS_BY_GPU[H100], 4))
+    got4 = tuning.thresholds(4, H100)
     assert got4["nvls_min"] == 1 << 20 and got4["ll_max"] == base4["ll_max"]
-    assert tuning.thresholds(8, "NVIDIA B200")["ll_max"] == 32 << 10
-    assert tuning.thresholds(2, "NVIDIA B200")["nvls_min"] == 1 << 20     # 2 < 4: the file's smallest entry applies
+    assert tuning.thresholds(8, H100)["ll_max"] == 32 << 10
+    assert tuning.thresholds(2, H100)["nvls_min"] == 1 << 20     # 2 < 4: the file's smallest entry applies
     monkeypatch.setenv("MPI4JAX_B200_TUNING_FILE", str(tmp_path / "missing.json"))
     with pytest.raises(FileNotFoundError):
         tuning.thresholds(8)
