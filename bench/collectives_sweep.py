@@ -57,7 +57,7 @@ except Exception as exc:  # pragma: no cover
 nc = comm._native_comm()
 has_nvls = nc.has_nvls
 if ns.max_blocks:
-    nc.set_tuning(max_blocks=ns.max_blocks)
+    nc.set_option("max_blocks", ns.max_blocks)
 if ns.nvls_pipeline >= 0:
     nc.set_option("nvls_pipeline", ns.nvls_pipeline)
 

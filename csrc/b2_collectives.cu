@@ -15,7 +15,6 @@
 // in-place allreduce of symmetric tensors (b2_k_allreduce_sym), the multicast bcast
 // (b2_k_bcast_mc), the reduce-to-root (b2_k_reduce_root_nvls) --, the size-based algorithm
 // selection and the grid cap that keeps every launch co-resident (coresident_blocks).
-#include <cstdio>
 #include <cstring>
 
 #include "b2_reduce.cuh"
@@ -23,17 +22,6 @@
 
 b2_reduce_launch_fn b2_reduce_table[B2_DTYPE_COUNT][B2_OP_COUNT];
 b2_ll_launch_fn b2_ll_table[B2_DTYPE_COUNT][B2_OP_COUNT];
-void b2_register_reduce_group_0();
-void b2_register_reduce_group_1();
-void b2_register_reduce_group_2();
-void b2_register_reduce_group_3();
-
-extern "C" void b2_set_error(const char* fmt, ...);
-extern "C" void b2_count_launch(B2Comm* c);
-struct B2DebugScope;
-extern "C" B2DebugScope* b2_debug_begin(B2Comm* c, const char* opname, const char* details,
-                                         cudaStream_t stream);
-extern "C" void b2_debug_end(B2DebugScope* s, int code);
 
 static void b2_ensure_tables() {
   static bool done = false;
@@ -557,8 +545,6 @@ b2_k_reduce_root_nvls(const B2DevComm c, const B2ReduceArgs a) {
 // ---------------------------------------------------------------------------
 // host helpers
 // ---------------------------------------------------------------------------
-static size_t round_up(size_t x, size_t m) { return (x + m - 1) / m * m; }
-
 // How many CTAs of `kernel` (B2_THREADS threads, no dynamic shared memory) are resident at the same
 // time on this GPU: occupancy x SM count, bounded by the communicator's max_blocks.  A launch of at
 // most that many CTAs has every CTA resident at once whatever order the hardware dispatches them in,
@@ -629,19 +615,30 @@ static int check_stage(B2Comm* c, int opcode, size_t blk_bytes, const char* name
   return 0;
 }
 
-static int finish_launch(B2Comm* c, cudaError_t err, const char* name) {
-  b2_count_launch(c);
-  if (err != cudaSuccess) {
-    b2_set_error("%s: kernel launch failed: %s", name, cudaGetErrorString(err));
-    return 1000 + (int)err;
-  }
-  return 0;
+// The in-switch reductions: multicast-bound staging, SUM, f32 / bf16 / f16.
+static bool nvls_capable(const B2Comm* c, int dtype, int op) {
+  return c->dev.stage_mc != nullptr && op == B2_SUM && (dtype == B2_F32 || dtype == B2_BF16 || dtype == B2_F16);
+}
+
+// Typed instances of the in-switch kernel families (dtype: f32, bf16 or f16, checked by the caller).
+typedef void (*b2_nvls_kernel)(const B2DevComm, const B2ReduceArgs);
+static b2_nvls_kernel nvls_kernel(int opcode, int dtype) {
+  if (opcode == B2_OPC_REDUCE)
+    return dtype == B2_F32 ? b2_k_reduce_root_nvls<B2_F32>
+           : dtype == B2_BF16 ? b2_k_reduce_root_nvls<B2_BF16> : b2_k_reduce_root_nvls<B2_F16>;
+  return dtype == B2_F32 ? b2_k_allreduce_nvls<B2_F32>
+         : dtype == B2_BF16 ? b2_k_allreduce_nvls<B2_BF16> : b2_k_allreduce_nvls<B2_F16>;
+}
+typedef void (*b2_sym_kernel)(const B2DevComm, const B2SymArgs);
+static b2_sym_kernel sym_kernel(int dtype) {
+  return dtype == B2_F32 ? b2_k_allreduce_sym<B2_F32>
+         : dtype == B2_BF16 ? b2_k_allreduce_sym<B2_BF16> : b2_k_allreduce_sym<B2_F16>;
 }
 
 extern "C" int b2_barrier(B2Comm* c, cudaStream_t stream) {
-  B2DebugScope* dbg = b2_debug_begin(c, "Barrier", "", stream);
+  B2DebugScope* dbg = b2_debug_begin(c, "Barrier", stream, nullptr);
   b2_k_barrier<<<1, 32, 0, stream>>>(c->dev);
-  int rc = finish_launch(c, cudaGetLastError(), "barrier");
+  int rc = b2_launched(c, "barrier");
   b2_debug_end(dbg, rc);
   return rc;
 }
@@ -662,8 +659,7 @@ static int reduce_common(B2Comm* c, const void* in, void* out, size_t count, int
     if (opcode != B2_OPC_ALLREDUCE) algo = B2_ALGO_ONESHOT;
     else if (P > 1 && nbytes <= c->ll_max && nbytes * 2 <= c->dev.lay.ll_cap) algo = B2_ALGO_LL;
     else if (P <= 2) algo = B2_ALGO_ONESHOT;
-    else if (c->dev.stage_mc != nullptr && op == B2_SUM && nbytes >= c->nvls_min &&
-             (dtype == B2_F32 || dtype == B2_BF16 || dtype == B2_F16)) algo = B2_ALGO_NVLS;
+    else if (nvls_capable(c, dtype, op) && nbytes >= c->nvls_min) algo = B2_ALGO_NVLS;
     else if (nbytes <= c->oneshot_max) algo = B2_ALGO_ONESHOT;
     else algo = B2_ALGO_TWOSHOT;
   }
@@ -679,7 +675,8 @@ static int reduce_common(B2Comm* c, const void* in, void* out, size_t count, int
     int grid = (int)((nv + B2_THREADS - 1) / B2_THREADS);
     if (grid > c->sm_count) grid = c->sm_count;
     if (grid < 1) grid = 1;
-    return finish_launch(c, b2_ll_table[dtype][op](c->dev, a, grid, stream), name);
+    b2_ll_table[dtype][op](c->dev, a, grid, stream);
+    return b2_launched(c, name);
   }
   int rc = check_stage(c, opcode, nbytes, name);
   if (rc) return rc;
@@ -689,44 +686,27 @@ static int reduce_common(B2Comm* c, const void* in, void* out, size_t count, int
   a.pipeline = c->nvls_pipeline;
   a.trace = c->trace; a.trace_cap = c->trace_cap;
   int grid;
-  const void* kern = nullptr;
   if (algo == B2_ALGO_NVLS) {
-    if (opcode == B2_OPC_REDUCE)
-      kern = dtype == B2_F32 ? (const void*)b2_k_reduce_root_nvls<B2_F32>
-             : dtype == B2_BF16 ? (const void*)b2_k_reduce_root_nvls<B2_BF16> : (const void*)b2_k_reduce_root_nvls<B2_F16>;
-    else
-      kern = dtype == B2_F32 ? (const void*)b2_k_allreduce_nvls<B2_F32>
-             : dtype == B2_BF16 ? (const void*)b2_k_allreduce_nvls<B2_BF16> : (const void*)b2_k_allreduce_nvls<B2_F16>;
-  }
-  pick_chunks(c, nbytes, coresident_blocks(c, kern), &a.chunk, &grid);     // (typed kernels: one CTA per SM)
-  if (algo == B2_ALGO_NVLS) {
-    if (c->dev.stage_mc == nullptr || op != B2_SUM ||
-        !(dtype == B2_F32 || dtype == B2_BF16 || dtype == B2_F16)) {
+    if (!nvls_capable(c, dtype, op)) {
       b2_set_error("%s: NVLS path needs a multicast-bound staging segment and SUM on f32/bf16/f16",
                    name);
       return B2_ERR_BAD_ARG;
     }
+    const b2_nvls_kernel kern = nvls_kernel(opcode, dtype);
+    pick_chunks(c, nbytes, coresident_blocks(c, (const void*)kern), &a.chunk, &grid);
     a.algo = B2_ALGO_NVLS;
-    if (opcode == B2_OPC_REDUCE) {
-      if (dtype == B2_F32) b2_k_reduce_root_nvls<B2_F32><<<grid, B2_THREADS, 0, stream>>>(c->dev, a);
-      else if (dtype == B2_BF16) b2_k_reduce_root_nvls<B2_BF16><<<grid, B2_THREADS, 0, stream>>>(c->dev, a);
-      else b2_k_reduce_root_nvls<B2_F16><<<grid, B2_THREADS, 0, stream>>>(c->dev, a);
-      return finish_launch(c, cudaGetLastError(), name);
-    }
-    if (dtype == B2_F32) b2_k_allreduce_nvls<B2_F32><<<grid, B2_THREADS, 0, stream>>>(c->dev, a);
-    else if (dtype == B2_BF16) b2_k_allreduce_nvls<B2_BF16><<<grid, B2_THREADS, 0, stream>>>(c->dev, a);
-    else b2_k_allreduce_nvls<B2_F16><<<grid, B2_THREADS, 0, stream>>>(c->dev, a);
-    return finish_launch(c, cudaGetLastError(), name);
+    kern<<<grid, B2_THREADS, 0, stream>>>(c->dev, a);
+    return b2_launched(c, name);
   }
+  pick_chunks(c, nbytes, coresident_blocks(c, nullptr), &a.chunk, &grid);     // (typed kernels: one CTA per SM)
   a.algo = (algo == B2_ALGO_TWOSHOT) ? B2_ALGO_TWOSHOT : B2_ALGO_ONESHOT;
-  return finish_launch(c, b2_reduce_table[dtype][op](c->dev, a, grid, stream), name);
+  b2_reduce_table[dtype][op](c->dev, a, grid, stream);
+  return b2_launched(c, name);
 }
 
 extern "C" int b2_allreduce(B2Comm* c, const void* in, void* out, size_t count, int dtype, int op,
                             int algo, cudaStream_t stream) {
-  char det[96];
-  snprintf(det, sizeof det, "with %zu items", count);
-  B2DebugScope* dbg = b2_debug_begin(c, "Allreduce", det, stream);
+  B2DebugScope* dbg = b2_debug_begin(c, "Allreduce", stream, "with %zu items", count);
   int rc = reduce_common(c, in, out, count, dtype, op, algo, 0, c->dev.size, 1, B2_OPC_ALLREDUCE,
                          "allreduce", stream);
   b2_debug_end(dbg, rc);
@@ -736,9 +716,7 @@ extern "C" int b2_allreduce(B2Comm* c, const void* in, void* out, size_t count, 
 // In-place allreduce (SUM; f32 / bf16 / f16) of a buffer inside a multicast-bound symmetric segment;
 // `mc` is the buffer's multicast address (segment multicast base + the buffer's offset).
 extern "C" int b2_allreduce_sym(B2Comm* c, void* mc, size_t count, int dtype, cudaStream_t stream) {
-  char det[96];
-  snprintf(det, sizeof det, "with %zu items (symmetric, in place)", count);
-  B2DebugScope* dbg = b2_debug_begin(c, "Allreduce", det, stream);
+  B2DebugScope* dbg = b2_debug_begin(c, "Allreduce", stream, "with %zu items (symmetric, in place)", count);
   int rc = 0;
   const size_t nbytes = count * b2_dtype_size(dtype);
   if (!(dtype == B2_F32 || dtype == B2_BF16 || dtype == B2_F16)) {
@@ -750,17 +728,14 @@ extern "C" int b2_allreduce_sym(B2Comm* c, void* mc, size_t count, int dtype, cu
   } else if (nbytes > 0) {
     B2SymArgs a;
     a.mc = (char*)mc; a.nbytes = nbytes; a.opcode = B2_OPC_ALLREDUCE;
-    const void* kern = dtype == B2_F32 ? (const void*)b2_k_allreduce_sym<B2_F32>
-                       : dtype == B2_BF16 ? (const void*)b2_k_allreduce_sym<B2_BF16> : (const void*)b2_k_allreduce_sym<B2_F16>;
+    const b2_sym_kernel kern = sym_kernel(dtype);
     // one tile of 4 x 512 vectors (32 KiB) per CTA and round at least; never more CTAs than co-resident
     const size_t slice = (nbytes / 16 + c->dev.size - 1) / c->dev.size;
     size_t want = (slice + 4 * B2_THREADS - 1) / (4 * B2_THREADS);
-    int grid = coresident_blocks(c, kern);
+    int grid = coresident_blocks(c, (const void*)kern);
     if (want < (size_t)grid) grid = (int)(want < 1 ? 1 : want);
-    if (dtype == B2_F32) b2_k_allreduce_sym<B2_F32><<<grid, B2_THREADS, 0, stream>>>(c->dev, a);
-    else if (dtype == B2_BF16) b2_k_allreduce_sym<B2_BF16><<<grid, B2_THREADS, 0, stream>>>(c->dev, a);
-    else b2_k_allreduce_sym<B2_F16><<<grid, B2_THREADS, 0, stream>>>(c->dev, a);
-    rc = finish_launch(c, cudaGetLastError(), "allreduce_");
+    kern<<<grid, B2_THREADS, 0, stream>>>(c->dev, a);
+    rc = b2_launched(c, "allreduce_");
   }
   b2_debug_end(dbg, rc);
   return rc;
@@ -768,17 +743,14 @@ extern "C" int b2_allreduce_sym(B2Comm* c, void* mc, size_t count, int dtype, cu
 
 extern "C" int b2_reduce(B2Comm* c, const void* in, void* out, size_t count, int dtype, int op,
                          int root, cudaStream_t stream) {
-  char det[96];
-  snprintf(det, sizeof det, "with %zu items to root %d", count, root);
-  B2DebugScope* dbg = b2_debug_begin(c, "Reduce", det, stream);
+  B2DebugScope* dbg = b2_debug_begin(c, "Reduce", stream, "with %zu items to root %d", count, root);
   int rc;
   if (root < 0 || root >= c->dev.size) {
     b2_set_error("reduce: invalid root %d", root);
     rc = B2_ERR_BAD_ARG;
   } else {
     const size_t nbytes = count * b2_dtype_size(dtype);
-    const bool nvls = c->dev.stage_mc != nullptr && op == B2_SUM && c->dev.size > 2 &&
-                      (dtype == B2_F32 || dtype == B2_BF16 || dtype == B2_F16) && nbytes >= c->nvls_min;
+    const bool nvls = c->dev.size > 2 && nvls_capable(c, dtype, op) && nbytes >= c->nvls_min;
     rc = reduce_common(c, in, out, count, dtype, op, nvls ? B2_ALGO_NVLS : B2_ALGO_ONESHOT, 0, c->dev.size,
                        c->dev.rank == root, B2_OPC_REDUCE, "reduce", stream);
   }
@@ -788,9 +760,7 @@ extern "C" int b2_reduce(B2Comm* c, const void* in, void* out, size_t count, int
 
 extern "C" int b2_scan(B2Comm* c, const void* in, void* out, size_t count, int dtype, int op,
                        cudaStream_t stream) {
-  char det[96];
-  snprintf(det, sizeof det, "with %zu items", count);
-  B2DebugScope* dbg = b2_debug_begin(c, "Scan", det, stream);
+  B2DebugScope* dbg = b2_debug_begin(c, "Scan", stream, "with %zu items", count);
   // small: rank r pulls the copies of ranks 0..r (one phase); large: rank s computes ALL prefixes of
   // sub-slice s and pushes prefix q to rank q (two phases, S bytes in and out per rank instead of
   // up to P * S into the last rank)
@@ -830,14 +800,12 @@ static int move_common(B2Comm* c, B2MoveArgs& a, const char* name, cudaStream_t 
   int grid;
   pick_chunks(c, a.blk_bytes, coresident_blocks(c, (const void*)b2_k_move), &a.chunk, &grid);
   b2_k_move<<<grid, B2_THREADS, 0, stream>>>(c->dev, a);
-  return finish_launch(c, cudaGetLastError(), name);
+  return b2_launched(c, name);
 }
 
 extern "C" int b2_allgather(B2Comm* c, const void* in, void* out, size_t blk_bytes, const B2Strided* lay,
                             cudaStream_t stream) {
-  char det[96];
-  snprintf(det, sizeof det, "sending %zu bytes", blk_bytes);
-  B2DebugScope* dbg = b2_debug_begin(c, "Allgather", det, stream);
+  B2DebugScope* dbg = b2_debug_begin(c, "Allgather", stream, "sending %zu bytes", blk_bytes);
   B2MoveArgs a;
   memset(&a, 0, sizeof a);
   a.in = in; a.out = out; a.blk_bytes = blk_bytes; a.opcode = B2_OPC_ALLGATHER;
@@ -852,9 +820,7 @@ extern "C" int b2_allgather(B2Comm* c, const void* in, void* out, size_t blk_byt
 
 extern "C" int b2_alltoall(B2Comm* c, const void* in, void* out, size_t blk_bytes, const B2Strided* lay,
                            cudaStream_t stream) {
-  char det[96];
-  snprintf(det, sizeof det, "sending %zu bytes per peer", blk_bytes);
-  B2DebugScope* dbg = b2_debug_begin(c, "Alltoall", det, stream);
+  B2DebugScope* dbg = b2_debug_begin(c, "Alltoall", stream, "sending %zu bytes per peer", blk_bytes);
   B2MoveArgs a;
   memset(&a, 0, sizeof a);
   a.in = in; a.out = out; a.blk_bytes = blk_bytes; a.opcode = B2_OPC_ALLTOALL;
@@ -871,9 +837,7 @@ extern "C" int b2_alltoall(B2Comm* c, const void* in, void* out, size_t blk_byte
 
 extern "C" int b2_bcast(B2Comm* c, const void* in, void* out, size_t nbytes, int root, const B2Strided* lay,
                         cudaStream_t stream) {
-  char det[96];
-  snprintf(det, sizeof det, "%zu bytes from root %d", nbytes, root);
-  B2DebugScope* dbg = b2_debug_begin(c, "Bcast", det, stream);
+  B2DebugScope* dbg = b2_debug_begin(c, "Bcast", stream, "%zu bytes from root %d", nbytes, root);
   int rc;
   if (root < 0 || root >= c->dev.size) {
     b2_set_error("bcast: invalid root %d", root);
@@ -898,7 +862,7 @@ extern "C" int b2_bcast(B2Comm* c, const void* in, void* out, size_t nbytes, int
           int grid;
           pick_chunks(c, a.blk_bytes, coresident_blocks(c, (const void*)b2_k_bcast_mc), &a.chunk, &grid);
           b2_k_bcast_mc<<<grid, B2_THREADS, 0, stream>>>(c->dev, a, root);
-          rc = finish_launch(c, cudaGetLastError(), "bcast");
+          rc = b2_launched(c, "bcast");
         }
       }
     } else if (rc == 0) {
@@ -911,9 +875,7 @@ extern "C" int b2_bcast(B2Comm* c, const void* in, void* out, size_t nbytes, int
 
 extern "C" int b2_gather(B2Comm* c, const void* in, void* out, size_t blk_bytes, int root, const B2Strided* lay,
                          cudaStream_t stream) {
-  char det[96];
-  snprintf(det, sizeof det, "sending %zu bytes to root %d", blk_bytes, root);
-  B2DebugScope* dbg = b2_debug_begin(c, "Gather", det, stream);
+  B2DebugScope* dbg = b2_debug_begin(c, "Gather", stream, "sending %zu bytes to root %d", blk_bytes, root);
   int rc;
   if (root < 0 || root >= c->dev.size) {
     b2_set_error("gather: invalid root %d", root);
@@ -936,9 +898,7 @@ extern "C" int b2_gather(B2Comm* c, const void* in, void* out, size_t blk_bytes,
 
 extern "C" int b2_scatter(B2Comm* c, const void* in, void* out, size_t blk_bytes, int root, const B2Strided* lay,
                           cudaStream_t stream) {
-  char det[96];
-  snprintf(det, sizeof det, "%zu bytes per rank from root %d", blk_bytes, root);
-  B2DebugScope* dbg = b2_debug_begin(c, "Scatter", det, stream);
+  B2DebugScope* dbg = b2_debug_begin(c, "Scatter", stream, "%zu bytes per rank from root %d", blk_bytes, root);
   int rc;
   if (root < 0 || root >= c->dev.size) {
     b2_set_error("scatter: invalid root %d", root);

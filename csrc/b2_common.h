@@ -16,7 +16,7 @@
 #include <cstddef>
 #include <cstdint>
 
-#define B2_ABI_VERSION 10   // bump whenever a struct shared with Python or a C signature changes
+#define B2_ABI_VERSION 11   // bump whenever a struct shared with Python or a C signature changes
 #define B2_MAX_RANKS 16          // ranks per NVLink domain we support (8 on HGX H100)
 #define B2_MAX_BLOCKS 1024       // max CTAs per collective launch (flag rows)
 #define B2_P2P_NSLOT 8           // ring slots per directed pair
@@ -97,18 +97,18 @@ static inline size_t b2_dtype_size(int dt) {
   }
 }
 
+static inline size_t round_up(size_t x, size_t m) { return (x + m - 1) / m * m; }
+
 // ---------------------------------------------------------------------------
 // Symmetric-heap layout (identical offsets on every rank).
 //
 //   [flags]      B2_MAX_BLOCKS x B2_MAX_RANKS u32   block-paired barrier flags
 //   [p2p hdr]    P x NSLOT x LANES x 16 B           inbox headers (written by the sender)
-//   [p2p ack]    P x NSLOT x LANES x 4 B            slot credits  (written by the receiver)
-//   [halo flags] 8 sides x 64 B                     fused halo exchange (arrival counters)
+//   [p2p ack]    P x NSLOT x 4 B                    slot credits  (written by the receiver)
 //   [ll]         2 parities x P x ll_cap            flag-in-data allreduce buffers
 //   [p2p slots]  P x NSLOT x slot_bytes             eager/streaming payload ring
 //   [p2p LL]     P x NSLOT x 16 KiB                 small messages, 8-byte {word, seq} stores
-//   [halo bufs]  2 parities x 8 sides x halo_cap
-//   [halo LL]    2 parities x 8 sides x 2*halo_cap  (fused stencil+halo kernels)
+//   [halo LL]    2 parities x 8 sides x halo_ll_cap flag-in-data halo exchange (b2_halo_ll.cuh)
 //   -- separate, growable segment --
 //   [staging]    2 parities x stage_half            collective staging
 // ---------------------------------------------------------------------------
@@ -116,17 +116,23 @@ struct B2Layout {
   size_t flags_off;
   size_t p2p_hdr_off;
   size_t p2p_ack_off;
-  size_t halo_flag_off;
   size_t ll_off;
   size_t ll_cap;          // bytes per (parity, source) LL buffer (wire bytes = 2x payload)
   size_t p2p_slot_off;
   size_t p2p_slot_bytes;
   size_t p2p_ll_off;      // P x NSLOT x (2 * B2_P2P_LL_MAX): flag-in-data copies of small messages
-  size_t halo_buf_off;
-  size_t halo_cap;        // bytes per (parity, direction)
-  size_t halo_ll_off;     // flag-in-data halo buffers of the fused stencil kernels
+  size_t halo_ll_off;     // flag-in-data halo buffers
   size_t halo_ll_cap;     // bytes per (parity, side): 8 B per element
   size_t total;
+};
+
+// Words of B2DevComm::ticket (local device memory).
+enum B2TicketWord : int {
+  TK_COLL = 0,        // collective ticket: staging parity and flag values, advanced once per launch
+  TK_COLL_FIN = 1,    // finish counter of the collective kernels
+  TK_FIN = 6,         // finish counter of the halo kernels
+  TK_RX = 32,         // [8] halo messages received per side
+  TK_TX = 40,         // [8] halo messages sent per side
 };
 
 // Device-visible communicator state; passed to kernels BY VALUE (pointers are
@@ -142,9 +148,7 @@ struct B2DevComm {
   B2Layout lay;
   // local (non-symmetric) device memory
   unsigned* epoch;                      // [B2_MAX_BLOCKS] per-CTA barrier epochs
-  unsigned* ticket;                     // [0] collective ticket [1] finish ctr [3] halo finish ctr
-                                        // [8..15] halo msgs received per side [16..23] sent per side
-                                        // [5] fused-halo ready ctr [6] finish ctr [32..47] fused rx/tx
+  unsigned* ticket;                     // [64] counters, see B2TicketWord
   unsigned* p2p_send_seq;               // [P] fragments sent to each destination
   unsigned* p2p_recv_seq;               // [P] fragments consumed from each source
   unsigned* p2p_ctl;                    // [8] arrive counters / any-source election word

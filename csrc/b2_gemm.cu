@@ -23,7 +23,6 @@
 // + per-tile collective, each owning 64 rows of the 128 x 128 tile.
 // Persistent: grid = min(#tiles, #SMs), every CTA walks tiles blockIdx.x, +gridDim.x, ...
 // Shapes: M, N multiples of 128, K multiple of 64 (checked by the host wrapper).
-#include <cstdio>
 #include <cstring>
 
 #include <cuda.h>
@@ -32,11 +31,6 @@
 #include "b2_device.cuh"
 #include "b2_runtime.h"
 #include "b2_gemm_raster.h"
-
-extern "C" void b2_set_error(const char* fmt, ...);
-extern "C" void b2_count_launch(B2Comm* c);
-extern "C" int b2_tensor_map_2d_bf16(CUtensorMap* out, const void* ptr, unsigned long long rows,
-                                     unsigned long long cols, unsigned box_rows, unsigned box_cols);
 
 namespace {
 
@@ -316,23 +310,15 @@ extern "C" int b2_gemm_allreduce(B2Comm* c, const void* A, const void* B, void* 
   const size_t smem = (size_t)STAGES * (A_STAGE_BYTES + B_STAGE_BYTES) + 1024;
   static bool attr_set = false;
   if (!attr_set) {
-    cudaError_t e = cudaFuncSetAttribute(b2_k_gemm_allreduce, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    if (e != cudaSuccess) {
-      b2_set_error("gemm_allreduce: cannot reserve %zu bytes of shared memory: %s", smem,
-                   cudaGetErrorString(e));
-      return 1000 + (int)e;
-    }
+    if (int rc = b2_cuda_check(cudaFuncSetAttribute(b2_k_gemm_allreduce, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                                    (int)smem),
+                               "gemm_allreduce: cannot reserve %zu bytes of shared memory", smem))
+      return rc;
     attr_set = true;
   }
   const int tiles = (M / BM) * (N / BN);
   int grid = tiles < c->sm_count ? tiles : c->sm_count;
   if (grid > B2_MAX_BLOCKS) grid = B2_MAX_BLOCKS;
   b2_k_gemm_allreduce<<<grid, GEMM_THREADS, smem, stream>>>(ta, tb, c->dev, g);
-  b2_count_launch(c);
-  cudaError_t err = cudaGetLastError();
-  if (err != cudaSuccess) {
-    b2_set_error("gemm_allreduce: kernel launch failed: %s", cudaGetErrorString(err));
-    return 1000 + (int)err;
-  }
-  return 0;
+  return b2_launched(c, "gemm_allreduce");
 }

@@ -4,20 +4,13 @@
 // A halo element travels as ONE 8-byte store {value, flag}; 8-byte stores are atomic, so a reader
 // that sees the flag sees the value: no fence, no separate signal, one NVLink one-way latency.
 // flag = (messages sent on this side so far) + 1, buffer parity = that count & 1; both ends of
-// a channel count the same messages in device memory (c.ticket[32..47]), so kernels using this
-// transport can be mixed freely and replayed from CUDA graphs.
+// a channel count the same messages in device memory (c.ticket[TK_RX + side] / [TK_TX + side]), so
+// kernels using this transport can be mixed freely and replayed from CUDA graphs.
 #pragma once
 
 #include "b2_device.cuh"
 
 enum { FS_W = 0, FS_E, FS_S, FS_N, FS_SW, FS_SE, FS_NW, FS_NE, FS_NSIDES };
-
-// ticket words (local device memory)
-#define TK_READY 5     // fused kernels: += 1 per unpacker CTA, reset by the last CTA of the kernel
-#define TK_FIN 6       // finish counter
-#define TK_TILE 7      // fused kernels: dynamic tile scheduler (reset by the last CTA)
-#define TK_RX 32       // [8] messages received per side
-#define TK_TX 40       // [8] messages sent per side
 
 __device__ __forceinline__ uint2* fz_buf(const B2DevComm& c, int rank, unsigned parity, int side) {
   return (uint2*)(c.heap[rank] + c.lay.halo_ll_off +
@@ -47,4 +40,24 @@ __device__ __forceinline__ float fz_get(const B2DevComm& c, const uint2* p, unsi
     }
   }
   return __uint_as_float(v);
+}
+
+// End of an exchange kernel: after every thread of the CTA is done, the last CTA to finish advances
+// the per-side message counters of the sides that have a neighbour.
+__device__ __forceinline__ void fz_finish(const B2DevComm& c, const int (&nb)[FS_NSIDES],
+                                          const unsigned* s_rx, const unsigned* s_tx) {
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    __threadfence();
+    const unsigned old = atomicAdd(c.ticket + TK_FIN, 1u);
+    if (old == gridDim.x - 1) {
+      b2_st_volatile(c.ticket + TK_FIN, 0u);
+      for (int k = 0; k < FS_NSIDES; ++k)
+        if (nb[k] >= 0) {
+          b2_st_volatile(c.ticket + TK_RX + k, s_rx[k] + 1u);
+          b2_st_volatile(c.ticket + TK_TX + k, s_tx[k] + 1u);
+        }
+      __threadfence();
+    }
+  }
 }

@@ -48,9 +48,21 @@ extern "C" int b2_pdl_enabled(void) {
   return g_pdl;
 }
 extern "C" void b2_set_pdl(int enable) { g_pdl = enable ? 1 : 0; }
-extern "C" void b2_count_launch(B2Comm* c) {
+extern "C" int b2_cuda_check(cudaError_t e, const char* fmt, ...) {
+  if (e == cudaSuccess) return 0;
+  char what[512];
+  va_list ap;
+  va_start(ap, fmt);
+  vsnprintf(what, sizeof what, fmt, ap);
+  va_end(ap);
+  b2_set_error("%s: %s", what, cudaGetErrorString(e));
+  return 1000 + (int)e;
+}
+
+extern "C" int b2_launched(B2Comm* c, const char* name) {
   ++g_launches;
   if (c) ++c->launches;
+  return b2_cuda_check(cudaGetLastError(), "%s: kernel launch failed", name);
 }
 
 static void emit(const std::string& line) {
@@ -76,8 +88,8 @@ struct B2DebugScope {
 
 // Logging is a debugging aid: it synchronises the stream in b2_debug_end to read the
 // device time, exactly like the reference's blocking calls; disabled -> zero overhead.
-extern "C" B2DebugScope* b2_debug_begin(B2Comm* c, const char* opname, const char* details,
-                                         cudaStream_t stream) {
+extern "C" B2DebugScope* b2_debug_begin(B2Comm* c, const char* opname, cudaStream_t stream,
+                                         const char* fmt, ...) {
   if (!g_logging) return nullptr;
   B2DebugScope* s = new B2DebugScope();
   char buf[256];
@@ -85,7 +97,14 @@ extern "C" B2DebugScope* b2_debug_begin(B2Comm* c, const char* opname, const cha
   s->prefix = buf;
   s->timed = false;
   s->stream = nullptr;
-  emit(s->prefix + (details && details[0] ? std::string(" ") + details : std::string()));
+  char details[160] = "";
+  if (fmt) {
+    va_list ap;
+    va_start(ap, fmt);
+    vsnprintf(details, sizeof details, fmt, ap);
+    va_end(ap);
+  }
+  emit(s->prefix + (details[0] ? std::string(" ") + details : std::string()));
   // events cannot be timed inside a stream capture; log without device time there
   cudaStreamCaptureStatus st = cudaStreamCaptureStatusNone;
   if (cudaStreamIsCapturing(stream, &st) == cudaSuccess && st == cudaStreamCaptureStatusNone &&

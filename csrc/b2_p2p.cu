@@ -38,18 +38,10 @@
 // so the header needs no release fence over the payload and the message costs ONE NVLink one-way
 // latency (the halo kernels' transport, b2_halo_ll.cuh).  Matching, tags, Status and credits are
 // unchanged: the header is still written, its size field tells the receiver which format to read.
-#include <cstdio>
 #include <cstring>
 
 #include "b2_device.cuh"
 #include "b2_runtime.h"
-
-extern "C" void b2_set_error(const char* fmt, ...);
-extern "C" void b2_count_launch(B2Comm* c);
-struct B2DebugScope;
-extern "C" B2DebugScope* b2_debug_begin(B2Comm* c, const char* opname, const char* details,
-                                         cudaStream_t stream);
-extern "C" void b2_debug_end(B2DebugScope* s, int code);
 
 // p2p_ctl words
 #define CTL_SEND_FIN 0     // finish counter, send role
@@ -453,20 +445,12 @@ static int launch_p2p(B2Comm* c, B2P2PArgs& a, const char* name, cudaStream_t st
   }
   a.anysource_scan = c->p2p_anysource_scan;
   b2_k_p2p<<<a.send_lanes + a.recv_lanes, B2_THREADS, 0, stream>>>(c->dev, a);
-  b2_count_launch(c);
-  cudaError_t err = cudaGetLastError();
-  if (err != cudaSuccess) {
-    b2_set_error("%s: kernel launch failed: %s", name, cudaGetErrorString(err));
-    return 1000 + (int)err;
-  }
-  return 0;
+  return b2_launched(c, name);
 }
 
 extern "C" int b2_send(B2Comm* c, const void* buf, size_t nbytes, int dest, int tag,
                        cudaStream_t stream) {
-  char det[128];
-  snprintf(det, sizeof det, "%zu bytes to %d with tag %d", nbytes, dest, tag);
-  B2DebugScope* dbg = b2_debug_begin(c, "Send", det, stream);
+  B2DebugScope* dbg = b2_debug_begin(c, "Send", stream, "%zu bytes to %d with tag %d", nbytes, dest, tag);
   B2P2PArgs a;
   memset(&a, 0, sizeof a);
   a.sendbuf = buf; a.send_bytes = nbytes; a.dest = dest; a.send_tag = tag;
@@ -479,9 +463,7 @@ extern "C" int b2_send(B2Comm* c, const void* buf, size_t nbytes, int dest, int 
 
 extern "C" int b2_recv(B2Comm* c, void* buf, size_t nbytes, int source, int tag,
                        B2StatusRecord* status, cudaStream_t stream) {
-  char det[128];
-  snprintf(det, sizeof det, "%zu bytes from %d with tag %d", nbytes, source, tag);
-  B2DebugScope* dbg = b2_debug_begin(c, "Recv", det, stream);
+  B2DebugScope* dbg = b2_debug_begin(c, "Recv", stream, "%zu bytes from %d with tag %d", nbytes, source, tag);
   B2P2PArgs a;
   memset(&a, 0, sizeof a);
   a.recvbuf = buf; a.recv_bytes = nbytes; a.source = source; a.recv_tag = tag;
@@ -496,10 +478,8 @@ extern "C" int b2_recv(B2Comm* c, void* buf, size_t nbytes, int source, int tag,
 extern "C" int b2_sendrecv(B2Comm* c, const void* sendbuf, size_t send_bytes, int dest, int sendtag,
                            void* recvbuf, size_t recv_bytes, int source, int recvtag,
                            B2StatusRecord* status, cudaStream_t stream) {
-  char det[160];
-  snprintf(det, sizeof det, "<%d (%zu bytes, tag %d) / >%d (%zu bytes, tag %d)", source, recv_bytes,
-           recvtag, dest, send_bytes, sendtag);
-  B2DebugScope* dbg = b2_debug_begin(c, "Sendrecv", det, stream);
+  B2DebugScope* dbg = b2_debug_begin(c, "Sendrecv", stream, "<%d (%zu bytes, tag %d) / >%d (%zu bytes, tag %d)",
+                                     source, recv_bytes, recvtag, dest, send_bytes, sendtag);
   B2P2PArgs a;
   memset(&a, 0, sizeof a);
   a.sendbuf = sendbuf; a.send_bytes = send_bytes; a.dest = dest; a.send_tag = sendtag;

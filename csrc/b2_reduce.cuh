@@ -200,27 +200,28 @@ b2_k_allreduce_ll(const B2DevComm c, const B2LLArgs a) {
 }
 
 // ---------------------------------------------------------------------------
-// host-side typed dispatch.  Each instance file defines B2_INST_GROUP and gets
-// the launchers for its dtype group only (keeps nvcc parallel and fast).
+// host-side typed dispatch.  Each b2_reduce_inst_N.cu registers the launchers of
+// one dtype group (keeps nvcc parallel and fast); the caller checks the launch.
 // ---------------------------------------------------------------------------
-typedef cudaError_t (*b2_reduce_launch_fn)(const B2DevComm&, const B2ReduceArgs&, int grid,
-                                           cudaStream_t);
-typedef cudaError_t (*b2_ll_launch_fn)(const B2DevComm&, const B2LLArgs&, int grid, cudaStream_t);
+typedef void (*b2_reduce_launch_fn)(const B2DevComm&, const B2ReduceArgs&, int grid, cudaStream_t);
+typedef void (*b2_ll_launch_fn)(const B2DevComm&, const B2LLArgs&, int grid, cudaStream_t);
 
 template <typename T, int OP>
-cudaError_t b2_launch_reduce(const B2DevComm& c, const B2ReduceArgs& a, int grid, cudaStream_t s) {
+void b2_launch_reduce(const B2DevComm& c, const B2ReduceArgs& a, int grid, cudaStream_t s) {
   b2_k_reduce_chunked<T, OP><<<grid, B2_THREADS, 0, s>>>(c, a);
-  return cudaGetLastError();
 }
 template <typename T, int OP>
-cudaError_t b2_launch_ll(const B2DevComm& c, const B2LLArgs& a, int grid, cudaStream_t s) {
+void b2_launch_ll(const B2DevComm& c, const B2LLArgs& a, int grid, cudaStream_t s) {
   b2_k_allreduce_ll<T, OP><<<grid, B2_THREADS, 0, s>>>(c, a);
-  return cudaGetLastError();
 }
 
 // tables filled by the instance files: [dtype][op] -> launcher (nullptr = invalid combo)
 extern b2_reduce_launch_fn b2_reduce_table[B2_DTYPE_COUNT][B2_OP_COUNT];
 extern b2_ll_launch_fn b2_ll_table[B2_DTYPE_COUNT][B2_OP_COUNT];
+void b2_register_reduce_group_0();
+void b2_register_reduce_group_1();
+void b2_register_reduce_group_2();
+void b2_register_reduce_group_3();
 
 #define B2_REG(DT, T, OP)                               \
   b2_reduce_table[DT][OP] = &b2_launch_reduce<T, OP>;   \

@@ -1,29 +1,9 @@
-// Typed instantiations of the fused reduce kernels, dtype group 1 (see b2_reduce.cuh).
+// Typed instantiations of the fused reduce kernels, dtype group 1: signed integers (see b2_reduce.cuh).
 #include "b2_reduce.cuh"
 
 void b2_register_reduce_group_1() {
-#if 1 == 0
-  B2_REG_ARITH(B2_F32, float)
-  B2_REG_ARITH(B2_F64, double)
-  B2_REG_ARITH(B2_F16, __half)
-  B2_REG_ARITH(B2_BF16, __nv_bfloat16)
-#elif 1 == 1
   B2_REG_INT(B2_I8, signed char)
   B2_REG_INT(B2_I16, short)
   B2_REG_INT(B2_I32, int)
   B2_REG_INT(B2_I64, long long)
-#elif 1 == 2
-  B2_REG_INT(B2_U8, unsigned char)
-  B2_REG_INT(B2_U16, unsigned short)
-  B2_REG_INT(B2_U32, unsigned int)
-  B2_REG_INT(B2_U64, unsigned long long)
-#else
-  B2_REG(B2_BOOL, b2_boolean, B2_LAND)
-  B2_REG(B2_BOOL, b2_boolean, B2_LOR)
-  B2_REG(B2_BOOL, b2_boolean, B2_LXOR)
-  B2_REG(B2_C64, b2_c64, B2_SUM)
-  B2_REG(B2_C64, b2_c64, B2_PROD)
-  B2_REG(B2_C128, b2_c128, B2_SUM)
-  B2_REG(B2_C128, b2_c128, B2_PROD)
-#endif
 }

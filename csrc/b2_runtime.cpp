@@ -15,8 +15,6 @@
 
 #include "b2_runtime.h"
 
-extern "C" void b2_set_error(const char* fmt, ...);
-
 // ---------------------------------------------------------------------------
 // driver API loader
 // ---------------------------------------------------------------------------
@@ -87,8 +85,6 @@ static const char* drv_err(CUresult r) {
       return ret;                                                             \
     }                                                                         \
   } while (0)
-
-static size_t round_up(size_t x, size_t m) { return (x + m - 1) / m * m; }
 
 extern "C" int b2_init(int device) {
   RT_CHECK(cudaSetDevice(device), 1);
@@ -358,15 +354,14 @@ static B2Layout make_layout(int nranks, size_t slot_bytes, size_t ll_cap, size_t
   L.flags_off = take((size_t)B2_MAX_BLOCKS * B2_MAX_RANKS * 4);
   L.p2p_hdr_off = take((size_t)nranks * B2_P2P_NSLOT * B2_P2P_MAX_LANES * 16);
   L.p2p_ack_off = take((size_t)nranks * B2_P2P_NSLOT * 4);
-  L.halo_flag_off = take(8 * 64);
   L.ll_cap = round_up(ll_cap, 4096);
   L.ll_off = take(2 * (size_t)nranks * L.ll_cap);
   L.p2p_slot_bytes = round_up(slot_bytes, 4096);
   L.p2p_slot_off = take((size_t)nranks * B2_P2P_NSLOT * L.p2p_slot_bytes);
   L.p2p_ll_off = take((size_t)nranks * B2_P2P_NSLOT * 2 * B2_P2P_LL_MAX);
-  L.halo_cap = round_up(halo_cap, 4096);
-  L.halo_buf_off = take(2 * 8 * L.halo_cap);
-  L.halo_ll_cap = 2 * L.halo_cap;
+  // 8 B per element: room for halo_cap payload bytes per side, plus the padding of every field's
+  // stride to a multiple of 4 elements (b2_halo_exchange): up to 3 x 8 B per field
+  L.halo_ll_cap = 2 * round_up(halo_cap, 4096) + 3 * 8 * B2_HALO_MAX_FIELDS;
   L.halo_ll_off = take(2 * 8 * L.halo_ll_cap);
   L.total = off;
   return L;
@@ -397,7 +392,7 @@ extern "C" B2Comm* b2_comm_create(int device, int rank, int nranks, B2Seg* ctl, 
   d.timeout_ns = (unsigned long long)(timeout_s * 1e9);
   d.lay = L;
   for (int p = 0; p < nranks; ++p) d.heap[p] = (char*)ctl->ptr[p];
-  // local counters: epoch[B2_MAX_BLOCKS] | ticket[8] | send_seq[16] | recv_seq[16] | p2p_ctl[32]
+  // local counters: epoch[B2_MAX_BLOCKS] | ticket[64] | send_seq[16] | recv_seq[16] | p2p_ctl[32]
   const size_t nwords = B2_MAX_BLOCKS + 64 + B2_MAX_RANKS + B2_MAX_RANKS + 32;
   unsigned* local = nullptr;
   if (cudaMalloc(&local, nwords * 4) != cudaSuccess || cudaMemset(local, 0, nwords * 4) != cudaSuccess) {
@@ -456,17 +451,23 @@ extern "C" int b2_comm_set_stage(B2Comm* c, B2Seg* stage, B2Mc* mc) {
 
 extern "C" size_t b2_comm_stage_half(B2Comm* c) { return c->dev.stage_half; }
 
-extern "C" int b2_comm_set_tuning(B2Comm* c, long long ll_max, long long oneshot_max,
-                                  long long nvls_min, int max_blocks) {
-  if (ll_max >= 0) c->ll_max = (size_t)ll_max;
-  if (oneshot_max >= 0) c->oneshot_max = (size_t)oneshot_max;
-  if (nvls_min >= 0) c->nvls_min = (size_t)nvls_min;
-  if (max_blocks > 0) c->max_blocks = max_blocks > B2_MAX_BLOCKS ? B2_MAX_BLOCKS : max_blocks;
-  return 0;
+// the transport thresholds (bytes)
+static size_t* threshold(B2Comm* c, const char* key) {
+  if (strcmp(key, "ll_max") == 0) return &c->ll_max;
+  if (strcmp(key, "oneshot_max") == 0) return &c->oneshot_max;
+  if (strcmp(key, "nvls_min") == 0) return &c->nvls_min;
+  return nullptr;
 }
 
 extern "C" int b2_comm_set_option(B2Comm* c, const char* key, long long value) {
-  if (strcmp(key, "bcast_mc_min") == 0) c->bcast_mc_min = (size_t)value;
+  size_t* t = threshold(c, key);
+  if ((t && value < 0) || (strcmp(key, "max_blocks") == 0 && value < 1)) {
+    b2_set_error("communicator option '%s': value %lld out of range", key, value);
+    return B2_ERR_BAD_ARG;
+  }
+  if (t) *t = (size_t)value;
+  else if (strcmp(key, "max_blocks") == 0) c->max_blocks = value > B2_MAX_BLOCKS ? B2_MAX_BLOCKS : (int)value;
+  else if (strcmp(key, "bcast_mc_min") == 0) c->bcast_mc_min = (size_t)value;
   else if (strcmp(key, "nvls_pipeline") == 0) c->nvls_pipeline = value != 0;
   else if (strcmp(key, "gemm_raster") == 0) c->gemm_raster = (int)value;
   else if (strcmp(key, "p2p_anysource_scan") == 0) c->p2p_anysource_scan = value != 0;
@@ -478,6 +479,7 @@ extern "C" int b2_comm_set_option(B2Comm* c, const char* key, long long value) {
 
 // read back what the launches use (tests/test_coresidency.py checks the grid cap against the SM count)
 extern "C" long long b2_comm_get_option(B2Comm* c, const char* key) {
+  if (const size_t* t = threshold(c, key)) return (long long)*t;
   if (strcmp(key, "max_blocks") == 0) return c->max_blocks;
   if (strcmp(key, "sm_count") == 0) return c->sm_count;
   if (strcmp(key, "bcast_mc_min") == 0) return (long long)c->bcast_mc_min;
@@ -547,6 +549,20 @@ extern "C" int b2_tensor_map_2d_bf16(CUtensorMap* out, const void* ptr, unsigned
     return 1;
   }
   return 0;
+}
+
+// Layout record for the import-time ABI check (mpi4jax_b200/_src/native/__init__.py): the Python
+// side mirrors these structs with ctypes, so a stale library with a different layout must be
+// rejected before the first call (the reference checks the MPI handle ABI the same way,
+// xla_bridge/__init__.py:23-89).
+extern "C" int b2_abi_info(int* out, int n) {
+  const int v[] = {B2_ABI_VERSION,
+                   (int)sizeof(B2StatusRecord), (int)sizeof(B2HaloDesc), (int)sizeof(B2SweParams),
+                   (int)sizeof(B2SweState), (int)sizeof(B2ErrorRecord), B2_MAX_RANKS, B2_P2P_NSLOT,
+                   (int)sizeof(B2SweCA)};
+  const int have = (int)(sizeof(v) / sizeof(v[0]));
+  for (int i = 0; i < n && i < have; ++i) out[i] = v[i];
+  return have;
 }
 
 // ---------------------------------------------------------------------------

@@ -109,10 +109,10 @@ B2Comm* b2_comm_create(int device, int rank, int nranks, B2Seg* ctl, size_t slot
                        size_t ll_cap, size_t halo_cap, double timeout_s);
 int b2_comm_set_stage(B2Comm* c, B2Seg* stage, B2Mc* mc);
 size_t b2_comm_stage_half(B2Comm* c);
-int b2_comm_set_tuning(B2Comm* c, long long ll_max, long long oneshot_max, long long nvls_min,
-                       int max_blocks);
+// keys: "ll_max", "oneshot_max", "nvls_min" (bytes), "max_blocks", "bcast_mc_min", "nvls_pipeline",
+// "gemm_raster", "p2p_anysource_scan", "trace_ptr", "trace_cap"; get_option also reads "sm_count"
 int b2_comm_set_option(B2Comm* c, const char* key, long long value);
-long long b2_comm_get_option(B2Comm* c, const char* key);   // "bcast_mc_min", "nvls_pipeline"
+long long b2_comm_get_option(B2Comm* c, const char* key);
 int b2_comm_check_error(B2Comm* c, char* buf, int buflen);     // 0 = ok
 int b2_comm_destroy(B2Comm* c);
 size_t b2_stage_need(int opcode, int nranks, size_t blk_bytes); // staging half needed by an op
@@ -177,6 +177,55 @@ struct B2HaloDesc {
   int at_north_wall;                  // last row of processes (v wall)
 };
 int b2_halo_exchange(B2Comm* c, const B2HaloDesc* d, cudaStream_t stream);
+
+struct B2SweParams {
+  int ny, nx, pitch;
+  float dx, dy, dt, gravity, viscosity;
+  float rdx, rdy;             // 1/dx, 1/dy: x * (1/dx) instead of x / dx (<= 1 ulp apart, ~8x cheaper)
+  float ab_a, ab_b;           // Adams-Bashforth weights
+  int first_step;
+  int south_wall, north_wall; // this rank touches the y walls (hc edge padding)
+  const float* coriolis;      // [ny]
+  // folded constants (fp32 products formed on the host, models/shallow_water.py)
+  float c_gx, c_gy;           // -gravity / dx, -gravity / dy
+  float c_nux, c_nuy;         // viscosity / dx, viscosity / dy
+  float c_fx, c_fy;           // dt * viscosity / dx^2, dt * viscosity / dy^2
+};
+
+// Device pointers of a model's fields (mirrored by ctypes in _src/native/__init__.py; the layout
+// is part of the ABI checked at import).  h0/h1, u/u1 and v/v1 are ping-pong pairs.
+struct B2SweState {
+  float *h0, *h1, *u, *v, *dh, *du, *dv, *fe, *fn, *q, *ke, *fe2, *fn2;
+  float* u1;
+  float* v1;
+};
+
+// "ext" arrays of the communication-avoiding step (b2_swe_ca_body.cuh): [(ny + 4) x epitch] floats,
+// cell (j, i) at (j + 2) * epitch + (i + 2); only cells beyond the interior (and the ring mirror) are used
+struct B2SweCA {
+  float *hx, *upx, *vpx, *uppx, *vppx;
+  int epitch;
+  int cb1;            // first column of the east frame: a multiple of 4, <= nx - 4 (filled in natively)
+};
+
+int b2_swe_multistep(B2Comm* c, const B2SweParams* p0, const B2SweState* st, const B2HaloDesc* topo,
+                     int nsteps, int first_step, cudaStream_t s);
+// struct sizes for the import-time ABI check (mpi4jax_b200/_src/native/__init__.py)
+int b2_abi_info(int* out, int n);
+
+// --- internal: shared by the translation units, not called from Python --------
+void b2_set_error(const char* fmt, ...) __attribute__((format(printf, 1, 2)));
+// 0 if `e` is cudaSuccess; otherwise sets the last error to "<fmt...>: <CUDA error string>" and returns 1000 + e
+int b2_cuda_check(cudaError_t e, const char* fmt, ...) __attribute__((format(printf, 2, 3)));
+// after a kernel launch: counts it (b2_launch_count), then b2_cuda_check(cudaGetLastError(), "<name>: kernel launch failed")
+int b2_launched(B2Comm* c, const char* name);
+// per-call debug log (b2_logging.cpp): `fmt` (may be null) formats the details only when logging is on
+struct B2DebugScope;
+B2DebugScope* b2_debug_begin(B2Comm* c, const char* opname, cudaStream_t stream, const char* fmt, ...)
+    __attribute__((format(printf, 4, 5)));
+void b2_debug_end(B2DebugScope* s, int code);
+int b2_tensor_map_2d_bf16(CUtensorMap* out, const void* ptr, unsigned long long rows, unsigned long long cols,
+                          unsigned box_rows, unsigned box_cols);
 
 #ifdef __cplusplus
 }

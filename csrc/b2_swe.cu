@@ -25,13 +25,6 @@
 // loads, only the two x-neighbours of the group are scalar loads (L1 hits).
 // These kernels are pure streaming stencils (1 FLOP per ~2 bytes): the roofline
 // is HBM bandwidth, there is no tensor-core work in this workload.
-#include <cstdio>
-
-#include "b2_runtime.h"
-
-extern "C" void b2_set_error(const char* fmt, ...);
-extern "C" void b2_count_launch(B2Comm* c);
-
 #include "b2_swe_body.cuh"
 #include "b2_launch.cuh"
 
@@ -85,16 +78,6 @@ static unsigned swe_blocks(const B2SweParams* p) {
   return (unsigned)((n + SWE_THREADS - 1) / SWE_THREADS);
 }
 
-static int swe_done(B2Comm* c, const char* name) {
-  b2_count_launch(c);
-  cudaError_t err = cudaGetLastError();
-  if (err != cudaSuccess) {
-    b2_set_error("%s: kernel launch failed: %s", name, cudaGetErrorString(err));
-    return 1000 + (int)err;
-  }
-  return 0;
-}
-
 static int swe_check(const B2SweParams* p) {
   if (p->pitch % 4 != 0 || p->pitch < p->nx || p->ny < 3 || p->nx < 3) {
     b2_set_error("swe: need ny,nx >= 3 and a row pitch that is a multiple of 4 floats and >= nx "
@@ -108,7 +91,7 @@ static int b2_swe_fluxes(B2Comm* c, const B2SweParams* p, const float* h, const 
                   float* fe, float* fn, float* q, float* ke, cudaStream_t s) {
   if (int rc = swe_check(p)) return rc;
   b2_launch(swe_k1_fluxes, swe_blocks(p), SWE_THREADS, 0, s, *p, h, u, v, fe, fn, q, ke);
-  return swe_done(c, "swe_fluxes");
+  return b2_launched(c, "swe_fluxes");
 }
 
 static int b2_swe_tendencies(B2Comm* c, const B2SweParams* p, const float* h, float* h_new, float* u,
@@ -116,7 +99,7 @@ static int b2_swe_tendencies(B2Comm* c, const B2SweParams* p, const float* h, fl
                       const float* q, const float* ke, cudaStream_t s) {
   if (int rc = swe_check(p)) return rc;
   b2_launch(swe_k2_tendencies, swe_blocks(p), SWE_THREADS, 0, s, *p, h, h_new, u, v, dh, du, dv, fe, fn, q, ke);
-  return swe_done(c, "swe_tendencies");
+  return b2_launched(c, "swe_tendencies");
 }
 
 // friction-u flux + apply + friction-v flux in one kernel (no fe/fn round trip through HBM)
@@ -129,14 +112,14 @@ static int b2_swe_friction_u_fused(B2Comm* c, const B2SweParams* p, const float*
     return B2_ERR_BAD_ARG;
   }
   b2_launch(swe_k34_friction_u, swe_blocks(p), SWE_THREADS, 0, s, *p, u, u_new, v, fe2, fn2, has_south);
-  return swe_done(c, "swe_friction_u_fused");
+  return b2_launched(c, "swe_friction_u_fused");
 }
 
 static int b2_swe_friction_v(B2Comm* c, const B2SweParams* p, float* v, const float* fe2, const float* fn2,
                       cudaStream_t s) {
   if (int rc = swe_check(p)) return rc;
   b2_launch(swe_k5_friction_v, swe_blocks(p), SWE_THREADS, 0, s, *p, v, fe2, fn2);
-  return swe_done(c, "swe_friction_v");
+  return b2_launched(c, "swe_friction_v");
 }
 
 extern "C" {
@@ -147,20 +130,6 @@ extern "C" {
 // capture turns into a single replayable graph.  `h0`/`h1` ping-pong (their wall rows are
 // initialised identically and never written); the state is returned in h0 (an odd step count
 // ends with one device copy).
-// Layout record for the import-time ABI check (mpi4jax_b200/_src/native/__init__.py): the Python
-// side mirrors these structs with ctypes, so a stale library with a different layout must be
-// rejected before the first call (the reference checks the MPI handle ABI the same way,
-// xla_bridge/__init__.py:23-89).
-int b2_abi_info(int* out, int n) {
-  const int v[] = {B2_ABI_VERSION,
-                   (int)sizeof(B2StatusRecord), (int)sizeof(B2HaloDesc), (int)sizeof(B2SweParams),
-                   (int)sizeof(B2SweState), (int)sizeof(B2ErrorRecord), B2_MAX_RANKS, B2_P2P_NSLOT,
-                   (int)sizeof(B2SweCA)};
-  const int have = (int)(sizeof(v) / sizeof(v[0]));
-  for (int i = 0; i < n && i < have; ++i) out[i] = v[i];
-  return have;
-}
-
 int b2_swe_multistep(B2Comm* c, const B2SweParams* p0, const B2SweState* st, const B2HaloDesc* topo,
                      int nsteps, int first_step, cudaStream_t s) {
   B2SweParams p = *p0;
@@ -202,22 +171,11 @@ int b2_swe_multistep(B2Comm* c, const B2SweParams* p0, const B2SweState* st, con
     }
     float* t = h; h = hn; hn = t;
   }
-  if (rc == 0 && u != st->u) {
-    cudaError_t e = cudaMemcpyAsync(st->u, u, (size_t)p.ny * p.pitch * sizeof(float),
-                                    cudaMemcpyDeviceToDevice, s);
-    if (e != cudaSuccess) {
-      b2_set_error("swe_multistep: copy failed: %s", cudaGetErrorString(e));
-      rc = 1000 + (int)e;
-    }
-  }
-  if (rc == 0 && h != st->h0) {
-    cudaError_t e = cudaMemcpyAsync(st->h0, h, (size_t)p.ny * p.pitch * sizeof(float),
-                                    cudaMemcpyDeviceToDevice, s);
-    if (e != cudaSuccess) {
-      b2_set_error("swe_multistep: copy failed: %s", cudaGetErrorString(e));
-      rc = 1000 + (int)e;
-    }
-  }
+  const size_t bytes = (size_t)p.ny * p.pitch * sizeof(float);
+  if (rc == 0 && u != st->u)
+    rc = b2_cuda_check(cudaMemcpyAsync(st->u, u, bytes, cudaMemcpyDeviceToDevice, s), "swe_multistep: copy failed");
+  if (rc == 0 && h != st->h0)
+    rc = b2_cuda_check(cudaMemcpyAsync(st->h0, h, bytes, cudaMemcpyDeviceToDevice, s), "swe_multistep: copy failed");
   return rc;
 }
 

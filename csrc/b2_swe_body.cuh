@@ -13,36 +13,6 @@
 
 #include "b2_runtime.h"
 
-struct B2SweParams {
-  int ny, nx, pitch;
-  float dx, dy, dt, gravity, viscosity;
-  float rdx, rdy;             // 1/dx, 1/dy: x * (1/dx) instead of x / dx (<= 1 ulp apart, ~8x cheaper)
-  float ab_a, ab_b;           // Adams-Bashforth weights
-  int first_step;
-  int south_wall, north_wall; // this rank touches the y walls (hc edge padding)
-  const float* coriolis;      // [ny]
-  // folded constants (fp32 products formed on the host, models/shallow_water.py)
-  float c_gx, c_gy;           // -gravity / dx, -gravity / dy
-  float c_nux, c_nuy;         // viscosity / dx, viscosity / dy
-  float c_fx, c_fy;           // dt * viscosity / dx^2, dt * viscosity / dy^2
-};
-
-// Device pointers of a model's fields (mirrored by ctypes in _src/native/__init__.py; the layout
-// is part of the ABI checked at import).  h0/h1, u/u1 and v/v1 are ping-pong pairs.
-struct B2SweState {
-  float *h0, *h1, *u, *v, *dh, *du, *dv, *fe, *fn, *q, *ke, *fe2, *fn2;
-  float* u1;
-  float* v1;
-};
-
-// "ext" arrays of the communication-avoiding step (b2_swe_ca_body.cuh): [(ny + 4) x epitch] floats,
-// cell (j, i) at (j + 2) * epitch + (i + 2); only cells beyond the interior (and the ring mirror) are used
-struct B2SweCA {
-  float *hx, *upx, *vpx, *uppx, *vppx;
-  int epitch;
-  int cb1;            // first column of the east frame: a multiple of 4, <= nx - 4 (filled in natively)
-};
-
 #define SWE_THREADS 256
 
 // An aligned group of four cells plus its west / east neighbours.

@@ -16,19 +16,12 @@
 // rank) 75 MB, more than the 50 MB L2 of an H100, so fewer passes means less HBM traffic.  The NVLink round of X is
 // hidden behind the bulk kernels.  Under CUDA-graph capture (mpi4jax_b200.jit) the event fork /
 // join becomes graph edges.  16 array passes per step instead of 32, one exchange instead of three.
-#include <cstdio>
-#include <cstdlib>
 
 #include "b2_device.cuh"
 #include "b2_halo_ll.cuh"
 #include "b2_runtime.h"
 #include "b2_swe_ca_body.cuh"
 #include "b2_swe_k12_body.cuh"
-
-extern "C" void b2_set_error(const char* fmt, ...);
-extern "C" void b2_count_launch(B2Comm* c);
-extern "C" int b2_swe_multistep(B2Comm* c, const B2SweParams* p0, const B2SweState* st,
-                                const B2HaloDesc* topo, int nsteps, int first_step, cudaStream_t s);
 
 #define CA_THREADS 256
 
@@ -211,20 +204,7 @@ __global__ void __launch_bounds__(CA_THREADS) b2_k_halo_ca(const B2DevComm c, co
     const float val = fz_get(c, fz_buf(c, c.rank, s_rx[s] & 1u, s) + e, s_rx[s] + 1u, s);
     ca_scatter(ny, nx, pitch, epitch, s, e, jlo, jhi, val, d.field, ext.a);
   }
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    __threadfence();
-    const unsigned old = atomicAdd(c.ticket + TK_FIN, 1u);
-    if (old == gridDim.x - 1) {
-      b2_st_volatile(c.ticket + TK_FIN, 0u);
-      for (int k = 0; k < FS_NSIDES; ++k)
-        if (nb[k] >= 0) {
-          b2_st_volatile(c.ticket + TK_RX + k, s_rx[k] + 1u);
-          b2_st_volatile(c.ticket + TK_TX + k, s_tx[k] + 1u);
-        }
-      __threadfence();
-    }
-  }
+  fz_finish(c, nb, s_rx, s_tx);
   ca_stamp_end(ts);
 }
 
@@ -251,15 +231,6 @@ static int ca_streams() {
   return 0;
 }
 
-static int ca_done(B2Comm* c, const char* name) {
-  b2_count_launch(c);
-  cudaError_t err = cudaGetLastError();
-  if (err != cudaSuccess) {
-    b2_set_error("%s: kernel launch failed: %s", name, cudaGetErrorString(err));
-    return 1000 + (int)err;
-  }
-  return 0;
-}
 static unsigned ca_blocks(long long tasks, int threads) { return (unsigned)((tasks + threads - 1) / threads); }
 
 static int ca_check(B2Comm* c, const B2SweParams& p, const B2SweCA& x) {
@@ -312,7 +283,7 @@ static int ca_exchange(B2Comm* c, const B2HaloDesc& topo, const B2SweParams& p, 
   if (ctas < 8) ctas = 8;
   if (ctas > 120) ctas = 120;                            // all co-resident next to the bulk kernel's CTAs
   b2_k_halo_ca<<<ctas, CA_THREADS, 0, s>>>(c->dev, d, ext, x.epitch, ts);
-  return ca_done(c, "halo_ca");
+  return b2_launched(c, "halo_ca");
 }
 
 extern "C" {
@@ -339,12 +310,12 @@ int b2_swe_ca_init(B2Comm* c, const B2SweParams* p0, const B2SweState* st, const
   const size_t bytes = (size_t)p.ny * p.pitch * sizeof(float);
   if (cudaMemcpyAsync(st->ke, st->du, bytes, cudaMemcpyDeviceToDevice, s) != cudaSuccess ||
       cudaMemcpyAsync(st->fe2, st->dv, bytes, cudaMemcpyDeviceToDevice, s) != cudaSuccess) {
-    b2_set_error("swe_ca_init: cudaMemcpyAsync failed: %s", cudaGetErrorString(cudaGetLastError()));
+    b2_cuda_check(cudaGetLastError(), "swe_ca_init: cudaMemcpyAsync failed");
     return 1000;
   }
   const long long tasks = ca_ext_total(p) + 2LL * (p.nx - 2) + 2LL * (p.ny - 2);
   swe_ca_init_ext<<<ca_blocks(tasks, CA_THREADS), CA_THREADS, 0, s>>>(p, x, st->u, st->v);
-  return ca_done(c, "swe_ca_init_ext");
+  return b2_launched(c, "swe_ca_init_ext");
 }
 
 int b2_swe_multistep_ca(B2Comm* c, const B2SweParams* p0, const B2SweState* st, const B2SweCA* x0,
@@ -369,14 +340,8 @@ int b2_swe_multistep_ca(B2Comm* c, const B2SweParams* p0, const B2SweState* st, 
   const unsigned tend_blocks = ca_blocks(fa.total, CA_CELLS);
   const unsigned fric_blocks = ca_blocks(fd.total + ca_ext_total(p), CA_CELLS);
   int rc = 0;
-#define CA_RT(call)                                                              \
-  if (rc == 0) {                                                                 \
-    cudaError_t e_ = (call);                                                     \
-    if (e_ != cudaSuccess) {                                                     \
-      b2_set_error("swe_multistep_ca: %s failed: %s", #call, cudaGetErrorString(e_)); \
-      rc = 1000 + (int)e_;                                                       \
-    }                                                                            \
-  }
+#define CA_RT(call) \
+  if (rc == 0) rc = b2_cuda_check((call), "swe_multistep_ca: %s failed", #call);
   CA_RT(cudaEventRecord(e0, s));
   CA_RT(cudaStreamWaitEvent(s2, e0, 0));
   int cur = 0;
@@ -393,7 +358,7 @@ int b2_swe_multistep_ca(B2Comm* c, const B2SweParams* p0, const B2SweState* st, 
     // flux + tendency kernel now; its friction partner follows once kernel A has written u', v' of the
     // band next to the bulk (enqueued below, after A's event)
     swe_ca_bulk_k12<<<bulk_blocks, SWE_THREADS, 0, s>>>(sa, upf, vpf, ca_slot(it, 1));
-    if ((rc = ca_done(c, "swe_ca_bulk_k12"))) break;
+    if ((rc = b2_launched(c, "swe_ca_bulk_k12"))) break;
     CA_RT(cudaEventRecord(eB, s));
     // ---- frame stream: needs the bulk kernel of the previous step (u'', v'', h next to the frame)
     if (it > 0) CA_RT(cudaStreamWaitEvent(s2, eS, 0));
@@ -406,12 +371,12 @@ int b2_swe_multistep_ca(B2Comm* c, const B2SweParams* p0, const B2SweState* st, 
     ctx.dub = st->ke; ctx.dvb = st->fe2;
     ctx.upf = upf; ctx.vpf = vpf;
     swe_ca_tend_frame<<<tend_blocks, CA_CELLS * CA_TEND_WARPS, 0, s2>>>(ctx, fa, ca_slot(it, 0));
-    if ((rc = ca_done(c, "swe_ca_tend_frame"))) break;
+    if ((rc = b2_launched(c, "swe_ca_tend_frame"))) break;
     CA_RT(cudaEventRecord(eA, s2));
     CA_RT(cudaStreamWaitEvent(s, eA, 0));
     if (rc) break;
     swe_ca_bulk_fric<<<bulk_blocks, SWE_THREADS, 0, s>>>(sa, upf, vpf, ca_slot(it, 3));
-    if ((rc = ca_done(c, "swe_ca_bulk_fric"))) break;
+    if ((rc = b2_launched(c, "swe_ca_bulk_fric"))) break;
     CA_RT(cudaEventRecord(eS, s));
     if ((rc = ca_exchange(c, *topo, p, x, H[nxt], upf, vpf, s2, ca_slot(it, 2)))) break;
     // D overwrites u, v of the frame IN PLACE: the bulk kernel, whose stencil reads them next to the
@@ -420,7 +385,7 @@ int b2_swe_multistep_ca(B2Comm* c, const B2SweParams* p0, const B2SweState* st, 
     CA_RT(cudaStreamWaitEvent(s2, eB, 0));
     if (rc) break;
     swe_ca_fric_frame<<<fric_blocks, CA_CELLS * 3, 0, s2>>>(ctx, fd, st->u, st->v, ca_slot(it, 4));
-    if ((rc = ca_done(c, "swe_ca_fric_frame"))) break;
+    if ((rc = b2_launched(c, "swe_ca_fric_frame"))) break;
     CA_RT(cudaEventRecord(eD, s2));
     cur = nxt;
   }

@@ -56,6 +56,14 @@ def _lib():
     return native.lib
 
 
+def stage_need(opcode: int, nranks: int, blk_bytes: int) -> int:
+    """Staging bytes per parity that an op with ``blk_bytes`` per block needs: the Python twin of
+    ``b2_stage_need`` (csrc/b2_collectives.cu), which validates every launch with the same formula."""
+    stride = (blk_bytes + 15) & ~15
+    mult = nranks if opcode in (codes.OPC_ALLTOALL, codes.OPC_SCATTER) else 1
+    return stride * mult + 4096
+
+
 def abort_or_raise(message: str, code: int = 1):
     """The reference's fail-fast path (mpi_ops_common.h:60-78): print
     ``r<rank> | MPI_<op> returned error code ... - aborting`` and kill the job."""
@@ -267,11 +275,8 @@ class NativeComm:
         seen = _all_gather_obj(comm, sorted(self.tuning.items()))
         if any(t != seen[0] for t in seen):
             raise MPIError(f"the ranks disagree on the transport thresholds (MPI4JAX_B200_TUNING_FILE?): {seen}")
-        if any(self.tuning[k] != tuning.NATIVE_DEFAULTS[k] for k in ("ll_max", "oneshot_max", "nvls_min")):
-            lib.b2_comm_set_tuning(self.handle, self.tuning["ll_max"], self.tuning["oneshot_max"],
-                                   self.tuning["nvls_min"], 0)
-        if self.tuning["bcast_mc_min"] != tuning.NATIVE_DEFAULTS["bcast_mc_min"]:
-            lib.b2_comm_set_option(self.handle, b"bcast_mc_min", self.tuning["bcast_mc_min"])
+        for key in ("ll_max", "oneshot_max", "nvls_min", "bcast_mc_min"):
+            self.set_option(key, self.tuning[key])
         self.stage: Optional[_Segment] = None
         self._stage_half = 0
         self._retired: list = []
@@ -315,20 +320,14 @@ class NativeComm:
             self._retired.append(old)
 
     def ensure_stage(self, opcode: int, blk_bytes: int) -> None:
-        # same formula as b2_stage_need() (csrc/b2_collectives.cu), evaluated without leaving Python
-        stride = (blk_bytes + 15) & ~15
-        mult = self.comm.size if opcode in (codes.OPC_ALLTOALL, codes.OPC_SCATTER) else 1
-        need = stride * mult + 4096
+        need = stage_need(opcode, self.comm.size, blk_bytes)
         if need > self._stage_half:
             self._grow_stage(2 * need + 8192)
 
     def reserve(self, nbytes: int) -> None:
         """Make sure collectives of up to ``nbytes`` per rank (alltoall / scatter: per peer block
         times size) never have to grow the staging segment again.  Collective."""
-        stride = (int(nbytes) + 15) & ~15
-        need = stride * self.comm.size + 4096
-        if need > self._stage_half:
-            self._grow_stage(2 * need + 8192)
+        self.ensure_stage(codes.OPC_ALLTOALL, int(nbytes))
 
     @property
     def has_nvls(self) -> bool:
@@ -360,16 +359,14 @@ class NativeComm:
             raise MPIError(f"CUDA failure while flushing communication: {exc}") from exc
         self.check_device_error()
 
-    def set_tuning(self, ll_max=-1, oneshot_max=-1, nvls_min=-1, max_blocks=0) -> None:
-        _lib().b2_comm_set_tuning(self.handle, ll_max, oneshot_max, nvls_min, max_blocks)
-
     def set_option(self, key: str, value: int) -> None:
-        """Runtime switches of the native communicator: ``bcast_mc_min`` (bytes), ``nvls_pipeline`` (0/1),
-        ``gemm_raster``, ``p2p_anysource_scan`` (0/1)."""
+        """Runtime switches of the native communicator: the transport thresholds ``ll_max``,
+        ``oneshot_max``, ``nvls_min`` and ``bcast_mc_min`` (bytes), the grid cap ``max_blocks``,
+        ``nvls_pipeline`` (0/1), ``gemm_raster``, ``p2p_anysource_scan`` (0/1)."""
         self._check(_lib().b2_comm_set_option(self.handle, key.encode(), int(value)), "Comm_set_option")
 
     def get_option(self, key: str) -> int:
-        """Current value of a launch parameter: ``max_blocks``, ``sm_count``, ``bcast_mc_min``, ``nvls_pipeline``."""
+        """Current value of a launch parameter: any key of :meth:`set_option` but the trace buffer, or ``sm_count``."""
         value = int(_lib().b2_comm_get_option(self.handle, key.encode()))
         if value < 0:
             raise ValueError(f"unknown communicator option {key!r}")

@@ -66,9 +66,6 @@ class HostStagedComm:
     def destroy(self) -> None:
         pass
 
-    def set_tuning(self, *a, **k) -> None:
-        pass
-
     # -- the 12 ops ------------------------------------------------------------------
     def barrier(self) -> None:
         self.flush()                      # the reference: stream sync, then MPI_Barrier (cuda.cpp:75-86)

@@ -160,7 +160,6 @@ _SIGNATURES = {
     "b2_comm_create": (c_void_p, [c_int, c_int, c_int, c_void_p, c_size_t, c_size_t, c_size_t, c_double]),
     "b2_comm_set_stage": (c_int, [c_void_p, c_void_p, c_void_p]),
     "b2_comm_stage_half": (c_size_t, [c_void_p]),
-    "b2_comm_set_tuning": (c_int, [c_void_p, c_longlong, c_longlong, c_longlong, c_int]),
     "b2_comm_set_option": (c_int, [c_void_p, c_char_p, c_longlong]),
     "b2_comm_get_option": (c_longlong, [c_void_p, c_char_p]),
     "b2_comm_check_error": (c_int, [c_void_p, c_char_p, c_int]),
@@ -208,7 +207,7 @@ _SIGNATURES = {
 
 
 #: must equal B2_ABI_VERSION in csrc/b2_common.h
-ABI_VERSION = 10
+ABI_VERSION = 11
 _ABI_FIELDS = ("abi_version", "sizeof_status_record", "sizeof_halo_desc", "sizeof_swe_params",
                "sizeof_swe_state", "sizeof_error_record", "max_ranks", "p2p_nslot", "sizeof_swe_ca")
 

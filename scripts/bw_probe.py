@@ -59,7 +59,7 @@ ops = {
 }
 sms = nc.get_option("sm_count")
 for mb in ((sms, 2 * sms) if size > 2 else (64, sms, 2 * sms)):
-    nc.set_tuning(max_blocks=mb)
+    nc.set_option("max_blocks", mb)
     for pipe in (0, 1):
         nc.set_option("nvls_pipeline", pipe)
         row = {}
@@ -70,7 +70,7 @@ for mb in ((sms, 2 * sms) if size > 2 else (64, sms, 2 * sms)):
             row[name] = (round(us, 1), round(moved / us / 1e3, 1))
         if rank == 0:
             print(f"{mib} MiB max_blocks={mb} nvls_pipeline={pipe}:", row, flush=True)
-nc.set_tuning(max_blocks=sms)
+nc.set_option("max_blocks", sms)
 t = x.clone()
 us = time_graph(lambda: dist.all_reduce(t))
 us2 = time_graph(lambda: dist.broadcast(t, 0))

@@ -190,6 +190,43 @@ def test_ca_pipeline_under_a_cuda_graph_and_after_load_state():
 
 
 @pytest.mark.gpu
+def test_halo_exchange_at_the_halo_buffer_limit(monkeypatch):
+    """ops.halo_exchange on three float32 fields whose longer side (341) is not a multiple of 4, on a
+    communicator with 4 KiB halo buffers: 3 * 341 * 4 bytes fit the payload capacity, the padded
+    flag-in-data stride (3 * 344 * 8 bytes) needs the slack the buffers are sized with.  The result
+    must match the numpy model of the 8-neighbour exchange."""
+    import numpy as np
+
+    from mpi4jax_b200.ops import halo_exchange
+
+    from ._halo_sim import neighbors, new_exchange
+
+    if not torch.cuda.is_available():
+        pytest.skip("needs CUDA")
+    monkeypatch.setenv("MPI4JAX_B200_HALO_BYTES", "4096")
+    c = comm.Clone()                     # its native side is created with the small halo buffers
+    try:
+        size, rank = c.Get_size(), c.Get_rank()
+        PY, PX = 1, size
+        ny, nx = 341, 100
+        kinds = ("h", "u", "v")
+        rng = np.random.default_rng(7)
+        arrs = {k: [rng.standard_normal((ny, nx)).astype(np.float32) for _ in range(size)] for k in kinds}
+        fields = [torch.from_numpy(arrs[k][rank].copy()).to(c.device) for k in kinds]
+        py, px = divmod(rank, PX)
+        nb, dg = neighbors(py, px, PY, PX)
+        halo_exchange(fields, kinds, west=nb["west"], east=nb["east"], south=nb["south"], north=nb["north"],
+                      sw=dg["sw"], se=dg["se"], nw=dg["nw"], ne=dg["ne"], periodic_x=True,
+                      at_north_wall=py == PY - 1, comm=c)
+        m.flush()
+        for k, f in zip(kinds, fields):
+            new_exchange(arrs[k], PY, PX, k)
+            assert np.array_equal(f.cpu().numpy(), arrs[k][rank]), k
+    finally:
+        c.Free()
+
+
+@pytest.mark.gpu
 @pytest.mark.parametrize("pipeline", ["ca", "standalone"])
 def test_native_kernels_match_ops_path(pipeline):
     """CUDA stencil kernels vs the plain-torch fp32 implementation of the same discrete system

@@ -69,3 +69,17 @@ def test_abi_check_raises_and_can_be_skipped(tmp_path):
     res = subprocess.run([sys.executable, str(script)], capture_output=True, text=True, env=env, timeout=120)
     assert res.returncode == 0, res.stderr
     assert "loaded True" in res.stdout
+
+
+def test_staging_formula_matches_native():
+    """The staging segment is sized in Python with the formula the native core validates every
+    launch with (b2_stage_need, host code): both must agree for every op, size and world size."""
+    from mpi4jax_b200._src import native
+    from mpi4jax_b200._src.backends.cuda import stage_need
+
+    sizes = [0, 1, 15, 16, 17, 4095, 4096, 65537, (1 << 20) + 3, 1 << 30]
+    for opcode in range(13):                       # every B2OpCode
+        for nranks in range(1, 17):
+            for nbytes in sizes:
+                assert stage_need(opcode, nranks, nbytes) == native.lib.b2_stage_need(opcode, nranks, nbytes), \
+                    (opcode, nranks, nbytes)
