@@ -193,11 +193,14 @@ struct B2SweParams {
 };
 
 // Device pointers of a model's fields (mirrored by ctypes in _src/native/__init__.py; the layout
-// is part of the ABI checked at import).  h0/h1, u/u1 and v/v1 are ping-pong pairs.
+// is part of the ABI checked at import).  h0/h1, u/u1, v/v1, du/du1 and dv/dv1 are ping-pong pairs;
+// the first of each pair holds the state between calls.
 struct B2SweState {
   float *h0, *h1, *u, *v, *dh, *du, *dv, *fe, *fn, *q, *ke, *fe2, *fn2;
   float* u1;
   float* v1;
+  float* du1;
+  float* dv1;
 };
 
 // "ext" arrays of the communication-avoiding step (b2_swe_ca_body.cuh): [(ny + 4) x epitch] floats,

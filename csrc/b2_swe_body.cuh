@@ -1,5 +1,5 @@
 // mpi4jax_b200 -- shallow-water stencil bodies shared by every launch schedule: the stand-alone
-// kernels (b2_swe.cu), the fused flux+tendency / friction kernels (b2_swe_k12_body.cuh) and the
+// kernels (b2_swe.cu), the one-pass bulk kernel (b2_swe_k12_body.cuh) and the
 // scalar frame kernels of the communication-avoiding step (b2_swe_ca_body.cuh).
 // Each vector body handles one aligned group of 4 cells of row j: loads, arithmetic, vector stores.
 //

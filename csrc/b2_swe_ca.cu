@@ -3,19 +3,17 @@
 //
 // One model step (the reference's shallow_water_step, examples/shallow_water.py:270-403):
 //
-//   stream s  (bulk) :  B  flux + tendency (bulk) -----+-----> Fb friction (bulk) ----------+--> next step
-//                                                    ^ |  (u', v' of the band next to the bulk; B done
-//                                                    | v   before D overwrites the frame's u, v)
+//   stream s  (bulk) :  S  flux + tendency + friction of the bulk, one pass ---------------> next step
 //   stream s2 (frame):  A (tendencies, frame band) -> X (deep halo exchange) -> D (friction, frame + ext)
 //
-// B / Fb write only bulk cells, A / X / D own the frame: two edges between the streams inside a step
-// (A -> Fb, B -> D), two at the step boundary (B(t+1) reads what D(t) wrote next to the bulk, A(t+1)
-// what Fb(t) wrote next to the frame).  Only h is double-buffered (its stencil is read while h' is written);
-// u', v' travel through their own arrays between the tendency and the friction kernels, so u'', v''
-// and the tendencies are updated in place: nine arrays are live per step -- at 8 GPUs (2 M cells per
-// rank) 75 MB, more than the 50 MB L2 of an H100, so fewer passes means less HBM traffic.  The NVLink round of X is
-// hidden behind the bulk kernels.  Under CUDA-graph capture (mpi4jax_b200.jit) the event fork /
-// join becomes graph edges.  16 array passes per step instead of 32, one exchange instead of three.
+// S writes only bulk cells, A / X / D own the frame.  h, u, v, du and dv are ping-pong pairs: every
+// kernel reads this step's buffers and writes the next step's, and dh is updated cell by cell by the
+// kernel that owns the cell.  So the streams meet only at the step boundary: S(t+1) reads what D(t)
+// wrote next to the bulk, A(t+1) what S(t) wrote next to the frame.  Seven arrays are read once and
+// written once per step (12 array passes instead of the stand-alone path's 32; at 8 GPUs, 2 M cells
+// per rank, the step's working set is larger than the 50 MB L2 of an H100, so passes are HBM traffic),
+// one exchange instead of three, and the NVLink round of X is hidden behind S.  Under CUDA-graph
+// capture (mpi4jax_b200.jit) the event fork / join becomes graph edges.
 
 #include "b2_device.cuh"
 #include "b2_halo_ll.cuh"
@@ -124,35 +122,23 @@ __global__ void __launch_bounds__(CA_THREADS) swe_ca_init_ext(const B2SweParams 
   }
 }
 
-// ---- bulk kernels: flux + tendency, then friction, on whole float4 groups at least four cells from the
-// block edge (b2_swe_k12_body.cuh); u', v' of the bulk travel through the frame band's store
-// (upf / vpf), whose bulk cells are otherwise unused --------------
-struct BulkArgs {
-  B2SweParams p;
-  int cb1;                                           // bulk columns [4, cb1), bulk rows [4, ny - 4)
-  const float *h;                                    // h of this step
-  float *h_o;                                        // h' (the other buffer of the pair)
-  float *u, *v, *dh, *du, *dv;                       // read, then updated in place
-};
-__global__ void __launch_bounds__(SWE_THREADS, 3)
-swe_ca_bulk_k12(const BulkArgs a, float* __restrict__ up, float* __restrict__ vp, const CAStamp ts) {
+// ---- S: the bulk, one pass per step (b2_swe_k12_body.cuh) ---------------------------------------
+__global__ void __launch_bounds__(CA_BULK_WARPS * 32)
+swe_ca_bulk_step(const CABulkArgs a, const CAStamp ts) {
   ca_stamp_begin(ts);
-  const long long t = (long long)blockIdx.x * SWE_THREADS + threadIdx.x;
-  if (t < ca_bulk_tasks(a.p, a.cb1)) {
-    int j, i0;
-    ca_bulk_task(a.p, a.cb1, t, j, i0);
-    swe_k12_body(a.p, a.h, a.h_o, a.u, up, a.v, vp, a.dh, a.du, a.dv, a.dh, a.du, a.dv, j, i0);
-  }
-  ca_stamp_end(ts);
-}
-__global__ void __launch_bounds__(SWE_THREADS, 4)
-swe_ca_bulk_fric(const BulkArgs a, const float* __restrict__ up, const float* __restrict__ vp, const CAStamp ts) {
-  ca_stamp_begin(ts);
-  const long long t = (long long)blockIdx.x * SWE_THREADS + threadIdx.x;
-  if (t < ca_bulk_tasks(a.p, a.cb1)) {
-    int j, i0;
-    ca_bulk_task(a.p, a.cb1, t, j, i0);
-    swe_k345_body(a.p, up, a.u, vp, a.v, j, i0);
+  const int w = (int)blockIdx.x * CA_BULK_WARPS + (int)(threadIdx.x >> 5), lane = threadIdx.x & 31;
+  if (w < ca_bulk_warps(a)) {                          // (whole warps: the lane exchange needs all 32)
+    int s, e;
+    ca_bulk_rows(a, w / a.wcols, s, e);
+    CABulkLane L;
+    L.store = ca_bulk_lane(a, w % a.wcols, lane, L.i0);
+    ca_bulk_begin(a, L, s);
+    for (int t = s - 2; t <= e; ++t) {
+      ca_bulk_tend(a, L, t, t >= s && t < e);
+      const float uw2 = __shfl_up_sync(0xffffffffu, L.upn[2], 1), uw3 = __shfl_up_sync(0xffffffffu, L.upn[3], 1);
+      const float ue = __shfl_down_sync(0xffffffffu, L.upn[0], 1), ve = __shfl_down_sync(0xffffffffu, L.vpn[0], 1);
+      ca_bulk_fric(a, L, t, uw2, uw3, ue, ve, t == s, t > s);
+    }
   }
   ca_stamp_end(ts);
 }
@@ -210,7 +196,7 @@ __global__ void __launch_bounds__(CA_THREADS) b2_k_halo_ca(const B2DevComm c, co
 
 // ---- host side --------------------------------------------------------------------------------------
 static cudaStream_t g_side = nullptr;
-static cudaEvent_t g_ev[5];
+static cudaEvent_t g_ev[3];
 
 static int ca_streams() {
   if (g_side) return 0;
@@ -223,7 +209,7 @@ static int ca_streams() {
     g_side = nullptr;
     return 1;
   }
-  for (int k = 0; k < 5; ++k)
+  for (int k = 0; k < 3; ++k)
     if (cudaEventCreateWithFlags(&g_ev[k], cudaEventDisableTiming) != cudaSuccess) {
       b2_set_error("swe_ca: cudaEventCreate failed");
       return 1;
@@ -251,13 +237,34 @@ static int ca_check(B2Comm* c, const B2SweParams& p, const B2SweCA& x) {
   return 0;
 }
 
-// timeline buffer: [step][kernel 0 = A, 1 = B, 2 = X, 3 = Fb, 4 = D][start, end]
+// timeline buffer: [step][kernel 0 = A, 1 = S, 2 = X, 3 = D][start, end]
 static unsigned long long* g_stamps = nullptr;
 static int g_stamp_steps = 0;
 static CAStamp ca_slot(int step, int kernel) {
   CAStamp s;
-  s.slot = (g_stamps != nullptr && step >= 0 && step < g_stamp_steps) ? g_stamps + ((size_t)step * 5 + kernel) * 2 : nullptr;
+  s.slot = (g_stamps != nullptr && step >= 0 && step < g_stamp_steps) ? g_stamps + ((size_t)step * 4 + kernel) * 2 : nullptr;
   return s;
+}
+
+// Rows per segment of the bulk kernel: about two waves of warps on this GPU, so that the frame chain's
+// CTAs find free slots while the bulk runs, and at least 16 rows (a segment evaluates the tendencies of
+// three rows beyond its own).
+static int ca_bulk_rows_per_segment(const B2SweParams& p, int cb1) {
+  static int slot_warps = 0;
+  if (slot_warps == 0) {
+    int dev = 0, sms = 0, per_sm = 0;
+    cudaGetDevice(&dev);
+    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+    cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, swe_ca_bulk_step, CA_BULK_WARPS * 32, 0);
+    slot_warps = sms * per_sm * CA_BULK_WARPS;
+    if (slot_warps <= 0) slot_warps = 132 * 16;
+  }
+  CABulkArgs g;
+  g.p = p;
+  ca_bulk_geometry(p, cb1, 1, g);
+  const int nseg = (2 * slot_warps) / g.wcols > 1 ? (2 * slot_warps) / g.wcols : 1;
+  const int rows = (p.ny - 8 + nseg - 1) / nseg;
+  return rows < 16 ? 16 : rows;
 }
 
 static int ca_exchange(B2Comm* c, const B2HaloDesc& topo, const B2SweParams& p, const B2SweCA& x, float* f0,
@@ -288,7 +295,7 @@ static int ca_exchange(B2Comm* c, const B2HaloDesc& topo, const B2SweParams& p, 
 
 extern "C" {
 
-// Debug timeline: `buf` holds nsteps * 5 * 2 u64 (device memory, start slots preset to ~0, end slots to 0);
+// Debug timeline: `buf` holds nsteps * 4 * 2 u64 (device memory, start slots preset to ~0, end slots to 0);
 // pass null to switch it off again.  Applies to multistep calls (and graphs captured) afterwards.
 void b2_swe_ca_timeline(unsigned long long* buf, int nsteps) {
   g_stamps = buf;
@@ -306,13 +313,6 @@ int b2_swe_ca_init(B2Comm* c, const B2SweParams* p0, const B2SweState* st, const
   if (int rc = ca_check(c, p, x)) return rc;
   if (int rc = ca_streams()) return rc;       // (here, never inside a stream capture: reset / load_state are eager)
   if (int rc = ca_exchange(c, *topo, p, x, st->h0, st->u, st->v, s)) return rc;
-  // kernel A's private du, dv of the band-only cells (CACtx::dub / dvb) start as copies
-  const size_t bytes = (size_t)p.ny * p.pitch * sizeof(float);
-  if (cudaMemcpyAsync(st->ke, st->du, bytes, cudaMemcpyDeviceToDevice, s) != cudaSuccess ||
-      cudaMemcpyAsync(st->fe2, st->dv, bytes, cudaMemcpyDeviceToDevice, s) != cudaSuccess) {
-    b2_cuda_check(cudaGetLastError(), "swe_ca_init: cudaMemcpyAsync failed");
-    return 1000;
-  }
   const long long tasks = ca_ext_total(p) + 2LL * (p.nx - 2) + 2LL * (p.ny - 2);
   swe_ca_init_ext<<<ca_blocks(tasks, CA_THREADS), CA_THREADS, 0, s>>>(p, x, st->u, st->v);
   return b2_launched(c, "swe_ca_init_ext");
@@ -329,13 +329,20 @@ int b2_swe_multistep_ca(B2Comm* c, const B2SweParams* p0, const B2SweState* st, 
   if (int rc = ca_check(c, p, x)) return rc;
   if (int rc = ca_streams()) return rc;
   const cudaStream_t s2 = g_side;
-  const cudaEvent_t e0 = g_ev[0], eS = g_ev[1], eD = g_ev[2], eA = g_ev[3], eB = g_ev[4];
-  const unsigned bulk_blocks = ca_blocks(ca_bulk_tasks(p, x.cb1), SWE_THREADS);
-  // the flux arrays of the stand-alone path are free here: fe / fn hold u', v' between the tendency and
-  // the friction kernels, ke / fe2 kernel A's copy of du, dv on the band-only cells
+  const cudaEvent_t e0 = g_ev[0], eS = g_ev[1], eD = g_ev[2];
+  // ping-pong pairs: [cur] = this step's, [nxt] = the next step's; the flux arrays of the stand-alone
+  // path are free here: fe / fn hold u', v' of the frame band between kernels A, X and D
   float* H[2] = {st->h0, st->h1};
+  float* U[2] = {st->u, st->u1};
+  float* V[2] = {st->v, st->v1};
+  float* DU[2] = {st->du, st->du1};
+  float* DV[2] = {st->dv, st->dv1};
   float* const upf = st->fe;
   float* const vpf = st->fn;
+  CABulkArgs sa;
+  sa.p = p;
+  ca_bulk_geometry(p, x.cb1, ca_bulk_rows_per_segment(p, x.cb1), sa);
+  const unsigned bulk_blocks = ca_blocks(ca_bulk_warps(sa), CA_BULK_WARPS);
   const CAFrame fa = ca_frame(p, 5, x.cb1 - 2), fd = ca_frame(p, 3, x.cb1);
   const unsigned tend_blocks = ca_blocks(fa.total, CA_CELLS);
   const unsigned fric_blocks = ca_blocks(fd.total + ca_ext_total(p), CA_CELLS);
@@ -348,50 +355,42 @@ int b2_swe_multistep_ca(B2Comm* c, const B2SweParams* p0, const B2SweState* st, 
   for (int it = 0; it < nsteps && rc == 0; ++it) {
     const int nxt = cur ^ 1;
     p.first_step = (first_step && it == 0) ? 1 : 0;
+    // ---- frame stream: needs the bulk kernel of the previous step (u'', v'', h next to the frame);
+    // enqueued before this step's bulk kernel re-records eS
+    if (it > 0) CA_RT(cudaStreamWaitEvent(s2, eS, 0));
     // ---- bulk stream: needs D of the previous step (u'', v'' of the frame, the arrays' halos)
     if (it > 0) CA_RT(cudaStreamWaitEvent(s, eD, 0));
     if (rc) break;
-    BulkArgs sa;
-    sa.p = p; sa.cb1 = x.cb1;
-    sa.h = H[cur]; sa.h_o = H[nxt];
-    sa.u = st->u; sa.v = st->v; sa.dh = st->dh; sa.du = st->du; sa.dv = st->dv;
-    // flux + tendency kernel now; its friction partner follows once kernel A has written u', v' of the
-    // band next to the bulk (enqueued below, after A's event)
-    swe_ca_bulk_k12<<<bulk_blocks, SWE_THREADS, 0, s>>>(sa, upf, vpf, ca_slot(it, 1));
-    if ((rc = b2_launched(c, "swe_ca_bulk_k12"))) break;
-    CA_RT(cudaEventRecord(eB, s));
-    // ---- frame stream: needs the bulk kernel of the previous step (u'', v'', h next to the frame)
-    if (it > 0) CA_RT(cudaStreamWaitEvent(s2, eS, 0));
-    if (rc) break;
+    sa.p = p;
+    sa.h = H[cur]; sa.u = U[cur]; sa.v = V[cur]; sa.du = DU[cur]; sa.dv = DV[cur];
+    sa.h_o = H[nxt]; sa.u_o = U[nxt]; sa.v_o = V[nxt]; sa.du_o = DU[nxt]; sa.dv_o = DV[nxt];
+    sa.dh = st->dh;
+    swe_ca_bulk_step<<<bulk_blocks, CA_BULK_WARPS * 32, 0, s>>>(sa, ca_slot(it, 1));
+    if ((rc = b2_launched(c, "swe_ca_bulk_step"))) break;
+    CA_RT(cudaEventRecord(eS, s));
     CACtx ctx;
     ctx.p = p; ctx.x = x;
     ctx.h = H[cur]; ctx.hn = H[nxt];
-    ctx.ua = st->u; ctx.va = st->v;
-    ctx.dh = st->dh; ctx.du = st->du; ctx.dv = st->dv;
-    ctx.dub = st->ke; ctx.dvb = st->fe2;
+    ctx.ua = U[cur]; ctx.va = V[cur];
+    ctx.dh = st->dh; ctx.du = DU[cur]; ctx.dv = DV[cur];
+    ctx.dub = ctx.dvb = nullptr; ctx.du_o = DU[nxt]; ctx.dv_o = DV[nxt];
     ctx.upf = upf; ctx.vpf = vpf;
     swe_ca_tend_frame<<<tend_blocks, CA_CELLS * CA_TEND_WARPS, 0, s2>>>(ctx, fa, ca_slot(it, 0));
     if ((rc = b2_launched(c, "swe_ca_tend_frame"))) break;
-    CA_RT(cudaEventRecord(eA, s2));
-    CA_RT(cudaStreamWaitEvent(s, eA, 0));
-    if (rc) break;
-    swe_ca_bulk_fric<<<bulk_blocks, SWE_THREADS, 0, s>>>(sa, upf, vpf, ca_slot(it, 3));
-    if ((rc = b2_launched(c, "swe_ca_bulk_fric"))) break;
-    CA_RT(cudaEventRecord(eS, s));
     if ((rc = ca_exchange(c, *topo, p, x, H[nxt], upf, vpf, s2, ca_slot(it, 2)))) break;
-    // D overwrites u, v of the frame IN PLACE: the bulk kernel, whose stencil reads them next to the
-    // frame, must be done (it is, long before, except on very large blocks -- where D then runs under the
-    // bulk friction kernel instead of under B)
-    CA_RT(cudaStreamWaitEvent(s2, eB, 0));
-    if (rc) break;
-    swe_ca_fric_frame<<<fric_blocks, CA_CELLS * 3, 0, s2>>>(ctx, fd, st->u, st->v, ca_slot(it, 4));
+    swe_ca_fric_frame<<<fric_blocks, CA_CELLS * 3, 0, s2>>>(ctx, fd, U[nxt], V[nxt], ca_slot(it, 3));
     if ((rc = b2_launched(c, "swe_ca_fric_frame"))) break;
     CA_RT(cudaEventRecord(eD, s2));
     cur = nxt;
   }
   CA_RT(cudaStreamWaitEvent(s, eD, 0));           // join (also required to end a stream capture)
-  if (rc == 0 && cur != 0)       // odd step count: h goes back to its home buffer
-    CA_RT(cudaMemcpyAsync(H[0], H[1], (size_t)p.ny * p.pitch * sizeof(float), cudaMemcpyDeviceToDevice, s));
+  // odd step count: the state goes back to its home buffers
+  const size_t bytes = (size_t)p.ny * p.pitch * sizeof(float);
+  if (cur != 0)
+    for (int k = 0; k < 5 && rc == 0; ++k) {
+      float* const pair[5][2] = {{H[0], H[1]}, {U[0], U[1]}, {V[0], V[1]}, {DU[0], DU[1]}, {DV[0], DV[1]}};
+      CA_RT(cudaMemcpyAsync(pair[k][0], pair[k][1], bytes, cudaMemcpyDeviceToDevice, s));
+    }
 #undef CA_RT
   return rc;
 }

@@ -14,9 +14,9 @@
 //   exchange X       3 layers of (h', u', v') to all eight neighbours (b2_swe_ca.cu).
 //   frame kernel D   friction (u' -> u'', v' -> v'') on the frame, and the neighbours' u'', v''
 //                    one / two cells beyond the edge, which next step's halo fluxes need.
-//   bulk kernels     flux + tendency, then friction, on everything else (b2_swe_k12_body.cuh): their
-//                    dependency cone stays inside the step's input arrays and kernel A's band, so they
-//                    need nothing from X and run concurrently with A -> X -> D.
+//   bulk kernel      flux + tendency, then friction, on everything else, one pass (b2_swe_k12_body.cuh):
+//                    its dependency cone stays inside the step's input arrays, so it needs nothing from
+//                    A, X or D and runs concurrently with A -> X -> D.
 //
 // Views.  The reference's discrete system is decomposition dependent: a rank computes its
 // fluxes from u, v whose HALO is stale by the friction update (the halo of u, v is exchanged
@@ -25,9 +25,10 @@
 // the pre-friction value u' at cells Q only sees as halo.  `ca_vu(Q, d)` implements exactly
 // that; with it (and the explicit-rounding helpers of b2_swe_body.cuh) this pipeline and the
 // stand-alone one produce the same bits on the same decomposition
-// (tests/test_swe_host_emulation.py runs both on 1x1 .. 3x2 process grids).
+// (tests/test_swe_ca_bulk_step.py runs both on 1x1 .. 2x4 process grids).
 //
-// Storage.  The main (ny, pitch) arrays keep their meaning (1-cell halo; u, v halos stale).
+// Storage.  The main (ny, pitch) arrays keep their meaning (1-cell halo; u, v halos stale).  h, u, v,
+// du and dv are ping-pong pairs: every kernel of a step reads one buffer and writes the other.
 // Five "ext" arrays [(ny + 4) x epitch], cell (j, i) at (j + 2) * epitch + (i + 2), hold what
 // lies beyond: hx (h, layers 1..2), upx / vpx (u', v': layers 1..3 and a mirror of this rank's
 // own ring cells, i.e. every STALE value a view can ask for), uppx / vppx (u'', v'' of the
@@ -49,12 +50,18 @@ struct CACtx {
   B2SweParams p;
   B2SweCA x;
   const float *h;                 // h of this step (halo fresh)
-  float *hn;                      // h' (ping-pong partner of h: the only array that needs one)
-  float *ua, *va;                 // u'', v'' of the previous step (interior; wall rows constant); kernel D
-                                  // overwrites the frame cells in place
-  float *dh, *du, *dv;            // tendencies: read (previous step) and written (this step) cell by cell
-  float *dub, *dvb;               // du, dv of the band-only cells (distance 4, 5), kernel A's private copy:
-                                  // the bulk kernel updates du, dv of those cells in place at the same time
+  float *hn;                      // h' (ping-pong partner of h)
+  const float *ua, *va;           // u'', v'' of the previous step (interior; wall rows constant); kernel D
+                                  // writes this step's into the partners
+  float *dh;                      // read (previous step) and written (this step) cell by cell
+  float *du, *dv;                 // previous step's du, dv
+  // Two layouts of this step's du, dv.  Ping-pong (dub == null; b2_swe_multistep_ca): written into the
+  // partners du_o, dv_o, because the bulk kernel reads du, dv of the band cells while kernel A runs.
+  // In place (the per-group bulk bodies of b2_swe_k12_body.cuh, which update du, dv in place): the
+  // frame cells' are written into du, dv, and the band-only cells (distance 4, 5) keep theirs in
+  // kernel A's private copy dub, dvb.
+  float *dub, *dvb;
+  float *du_o, *dv_o;
   float *upf, *vpf;               // u', v' of the frame band (cells within 5 of the edge) and, after X, their halo
 };
 
@@ -225,15 +232,18 @@ __device__ __forceinline__ void swe_ca_tend_finish(const CACtx& c, int j, int i,
   in.u_o = c.ua[off]; in.v_o = c.va[off];
   const bool frame = ca_is_frame(p, c.x.cb1, j, i);
   in.dh_o = (p.first_step || !frame) ? 0.f : c.dh[off];
-  in.du_o = p.first_step ? 0.f : (frame ? c.du[off] : c.dub[off]);
-  in.dv_o = p.first_step ? 0.f : (frame ? c.dv[off] : c.dvb[off]);
+  const bool inplace = c.dub != nullptr;
+  in.du_o = p.first_step ? 0.f : (frame || !inplace ? c.du[off] : c.dub[off]);
+  in.dv_o = p.first_step ? 0.f : (frame || !inplace ? c.dv[off] : c.dvb[off]);
   SweK2Out o = swe_k2_cell(p, in);
   if (p.north_wall && j == p.ny - 2) o.v = 0.f;       // "v" wall rule, after the update
   c.upf[off] = o.u; c.vpf[off] = o.v;
-  if (frame) {
+  if (frame) {                                        // (the band-only cells are the bulk kernel's)
     c.hn[off] = o.h;
-    c.dh[off] = o.dh; c.du[off] = o.du; c.dv[off] = o.dv;
-  } else {
+    c.dh[off] = o.dh;
+    (inplace ? c.du : c.du_o)[off] = o.du;
+    (inplace ? c.dv : c.dv_o)[off] = o.dv;
+  } else if (inplace) {
     c.dub[off] = o.du; c.dvb[off] = o.dv;
   }
 }
@@ -389,16 +399,6 @@ __device__ __forceinline__ void swe_ca_fric_task(const CACtx& c, const CAFrame& 
   if (ca_needs_vpp(c.p, j, i)) { upp[1] = ca_upp_slot(c, j, i, 1); upp[2] = ca_upp_slot(c, j, i, 2); }
   if (ext) swe_ca_fric_ext_finish(c, ua_out, va_out, j, i, upp);
   else swe_ca_fric_finish(c, ua_out, va_out, j, i, upp);
-}
-
-// the two-kernel bulk (b2_swe_k12_body.cuh): rows [4, ny-5] x whole float4 groups of columns [4, cb1)
-__host__ __device__ inline long long ca_bulk_tasks(const B2SweParams& p, int cb1) {
-  return (long long)(p.ny - 8) * ((cb1 >> 2) - 1);
-}
-__host__ __device__ inline void ca_bulk_task(const B2SweParams& p, int cb1, long long idx, int& j, int& i0) {
-  const int ng = (cb1 >> 2) - 1;
-  j = 4 + (int)(idx / ng);
-  i0 = (1 + (int)(idx % ng)) << 2;
 }
 
 // ---- exchange geometry -----------------------------------------------------------------------------

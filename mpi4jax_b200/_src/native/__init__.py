@@ -101,7 +101,7 @@ class B2SweParams(Structure):
 
 class B2SweState(Structure):
     _fields_ = [(name, c_void_p) for name in
-                ("h0", "h1", "u", "v", "dh", "du", "dv", "fe", "fn", "q", "ke", "fe2", "fn2", "u1", "v1")]
+                ("h0", "h1", "u", "v", "dh", "du", "dv", "fe", "fn", "q", "ke", "fe2", "fn2", "u1", "v1", "du1", "dv1")]
 
 
 class B2SweCA(Structure):
@@ -207,7 +207,7 @@ _SIGNATURES = {
 
 
 #: must equal B2_ABI_VERSION in csrc/b2_common.h
-ABI_VERSION = 11
+ABI_VERSION = 12
 _ABI_FIELDS = ("abi_version", "sizeof_status_record", "sizeof_halo_desc", "sizeof_swe_params",
                "sizeof_swe_state", "sizeof_error_record", "max_ranks", "p2p_nslot", "sizeof_swe_ca")
 

@@ -9,7 +9,7 @@ balanced jet (:138-169).  Two execution paths integrate it:
 ``backend="native"`` (CUDA tensors)
     Hand-written sm_90a kernels, enqueued by one native call per ``multistep`` and captured
     into a CUDA graph by :func:`mpi4jax_b200.jit`.  Default schedule: the communication-avoiding
-    step (csrc/b2_swe_ca.cu) -- two fused bulk kernels (16 array passes instead of 32) running
+    step (csrc/b2_swe_ca.cu) -- a one-pass bulk kernel (12 array passes instead of 32) running
     concurrently with a thin frame pipeline that needs ONE three-cell-deep halo exchange per
     step.  This replaces the reference's per-step sequence of XLA elementwise kernels + 48
     blocking MPI custom calls.
@@ -94,7 +94,7 @@ class ShallowWaterModel:
         # Native launch schedules (csrc/):
         #   "ca"          communication-avoiding step: ONE three-cell-deep exchange per step, the rest
         #                 recomputed on a thin frame, bulk and frame on two streams (b2_swe_ca.cu);
-        #                 16 array passes per step.  Default.
+        #                 12 array passes per step.  Default.
         #   "standalone"  4 stencil kernels + 3 fused exchanges, 32 passes (b2_swe.cu): the oracle the
         #                 default schedule is compared with, bit for bit.
         if pipeline is None:
@@ -166,7 +166,8 @@ class ShallowWaterModel:
         self.dh, self.du, self.dv = z(), z(), z()
         self._h1 = z()
         self._u1 = z()      # ping-pong partner of u for the friction update
-        self._v1 = z()      # ping-pong partner of v (fused flux+tendency path only)
+        self._v1 = z()      # ping-pong partner of v
+        self._du1, self._dv1 = z(), z()      # ping-pong partners of du, dv (communication-avoiding step)
         self.fe, self.fn, self.q, self.ke, self.fe2, self.fn2 = z(), z(), z(), z(), z(), z()
         y_global = (np.arange(-1, self.ny_global - 1) * self.cfg.dy)
         cor = self.cfg.coriolis_f + y_global[self.local_slice[0]] * self.cfg.coriolis_beta
@@ -193,6 +194,7 @@ class ShallowWaterModel:
             st.h0, st.h1 = self.h.data_ptr(), self._h1.data_ptr()
             st.u1 = self._u1.data_ptr()
             st.v1 = self._v1.data_ptr()
+            st.du1, st.dv1 = self._du1.data_ptr(), self._dv1.data_ptr()
             for name in ("u", "v", "dh", "du", "dv", "fe", "fn", "q", "ke", "fe2", "fn2"):
                 setattr(st, name, getattr(self, name).data_ptr())
             t = self._topo = native.B2HaloDesc()
@@ -256,6 +258,8 @@ class ShallowWaterModel:
         self._h1.copy_(self.h)
         self._u1.copy_(self.u)
         self._v1.copy_(self.v)
+        self._du1.copy_(self.du)
+        self._dv1.copy_(self.dv)
         if self.backend == "native" and self.pipeline == "ca":
             nc = self.comm._native_comm()
             rc = native.lib.b2_swe_ca_init(

@@ -11,7 +11,7 @@ OUT = os.path.join(REPO, "profiles", "sass")
 WANT = {       # substring of the mangled name (with its length prefix where names share a stem) -> file
     "9b2_k_halo9": "halo", "12b2_k_halo_ll": "halo_ll", "12b2_k_halo_ca": "halo_ca_deep_exchange",
     "swe_k1_fluxes": "swe_k1_fluxes", "swe_k2_tendencies": "swe_k2_tendencies", "swe_k34": "swe_k34_friction_u",
-    "swe_k5": "swe_k5_friction_v", "swe_ca_bulk_k12": "swe_ca_bulk_k12", "swe_ca_bulk_fric": "swe_ca_bulk_fric",
+    "swe_k5": "swe_k5_friction_v", "swe_ca_bulk_step": "swe_ca_bulk_step",
     "swe_ca_tend_frame": "swe_ca_tend_frame", "swe_ca_fric_frame": "swe_ca_fric_frame",
     "b2_k_barrier": "barrier", "9b2_k_move": "move", "b2_k_bcast_mc": "bcast_multicast",
     "b2_k_reduce_root_nvlsILi0": "reduce_root_nvls_f32", "b2_k_allreduce_symILi0": "allreduce_symmetric_inplace_f32",

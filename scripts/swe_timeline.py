@@ -21,7 +21,7 @@ steps = int(sys.argv[2]) if len(sys.argv) > 2 else 8
 comm = MPI.COMM_WORLD
 model = ShallowWaterModel(ShallowWaterConfig.for_resolution(grid, grid), comm=comm, device=comm.device)
 model.step(first_step=True)
-buf = torch.zeros((steps, 5, 2), dtype=torch.int64, device=comm.device)
+buf = torch.zeros((steps, 4, 2), dtype=torch.int64, device=comm.device)
 native.lib.b2_swe_ca_timeline(buf.data_ptr(), steps)
 run = m.jit(lambda: model.multistep(steps, first_step=False), warmup=0)
 run()                                   # capture + one replay
@@ -36,14 +36,14 @@ run()
 torch.cuda.synchronize()
 native.lib.b2_swe_ca_timeline(None, 0)
 t = buf.cpu().double()
-names = ["A", "B", "X", "Fb", "D"]
+names = ["A", "S", "X", "D"]
 if comm.Get_rank() in (0, comm.Get_size() - 1):
     print(f"rank {comm.Get_rank()} of {comm.Get_size()}: local block {model.ny_local}x{model.nx_local}", flush=True)
     t0 = t[0, :, 0].min()
     prev_end = None
     for s in range(steps):
         base = t[s, :, 0].min()
-        row = "  ".join(f"{names[k]} {(t[s, k, 0] - base) / 1e3:6.1f}-{(t[s, k, 1] - base) / 1e3:6.1f}" for k in range(5))
+        row = "  ".join(f"{names[k]} {(t[s, k, 0] - base) / 1e3:6.1f}-{(t[s, k, 1] - base) / 1e3:6.1f}" for k in range(4))
         end = t[s, :, 1].max()
         print(f"step {s}: start +{(base - t0) / 1e3:7.1f} us | {row} | step {(end - base) / 1e3:6.1f} us", flush=True)
     total = (t[:, :, 1].max() - t0) / 1e3
