@@ -19,7 +19,7 @@
 #include "b2_halo_ll.cuh"
 #include "b2_runtime.h"
 #include "b2_swe_ca_body.cuh"
-#include "b2_swe_k12_body.cuh"
+#include "b2_swe_ca_bulk.cuh"
 
 #define CA_THREADS 256
 
@@ -122,7 +122,7 @@ __global__ void __launch_bounds__(CA_THREADS) swe_ca_init_ext(const B2SweParams 
   }
 }
 
-// ---- S: the bulk, one pass per step (b2_swe_k12_body.cuh) ---------------------------------------
+// ---- S: the bulk, one pass per step (b2_swe_ca_bulk.cuh) ----------------------------------------
 __global__ void __launch_bounds__(CA_BULK_WARPS * 32)
 swe_ca_bulk_step(const CABulkArgs a, const CAStamp ts) {
   ca_stamp_begin(ts);
@@ -373,7 +373,7 @@ int b2_swe_multistep_ca(B2Comm* c, const B2SweParams* p0, const B2SweState* st, 
     ctx.h = H[cur]; ctx.hn = H[nxt];
     ctx.ua = U[cur]; ctx.va = V[cur];
     ctx.dh = st->dh; ctx.du = DU[cur]; ctx.dv = DV[cur];
-    ctx.dub = ctx.dvb = nullptr; ctx.du_o = DU[nxt]; ctx.dv_o = DV[nxt];
+    ctx.du_o = DU[nxt]; ctx.dv_o = DV[nxt];
     ctx.upf = upf; ctx.vpf = vpf;
     swe_ca_tend_frame<<<tend_blocks, CA_CELLS * CA_TEND_WARPS, 0, s2>>>(ctx, fa, ca_slot(it, 0));
     if ((rc = b2_launched(c, "swe_ca_tend_frame"))) break;

@@ -14,7 +14,7 @@
 //   exchange X       3 layers of (h', u', v') to all eight neighbours (b2_swe_ca.cu).
 //   frame kernel D   friction (u' -> u'', v' -> v'') on the frame, and the neighbours' u'', v''
 //                    one / two cells beyond the edge, which next step's halo fluxes need.
-//   bulk kernel      flux + tendency, then friction, on everything else, one pass (b2_swe_k12_body.cuh):
+//   bulk kernel      flux + tendency, then friction, on everything else, one pass (b2_swe_ca_bulk.cuh):
 //                    its dependency cone stays inside the step's input arrays, so it needs nothing from
 //                    A, X or D and runs concurrently with A -> X -> D.
 //
@@ -25,7 +25,7 @@
 // the pre-friction value u' at cells Q only sees as halo.  `ca_vu(Q, d)` implements exactly
 // that; with it (and the explicit-rounding helpers of b2_swe_body.cuh) this pipeline and the
 // stand-alone one produce the same bits on the same decomposition
-// (tests/test_swe_ca_bulk_step.py runs both on 1x1 .. 2x4 process grids).
+// (tests/test_swe_host_emulation.py runs both on 1x1 .. 2x4 process grids).
 //
 // Storage.  The main (ny, pitch) arrays keep their meaning (1-cell halo; u, v halos stale).  h, u, v,
 // du and dv are ping-pong pairs: every kernel of a step reads one buffer and writes the other.
@@ -54,14 +54,8 @@ struct CACtx {
   const float *ua, *va;           // u'', v'' of the previous step (interior; wall rows constant); kernel D
                                   // writes this step's into the partners
   float *dh;                      // read (previous step) and written (this step) cell by cell
-  float *du, *dv;                 // previous step's du, dv
-  // Two layouts of this step's du, dv.  Ping-pong (dub == null; b2_swe_multistep_ca): written into the
-  // partners du_o, dv_o, because the bulk kernel reads du, dv of the band cells while kernel A runs.
-  // In place (the per-group bulk bodies of b2_swe_k12_body.cuh, which update du, dv in place): the
-  // frame cells' are written into du, dv, and the band-only cells (distance 4, 5) keep theirs in
-  // kernel A's private copy dub, dvb.
-  float *dub, *dvb;
-  float *du_o, *dv_o;
+  const float *du, *dv;           // du, dv of this step (the previous step's tendencies)
+  float *du_o, *dv_o;             // their ping-pong partners: the bulk kernel reads du, dv while kernel A runs
   float *upf, *vpf;               // u', v' of the frame band (cells within 5 of the edge) and, after X, their halo
 };
 
@@ -231,20 +225,18 @@ __device__ __forceinline__ void swe_ca_tend_finish(const CACtx& c, int j, int i,
   in.h_c = c.h[off]; in.h_e = ca_h(c, j, i + 1); in.h_n = ca_h(c, j + 1, i);
   in.u_o = c.ua[off]; in.v_o = c.va[off];
   const bool frame = ca_is_frame(p, c.x.cb1, j, i);
+  // not read for a band-only cell: the bulk kernel updates that cell's dh in place meanwhile
   in.dh_o = (p.first_step || !frame) ? 0.f : c.dh[off];
-  const bool inplace = c.dub != nullptr;
-  in.du_o = p.first_step ? 0.f : (frame || !inplace ? c.du[off] : c.dub[off]);
-  in.dv_o = p.first_step ? 0.f : (frame || !inplace ? c.dv[off] : c.dvb[off]);
+  in.du_o = p.first_step ? 0.f : c.du[off];
+  in.dv_o = p.first_step ? 0.f : c.dv[off];
   SweK2Out o = swe_k2_cell(p, in);
   if (p.north_wall && j == p.ny - 2) o.v = 0.f;       // "v" wall rule, after the update
   c.upf[off] = o.u; c.vpf[off] = o.v;
   if (frame) {                                        // (the band-only cells are the bulk kernel's)
     c.hn[off] = o.h;
     c.dh[off] = o.dh;
-    (inplace ? c.du : c.du_o)[off] = o.du;
-    (inplace ? c.dv : c.dv_o)[off] = o.dv;
-  } else if (inplace) {
-    c.dub[off] = o.du; c.dvb[off] = o.dv;
+    c.du_o[off] = o.du;
+    c.dv_o[off] = o.dv;
   }
 }
 __device__ __forceinline__ void swe_ca_tend_cell(const CACtx& c, int j, int i) {
@@ -324,7 +316,7 @@ __device__ __forceinline__ void swe_ca_fric_ext_finish(const CACtx& c, float* __
   }
 }
 // ---- task enumeration ----------------------------------------------------------------------------
-// Bulk (b2_swe_k12_body.cuh) = rows [4, ny-5] x columns [4, cb1); frame = every other interior cell.
+// Bulk (b2_swe_ca_bulk.cuh) = rows [4, ny-5] x columns [4, cb1); frame = every other interior cell.
 // A band of width w: rows [1, w] and [ny-1-w, ny-2] completely, of the rows in between the columns
 // [1, w] and [ce, nx-2].  Kernel D walks the frame (w = 3, ce = cb1), kernel A the frame plus the two
 // cells beyond it (w = 5, ce = cb1 - 2).

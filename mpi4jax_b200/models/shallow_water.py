@@ -77,6 +77,17 @@ class ShallowWaterConfig:
         return 0.125 * min(self.dx, self.dy) / math.sqrt(self.gravity * self.depth)
 
 
+def fold_constants(p: native.B2SweParams) -> native.B2SweParams:
+    """Fill the constant factors of the kernel parameters ``p`` from its dt, gravity, viscosity,
+    rdx and rdy, folded once in fp32 (csrc/b2_swe_body.cuh); returns ``p``."""
+    f32 = np.float32
+    rdx, rdy, nu, dt, g = f32(p.rdx), f32(p.rdy), f32(p.viscosity), f32(p.dt), f32(p.gravity)
+    p.c_gx, p.c_gy = float(-g * rdx), float(-g * rdy)
+    p.c_nux, p.c_nuy = float(nu * rdx), float(nu * rdy)
+    p.c_fx, p.c_fy = float(dt * nu * rdx * rdx), float(dt * nu * rdy * rdy)
+    return p
+
+
 class ShallowWaterModel:
     def __init__(self, config: Optional[ShallowWaterConfig] = None, comm: Optional[Comm] = None,
                  device: Optional[torch.device] = None, backend: str = "auto",
@@ -181,12 +192,7 @@ class ShallowWaterModel:
             p.rdx = float(np.float32(1.0) / np.float32(self.cfg.dx))
             p.rdy = float(np.float32(1.0) / np.float32(self.cfg.dy))
             p.ab_a, p.ab_b = self.cfg.ab_a, self.cfg.ab_b
-            # constant factors folded once, in fp32 (csrc/b2_swe_body.cuh)
-            f32 = np.float32
-            rdx, rdy, nu, dt = f32(p.rdx), f32(p.rdy), f32(p.viscosity), f32(p.dt)
-            p.c_gx, p.c_gy = float(-f32(p.gravity) * rdx), float(-f32(p.gravity) * rdy)
-            p.c_nux, p.c_nuy = float(nu * rdx), float(nu * rdy)
-            p.c_fx, p.c_fy = float(dt * nu * rdx * rdx), float(dt * nu * rdy * rdy)
+            fold_constants(p)
             p.first_step = 0
             p.south_wall, p.north_wall = int(self.at_south_wall), int(self.at_north_wall)
             p.coriolis = self.coriolis.data_ptr()

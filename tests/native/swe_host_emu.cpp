@@ -1,9 +1,11 @@
-// Host emulation of the shallow-water stencil bodies (csrc/b2_swe_body.cuh, b2_swe_k12_body.cuh,
+// Host emulation of the shallow-water stencil bodies (csrc/b2_swe_body.cuh, b2_swe_ca_bulk.cuh,
 // b2_swe_ca_body.cuh): the same source, compiled by g++ with the CUDA qualifiers defined away, driven
 // by plain loops instead of a grid.  Lets the CPU test-suite check the INDEXING of kernels it cannot
-// launch -- in particular the communication-avoiding step (frame kernels with owner views, deep halo
-// exchange geometry, bulk / frame partition) against the stand-alone K1 -> K2 -> K34 -> K5 pipeline,
-// bit for bit (every rounding in the bodies is explicit, so host and device agree on the arithmetic).
+// launch -- in particular the communication-avoiding step as b2_swe_multistep_ca launches it (one-pass
+// bulk kernel with its 32 lanes in lockstep, frame kernels with owner views, deep halo exchange
+// geometry, bulk / frame partition, ping-pong storage) against the stand-alone K1 -> K2 -> K34 -> K5
+// pipeline, bit for bit (every rounding in the bodies is explicit, so host and device agree on the
+// arithmetic).
 // Build: g++ -O1 -ffp-contract=off -shared -fPIC -I csrc -I $CUDA/include tests/native/swe_host_emu.cpp
 #include <cmath>
 #include <cstring>
@@ -19,18 +21,23 @@ struct FakeIdx { unsigned x; };
 static FakeIdx blockIdx, threadIdx;
 
 #include "b2_swe_ca_body.cuh"
-#include "b2_swe_k12_body.cuh"
+#include "b2_swe_ca_bulk.cuh"
 
 static void masks(const B2SweParams& p, int i0, bool m[4]) {
   for (int k = 0; k < 4; ++k) m[k] = (i0 + k >= 1) && (i0 + k <= p.nx - 2);
 }
 
-struct EmuStep {      // the arrays of one rank for one step (B2SweState roles of b2_swe_multistep_ca)
-  const float *h;
-  float *h_o, *u, *v, *dh, *du, *dv, *dub, *dvb, *upf, *vpf;
+struct EmuStep {      // one rank's arrays for one step, B2SweState roles of b2_swe_multistep_ca
+  const float *h, *u, *v, *du, *dv;            // this step
+  float *h_o, *u_o, *v_o, *du_o, *dv_o;        // the next step (ping-pong partners)
+  float *dh, *upf, *vpf;
 };
 
 extern "C" {
+
+// the ABI structs as this compiler lays them out
+int emu_sizeof_swe_params() { return (int)sizeof(B2SweParams); }
+int emu_sizeof_swe_ca() { return (int)sizeof(B2SweCA); }
 
 // K1 on every interior row / group (what swe_k1_fluxes does)
 void emu_k1_all(const B2SweParams* p, const float* h, const float* u, const float* v, float* fe, float* fn,
@@ -78,21 +85,28 @@ void emu_k34(const B2SweParams* p, const float* u, float* u_new, const float* v,
     }
 }
 
-// ---- communication-avoiding step (csrc/b2_swe_ca_body.cuh, b2_swe_k12_body.cuh): the kernels of
+// ---- communication-avoiding step (csrc/b2_swe_ca_body.cuh, b2_swe_ca_bulk.cuh): the kernels of
 // b2_swe_ca.cu as loops.  `reverse` walks the tasks backwards: a kernel whose threads only read what no
 // thread of the same launch (or phase) writes gives the same bits in any order.
 static CACtx make_ctx(const B2SweParams* p, const B2SweCA* x, const EmuStep* e) {
   CACtx c;
   c.p = *p; c.x = *x; c.x.cb1 = swe_ca_cb1(*p);
-  c.h = e->h; c.hn = e->h_o; c.ua = e->u; c.va = e->v; c.dh = e->dh; c.du = e->du; c.dv = e->dv;
-  c.dub = e->dub; c.dvb = e->dvb;
+  c.h = e->h; c.hn = e->h_o; c.ua = e->u; c.va = e->v; c.dh = e->dh;
+  c.du = e->du; c.dv = e->dv; c.du_o = e->du_o; c.dv_o = e->dv_o;
   c.upf = e->upf; c.vpf = e->vpf;
   return c;
 }
 
-int emu_ca_supported(const B2SweParams* p) { return swe_ca_supported(*p) ? 1 : 0; }
-int emu_ca_cb1(const B2SweParams* p) { return swe_ca_cb1(*p); }
+static CABulkArgs bulk_args(const B2SweParams* p, int rows) {
+  CABulkArgs a;
+  a.p = *p;
+  ca_bulk_geometry(*p, swe_ca_cb1(*p), rows, a);
+  return a;
+}
 
+int emu_ca_supported(const B2SweParams* p) { return swe_ca_supported(*p) ? 1 : 0; }
+
+// kernel A / kernel D
 void emu_ca_tend_frame(const B2SweParams* p, const B2SweCA* x, const EmuStep* e, int reverse) {
   const CACtx c = make_ctx(p, x, e);
   const CAFrame f = ca_frame(c.p, 5, c.x.cb1 - 2);
@@ -101,37 +115,48 @@ void emu_ca_tend_frame(const B2SweParams* p, const B2SweCA* x, const EmuStep* e,
     if (ca_frame_cell(c.p, f, (int)(reverse ? f.total - 1 - k : k), j, i)) swe_ca_tend_cell(c, j, i);
   }
 }
-
 void emu_ca_fric_frame(const B2SweParams* p, const B2SweCA* x, const EmuStep* e, int reverse) {
   const CACtx c = make_ctx(p, x, e);
   const CAFrame f = ca_frame(c.p, 3, c.x.cb1);
   const long long n = f.total + ca_ext_total(c.p);
-  for (long long k = 0; k < n; ++k) swe_ca_fric_task(c, f, e->u, e->v, reverse ? n - 1 - k : k);
+  for (long long k = 0; k < n; ++k) swe_ca_fric_task(c, f, e->u_o, e->v_o, reverse ? n - 1 - k : k);
 }
 
-// swe_ca_bulk_step: CTAs one after the other, every phase as a loop over the CTA's threads
-// (`reverse`: CTAs and threads backwards -- a phase only reads what earlier phases wrote)
-// swe_ca_bulk_k12 + swe_ca_bulk_fric (the friction kernel runs after kernel A: it reads the band's u', v')
-void emu_ca_bulk_k12(const B2SweParams* p, const EmuStep* e) {
-  const int cb1 = swe_ca_cb1(*p);
-  for (long long t = 0; t < ca_bulk_tasks(*p, cb1); ++t) {
-    int j, i0;
-    ca_bulk_task(*p, cb1, t, j, i0);
-    swe_k12_body(*p, e->h, e->h_o, e->u, e->upf, e->v, e->vpf, e->dh, e->du, e->dv, e->dh, e->du, e->dv, j, i0);
-  }
-}
-void emu_ca_bulk_fric(const B2SweParams* p, const EmuStep* e) {
-  const int cb1 = swe_ca_cb1(*p);
-  for (long long t = 0; t < ca_bulk_tasks(*p, cb1); ++t) {
-    int j, i0;
-    ca_bulk_task(*p, cb1, t, j, i0);
-    swe_k345_body(*p, e->upf, e->u, e->vpf, e->v, j, i0);
+// swe_ca_bulk_step with `rows` rows per segment: warps one after the other (`reverse`: backwards), the
+// 32 lanes of a warp in lockstep, every phase of a row as a loop over the lanes; the lane exchange is
+// __shfl_up_sync / __shfl_down_sync by one lane (a lane without a partner gets its own value)
+void emu_ca_bulk_step(const B2SweParams* p, const EmuStep* e, int rows, int reverse) {
+  CABulkArgs a = bulk_args(p, rows);
+  a.h = e->h; a.u = e->u; a.v = e->v; a.du = e->du; a.dv = e->dv;
+  a.h_o = e->h_o; a.u_o = e->u_o; a.v_o = e->v_o; a.du_o = e->du_o; a.dv_o = e->dv_o;
+  a.dh = e->dh;
+  const long long nw = ca_bulk_warps(a);
+  static CABulkLane L[32];
+  for (long long k = 0; k < nw; ++k) {
+    const int w = (int)(reverse ? nw - 1 - k : k);
+    int s, en;
+    ca_bulk_rows(a, w / a.wcols, s, en);
+    for (int l = 0; l < 32; ++l) {
+      L[l].store = ca_bulk_lane(a, w % a.wcols, l, L[l].i0);
+      ca_bulk_begin(a, L[l], s);
+    }
+    for (int t = s - 2; t <= en; ++t) {
+      float uw2[32], uw3[32], ue[32], ve[32];
+      for (int l = 0; l < 32; ++l) ca_bulk_tend(a, L[l], t, t >= s && t < en);
+      for (int l = 0; l < 32; ++l) {
+        const int lw = l > 0 ? l - 1 : l, le = l < 31 ? l + 1 : l;
+        uw2[l] = L[lw].upn[2]; uw3[l] = L[lw].upn[3];
+        ue[l] = L[le].upn[0]; ve[l] = L[le].vpn[0];
+      }
+      for (int l = 0; l < 32; ++l) ca_bulk_fric(a, L[l], t, uw2[l], uw3[l], ue[l], ve[l], t == s, t > s);
+    }
   }
 }
 
-// which interior cells do the bulk kernel and the frame kernels WRITE?  marks[j * nx + i]: +1 frame
-// (kernel D's cells = kernel A's full updates), +16 bulk, +256 kernel A's u' / v' band
-void emu_ca_marks(const B2SweParams* p, int* marks) {
+// which interior cells do the bulk kernel (`rows` rows per segment) and the frame kernels WRITE?
+// marks[j * nx + i]: +1 frame (kernel D's cells = kernel A's full updates), +16 bulk (per store),
+// +256 kernel A's u' / v' band
+void emu_ca_marks(const B2SweParams* p, int rows, int* marks) {
   const int cb1 = swe_ca_cb1(*p);
   const CAFrame fd = ca_frame(*p, 3, cb1), fa = ca_frame(*p, 5, cb1 - 2);
   int j, i;
@@ -139,10 +164,16 @@ void emu_ca_marks(const B2SweParams* p, int* marks) {
     if (ca_frame_cell(*p, fd, (int)t, j, i)) marks[j * p->nx + i] += 1;
   for (long long t = 0; t < fa.total; ++t)
     if (ca_frame_cell(*p, fa, (int)t, j, i)) marks[j * p->nx + i] += 256;
-  for (long long t = 0; t < ca_bulk_tasks(*p, cb1); ++t) {
-    int i0;
-    ca_bulk_task(*p, cb1, t, j, i0);
-    for (int k = 0; k < 4; ++k) marks[j * p->nx + i0 + k] += 16;
+  const CABulkArgs a = bulk_args(p, rows);
+  for (long long w = 0; w < ca_bulk_warps(a); ++w) {
+    int s, e;
+    ca_bulk_rows(a, (int)(w / a.wcols), s, e);
+    for (int l = 0; l < 32; ++l) {
+      int i0;
+      if (!ca_bulk_lane(a, (int)(w % a.wcols), l, i0)) continue;
+      for (j = s; j < e; ++j)
+        for (int k = 0; k < 4; ++k) marks[j * p->nx + i0 + k] += 16;
+    }
   }
 }
 
