@@ -3,13 +3,14 @@
 * allreduce 1 KB - 1 GB, fp32 + bf16, every transport (ll / oneshot / twoshot / nvls / auto)
   next to NCCL on the same box                                   (configs 2)
 * allgather and alltoall 1 KB - 1 GB per-rank payload vs NCCL     (config 4)
+* reduce_scatter (P, n) fp32 + bf16, 1 KB - 1 GB per-rank input, vs NCCL and vs allreduce
 * bcast, reduce, gather, scatter (root = last rank) vs NCCL, scan (no NCCL counterpart)
 * sendrecv ring, halo exchange latency
 
 Timing: ``reps`` back-to-back ops captured in ONE CUDA graph, one replay timed with CUDA
 events on the launching stream (barrier + synchronize before), max over ranks -- i.e. the
 kernels' time, not the Python launch path.  Bus bandwidth uses the NCCL-tests conventions:
-allreduce S/t*2(P-1)/P, allgather/alltoall (P-1)/P * total/t.
+allreduce S/t*2(P-1)/P, allgather/alltoall/reduce_scatter (P-1)/P * total/t.
 
     python -m mpi4jax_b200.run -n 8 bench/collectives_sweep.py [--max-bytes 1073741824] [--out f.json]
 """
@@ -202,6 +203,35 @@ for nbytes in sizes:
     if rank == 0:
         print("allgather/alltoall", nbytes, row, result["alltoall"].get(str(nbytes)), flush=True)
     del x
+
+# ---------------------------------------------------------------- reduce_scatter (per-rank input |x| = nbytes)
+# next to NCCL's reduce_scatter_tensor and to allreduce(x)[rank], what a user without it would call
+result["reduce_scatter"] = {}
+for dtype, dname in ((torch.float32, "fp32"), (torch.bfloat16, "bf16")):
+    table = {}
+    esize = torch.empty((), dtype=dtype).element_size()
+    for nbytes in sizes:
+        if nbytes < size * 16:
+            continue
+        x = torch.ones(size, nbytes // esize // size, dtype=dtype, device=dev)
+        tot = x.numel() * esize
+        reps = reps_for(nbytes)
+        bw = lambda us: round(tot * (size - 1) / size / us / 1e3, 1)
+        row = {}
+        us = time_graph(lambda: m.reduce_scatter(x, MPI.SUM, comm=comm), reps)
+        row["ours"] = {"us": round(us, 2), "busbw": bw(us)}
+        us = time_graph(lambda: m.allreduce(x, MPI.SUM, comm=comm), reps)
+        row["allreduce"] = {"us": round(us, 2), "busbw": bw(us)}
+        if nccl is not None:
+            out = torch.empty(x.shape[1:], dtype=dtype, device=dev)
+            us = time_nccl(lambda: dist.reduce_scatter_tensor(out, x, group=nccl), reps)
+            row["nccl"] = {"us": round(us, 2), "busbw": bw(us)}
+            del out
+        table[str(nbytes)] = row
+        if rank == 0:
+            print("reduce_scatter", dname, nbytes, {k: (v["us"], v["busbw"]) for k, v in row.items()}, flush=True)
+        del x
+    result["reduce_scatter"][dname] = table
 
 # ---------------------------------------------------------------- rooted ops + scan (per-rank payload = nbytes)
 result.update({"bcast": {}, "reduce": {}, "gather": {}, "scatter": {}, "scan": {}})

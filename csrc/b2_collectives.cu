@@ -10,8 +10,8 @@
 // (mpi_ops_common.h:222-306; mpi_xla_bridge_cuda.cpp:99-148, 227-503) is fused
 // into the NVLink pull; there is no host sync and no host staging.
 //
-// Reduction collectives live in b2_reduce.cuh; this file adds the kernels that go through the
-// NVSwitch multicast object -- the NVLS allreduce of staged data (b2_k_allreduce_nvls), the
+// Reduction collectives (allreduce, reduce, scan, reduce-scatter) live in b2_reduce.cuh; this file
+// adds their entry points and the kernels that go through the NVSwitch multicast object -- the NVLS allreduce of staged data (b2_k_allreduce_nvls), the
 // in-place allreduce of symmetric tensors (b2_k_allreduce_sym), the multicast bcast
 // (b2_k_bcast_mc), the reduce-to-root (b2_k_reduce_root_nvls) --, the size-based algorithm
 // selection and the grid cap that keeps every launch co-resident (coresident_blocks).
@@ -599,6 +599,7 @@ extern "C" size_t b2_stage_need(int opcode, int nranks, size_t blk_bytes) {
   switch (opcode) {
     case B2_OPC_ALLTOALL:
     case B2_OPC_SCATTER:
+    case B2_OPC_REDUCE_SCATTER:
       return stride * (size_t)nranks + 4096;
     default:
       return stride + 4096;
@@ -655,22 +656,28 @@ static int reduce_common(B2Comm* c, const void* in, void* out, size_t count, int
   const size_t nbytes = count * b2_dtype_size(dtype);
   if (nbytes == 0) return 0;
   const int P = c->dev.size;
+  // reduce-scatter: `count` and `nbytes` are per block; a block travels to each peer like a whole
+  // allreduce payload (LL) or is pulled from every peer's staging (the one-shot branch of the kernel)
+  const bool rs = opcode == B2_OPC_REDUCE_SCATTER;
+  const bool ll_fits = P > 1 && nbytes <= c->ll_max && nbytes * 2 <= c->dev.lay.ll_cap;
   if (algo == B2_ALGO_AUTO) {
-    if (opcode != B2_OPC_ALLREDUCE) algo = B2_ALGO_ONESHOT;
-    else if (P > 1 && nbytes <= c->ll_max && nbytes * 2 <= c->dev.lay.ll_cap) algo = B2_ALGO_LL;
+    if (rs) algo = ll_fits ? B2_ALGO_LL : B2_ALGO_ONESHOT;
+    else if (opcode != B2_OPC_ALLREDUCE) algo = B2_ALGO_ONESHOT;
+    else if (ll_fits) algo = B2_ALGO_LL;
     else if (P <= 2) algo = B2_ALGO_ONESHOT;
     else if (nvls_capable(c, dtype, op) && nbytes >= c->nvls_min) algo = B2_ALGO_NVLS;
     else if (nbytes <= c->oneshot_max) algo = B2_ALGO_ONESHOT;
     else algo = B2_ALGO_TWOSHOT;
   }
   if (algo == B2_ALGO_LL) {
-    if (opcode != B2_OPC_ALLREDUCE || nbytes * 2 > c->dev.lay.ll_cap) {
+    if ((opcode != B2_OPC_ALLREDUCE && !rs) || nbytes * 2 > c->dev.lay.ll_cap) {
       b2_set_error("%s: LL algorithm needs an allreduce of <= %zu bytes", name,
                    c->dev.lay.ll_cap / 2);
       return B2_ERR_BAD_ARG;
     }
     B2LLArgs a;
     a.in = in; a.out = out; a.nbytes = nbytes; a.opcode = opcode;
+    a.src_stride = rs ? nbytes : 0;
     const size_t nv = (nbytes + 15) / 16;
     int grid = (int)((nv + B2_THREADS - 1) / B2_THREADS);
     if (grid > c->sm_count) grid = c->sm_count;
@@ -767,6 +774,17 @@ extern "C" int b2_scan(B2Comm* c, const void* in, void* out, size_t count, int d
   const size_t nbytes = count * b2_dtype_size(dtype);
   const int algo = (c->dev.size > 2 && nbytes > c->oneshot_max) ? B2_ALGO_TWOSHOT : B2_ALGO_ONESHOT;
   int rc = reduce_common(c, in, out, count, dtype, op, algo, 0, c->dev.rank + 1, 1, B2_OPC_SCAN, "scan", stream);
+  b2_debug_end(dbg, rc);
+  return rc;
+}
+
+// MPI_Reduce_scatter_block: `in` holds P blocks of `count` elements, rank r receives the reduction of
+// block r over all ranks, folded in rank order.  P == 1 copies the one block.
+extern "C" int b2_reduce_scatter(B2Comm* c, const void* in, void* out, size_t count, int dtype, int op,
+                                 cudaStream_t stream) {
+  B2DebugScope* dbg = b2_debug_begin(c, "Reduce_scatter_block", stream, "with %zu items per block", count);
+  int rc = reduce_common(c, in, out, count, dtype, op, B2_ALGO_AUTO, 0, c->dev.size, 1, B2_OPC_REDUCE_SCATTER,
+                         "reduce_scatter", stream);
   b2_debug_end(dbg, rc);
   return rc;
 }

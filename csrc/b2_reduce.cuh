@@ -1,4 +1,4 @@
-// mpi4jax_b200 -- reduction collectives over peer-mapped HBM (allreduce, reduce, scan).
+// mpi4jax_b200 -- reduction collectives over peer-mapped HBM (allreduce, reduce, scan, reduce-scatter).
 //
 // Replaces the reference's MPI_Allreduce / MPI_Reduce / MPI_Scan call sites
 // (mpi4jax/_src/xla_bridge/mpi_ops_common.h:236-249, 310-338 and their CUDA
@@ -52,6 +52,27 @@ b2_k_reduce_chunked(const B2DevComm c, const B2ReduceArgs a) {
     const size_t off = ch * a.chunk;
     const size_t len = (a.nbytes - off < a.chunk) ? (a.nbytes - off) : a.chunk;
     const size_t nv = (len + 15) >> 4;        // vectors incl. a padded tail vector
+    if (a.opcode == B2_OPC_REDUCE_SCATTER) {
+      // reduce-scatter: nbytes is ONE block and chunks index into it.  Stage this chunk of all P
+      // input blocks (block q at q * bs), then pull block `rank` from every peer and reduce it in
+      // rank order.  One barrier: the staging parity alternates per launch as for one-shot.
+      const size_t bs = (a.nbytes + 15) & ~(size_t)15;
+      for (int q = 0; q < c.size; ++q)
+        b2_copy_bytes<false>(mine + (size_t)q * bs + off, in + (size_t)q * a.nbytes + off, len);
+      b2_barrier_all(c, ++e, a.opcode);
+      const size_t src = (size_t)c.rank * bs + off;
+      for (size_t i = t; i < nv; i += nt) {
+        B2Vec<T> acc;
+        acc.load(b2_ld_peer16(c.stage[0] + par + src + (i << 4)));
+        for (int q = 1; q < c.size; ++q)
+          acc.template accumulate<OP>(b2_ld_peer16(c.stage[q] + par + src + (i << 4)));
+        const uint4 r = acc.store();
+        const size_t b = i << 4;
+        if (b + 16 <= len) b2_st16(out + off + b, r);
+        else b2_store_partial(out + off + b, r, (int)(len - b));
+      }
+      continue;
+    }
     // 1. stage my contribution (local HBM -> local symmetric staging)
     b2_copy_bytes<false>(mine + off, in + off, len);
     // 2. everybody's copy of this chunk is staged
@@ -126,13 +147,26 @@ b2_k_reduce_chunked(const B2DevComm c, const B2ReduceArgs a) {
 // ticket parity so a sender can never overwrite data that is still being read:
 // to be two tickets ahead it needs this rank's contribution to the ticket in
 // between, which this rank only sends after it finished reading).
+//
+// Reduce-scatter uses the same kernel with `src_stride` = the block size: peer p receives block p
+// (in + p * src_stride) and this rank folds its own block (in + rank * src_stride) with the P - 1 it
+// received.  Allreduce passes 0: every peer receives the whole input.
 // ---------------------------------------------------------------------------
 struct B2LLArgs {
   const void* in;
   void* out;
-  size_t nbytes;
+  size_t nbytes;       // payload bytes per destination (allreduce: all of it; reduce-scatter: one block)
+  size_t src_stride;   // bytes between the inputs of consecutive destinations (0: one input for all)
   int opcode;
 };
+
+// vector i of a payload of nbytes bytes, zero padded past the end
+__device__ __forceinline__ uint4 b2_ll_load(const char* in, size_t b, size_t nbytes, bool aligned) {
+  if (aligned && b + 16 <= nbytes) return *reinterpret_cast<const uint4*>(in + b);
+  alignas(16) unsigned char tmp[16];
+  for (int k = 0; k < 16; ++k) tmp[k] = (b + k < nbytes) ? ((const unsigned char*)in)[b + k] : 0;
+  return *reinterpret_cast<const uint4*>(tmp);
+}
 
 template <typename T, int OP>
 __global__ void __launch_bounds__(B2_THREADS)
@@ -143,27 +177,20 @@ b2_k_allreduce_ll(const B2DevComm c, const B2LLArgs a) {
   const size_t nv = (a.nbytes + 15) >> 4;
   const char* in = (const char*)a.in;
   char* out = (char*)a.out;
-  const bool aligned = (((uintptr_t)in) & 15) == 0;
+  const size_t stride = a.src_stride;
+  const bool aligned = ((((uintptr_t)in) | stride) & 15) == 0;     // every block start is 16-byte aligned
 
   for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < nv;
        i += (size_t)gridDim.x * blockDim.x) {
     const size_t b = i << 4;
-    uint4 mine;
-    if (aligned && b + 16 <= a.nbytes) {
-      mine = *reinterpret_cast<const uint4*>(in + b);
-    } else {
-      alignas(16) unsigned char tmp[16];
-      for (int k = 0; k < 16; ++k) tmp[k] = (b + k < a.nbytes) ? ((const unsigned char*)in)[b + k] : 0;
-      mine = *reinterpret_cast<const uint4*>(tmp);
-    }
+    const uint4 mine = b2_ll_load(in + (size_t)c.rank * stride, b, a.nbytes, aligned);
     // push to every peer's LL buffer, slot [source = my rank][vector i]
-    const uint4 lo = make_uint4(mine.x, flag, mine.y, flag);
-    const uint4 hi = make_uint4(mine.z, flag, mine.w, flag);
     for (int q = 1; q < c.size; ++q) {
       const int p = (c.rank + q) % c.size;
+      const uint4 v = stride ? b2_ll_load(in + (size_t)p * stride, b, a.nbytes, aligned) : mine;
       char* dst = c.heap[p] + par_off + (size_t)c.rank * c.lay.ll_cap + (i << 5);
-      b2_st16_sys(dst, lo);
-      b2_st16_sys(dst + 16, hi);
+      b2_st16_sys(dst, make_uint4(v.x, flag, v.y, flag));
+      b2_st16_sys(dst + 16, make_uint4(v.z, flag, v.w, flag));
     }
     // gather + reduce in rank order (bitwise identical result on every rank)
     B2Vec<T> acc;

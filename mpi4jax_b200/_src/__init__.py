@@ -3,7 +3,7 @@
 The reference imports mpi4py first (MPI_Init + finalize-atexit), gates on the JAX version,
 registers the FFI targets and installs an atexit ``flush`` so that pending asynchronous
 custom calls finish before MPI_Finalize.  Here: gate on the torch version, load the native
-library (``native``), import the 12 ops; ``comm`` registers an atexit hook that drains
+library (``native``), import the 13 ops; ``comm`` registers an atexit hook that drains
 every stream / pending isend and tears the symmetric heaps down *before* the process group
 is destroyed (same purpose: no deadlock or crash at interpreter exit,
 tests/collective_ops/test_common.py:91-115 in the reference).
@@ -25,6 +25,7 @@ from .collective_ops.bcast import bcast  # noqa: E402,F401
 from .collective_ops.gather import gather  # noqa: E402,F401
 from .collective_ops.recv import recv  # noqa: E402,F401
 from .collective_ops.reduce import reduce  # noqa: E402,F401
+from .collective_ops.reduce_scatter import reduce_scatter  # noqa: E402,F401
 from .collective_ops.scan import scan  # noqa: E402,F401
 from .collective_ops.scatter import scatter  # noqa: E402,F401
 from .collective_ops.send import send, send_with_grad  # noqa: E402,F401

@@ -1,4 +1,4 @@
-"""CPU backend: the 12 ops on host tensors over ``torch.distributed`` (gloo).
+"""CPU backend: the 13 ops on host tensors over ``torch.distributed`` (gloo).
 
 Role: what the reference's CPU bridge (mpi_xla_bridge_cpu.cpp, one blocking MPI call
 per op) is to its GPU bridge -- the correctness path that runs anywhere, including the
@@ -136,6 +136,11 @@ def reduce(comm: Comm, x: torch.Tensor, op_code: int, root: int) -> Optional[tor
 def scan(comm: Comm, x: torch.Tensor, op_code: int) -> torch.Tensor:
     stack = _gather_stack(comm, x)
     return reduce_stack(stack[: comm.rank + 1], op_code)
+
+
+def reduce_scatter(comm: Comm, x: torch.Tensor, op_code: int) -> torch.Tensor:
+    # x: (P, *S).  Everybody gathers everything and reduces its own block (correctness path).
+    return reduce_stack(_gather_stack(comm, x)[:, comm.rank], op_code)
 
 
 def allgather(comm: Comm, x: torch.Tensor) -> torch.Tensor:

@@ -60,7 +60,7 @@ def stage_need(opcode: int, nranks: int, blk_bytes: int) -> int:
     """Staging bytes per parity that an op with ``blk_bytes`` per block needs: the Python twin of
     ``b2_stage_need`` (csrc/b2_collectives.cu), which validates every launch with the same formula."""
     stride = (blk_bytes + 15) & ~15
-    mult = nranks if opcode in (codes.OPC_ALLTOALL, codes.OPC_SCATTER) else 1
+    mult = nranks if opcode in (codes.OPC_ALLTOALL, codes.OPC_SCATTER, codes.OPC_REDUCE_SCATTER) else 1
     return stride * mult + 4096
 
 
@@ -325,8 +325,8 @@ class NativeComm:
             self._grow_stage(2 * need + 8192)
 
     def reserve(self, nbytes: int) -> None:
-        """Make sure collectives of up to ``nbytes`` per rank (alltoall / scatter: per peer block
-        times size) never have to grow the staging segment again.  Collective."""
+        """Make sure collectives of up to ``nbytes`` per rank (alltoall / scatter / reduce_scatter: per
+        peer block times size) never have to grow the staging segment again.  Collective."""
         self.ensure_stage(codes.OPC_ALLTOALL, int(nbytes))
 
     @property
@@ -477,6 +477,16 @@ class NativeComm:
         rc = _lib().b2_scan(self.handle, x.data_ptr(), out.data_ptr(), x.numel(), dt, op_code,
                             self._stream())
         self._check(rc, "Scan")
+        return out
+
+    def reduce_scatter(self, x: torch.Tensor, op_code: int) -> torch.Tensor:
+        """``x`` of shape ``(size, *S)``: this rank's ``S``-shaped block of the reduction over ranks."""
+        x, dt, op_code = _prep_reduce(x, op_code)
+        out = torch.empty(x.shape[1:], dtype=x.dtype, device=x.device)
+        self.ensure_stage(codes.OPC_REDUCE_SCATTER, out.numel() * out.element_size())
+        rc = _lib().b2_reduce_scatter(self.handle, x.data_ptr(), out.data_ptr(), out.numel(), dt, op_code,
+                                      self._stream())
+        self._check(rc, "Reduce_scatter_block")
         return out
 
     def allgather(self, x: torch.Tensor) -> torch.Tensor:
@@ -641,7 +651,7 @@ def _nvtx_wrap(name: str, fn):
 #: ``MPI4JAX_B200_NVTX=1``: one NVTX range per op (visible in Nsight Systems timelines); the
 #: methods are left untouched otherwise, so the fast path pays nothing (SURVEY 5.1)
 NVTX_OPS = ("barrier", "allreduce", "reduce", "scan", "allgather", "alltoall", "bcast", "gather", "scatter",
-            "send", "recv", "sendrecv", "gemm_allreduce", "halo_exchange")
+            "send", "recv", "sendrecv", "reduce_scatter", "gemm_allreduce", "halo_exchange")
 if env_flag("MPI4JAX_B200_NVTX", False):
     for _name in NVTX_OPS:
         setattr(NativeComm, _name, _nvtx_wrap(_name, getattr(NativeComm, _name)))

@@ -9,7 +9,7 @@ fallback, never the default on one node:
   needs peer-mapped HBM, i.e. one NVLink domain), with a one-time warning;
 * forced by ``MPI4JAX_B200_TRANSPORT=host`` or the reference's ``MPI4JAX_USE_CUDA_MPI=0``.
 
-Same method surface as ``backends.cuda.NativeComm`` for the 12 ops; the fused / H100-only entry
+Same method surface as ``backends.cuda.NativeComm`` for the 13 ops; the fused / H100-only entry
 points (halo exchange, GEMM+allreduce) raise.  Ops synchronise the stream and block the host, so
 they cannot be captured into CUDA graphs: ``mpi4jax_b200.jit`` runs such functions eagerly.
 """
@@ -53,7 +53,7 @@ class HostStagedComm:
 
     def _unsupported(self, what: str):
         raise MPIError(f"{what} needs the native NVLink transport, but this communicator uses host "
-                       f"staging ({self.reason or 'requested'}); use the 12 primitives instead")
+                       f"staging ({self.reason or 'requested'}); use the 13 primitives instead")
 
     # -- lifecycle (NativeComm surface) ---------------------------------------------
     def flush(self) -> None:
@@ -66,7 +66,7 @@ class HostStagedComm:
     def destroy(self) -> None:
         pass
 
-    # -- the 12 ops ------------------------------------------------------------------
+    # -- the 13 ops ------------------------------------------------------------------
     def barrier(self) -> None:
         self.flush()                      # the reference: stream sync, then MPI_Barrier (cuda.cpp:75-86)
         _cpu.barrier(self.comm)
@@ -79,6 +79,9 @@ class HostStagedComm:
 
     def scan(self, x, op_code: int):
         return self._up(_cpu.scan(self.comm, self._down(x), op_code), x)
+
+    def reduce_scatter(self, x, op_code: int):
+        return self._up(_cpu.reduce_scatter(self.comm, self._down(x), op_code), x)
 
     def allgather(self, x):
         return self._up(_cpu.allgather(self.comm, self._down(x)), x)

@@ -1,2 +1,2 @@
-"""The 12 communication primitives (one module per op, like the reference's
+"""The 13 communication primitives (one module per op, like the reference's
 mpi4jax/_src/collective_ops/)."""

@@ -1,4 +1,4 @@
-"""Backend dispatch for the 12 ops: CUDA tensors -> native kernels, CPU tensors -> gloo.
+"""Backend dispatch for the 13 ops: CUDA tensors -> native kernels, CPU tensors -> gloo.
 
 This is the analogue of the per-platform lowering registration each reference op does
 (``register_lowering(..., platform="cpu"|"cuda"|"xpu")``, e.g.
@@ -109,6 +109,17 @@ def scan(comm: Comm, x: torch.Tensor, op_code: int) -> torch.Tensor:
         return comm._native_comm().scan(x, op_code)
     done = _log(comm, "Scan", f"with {x.numel()} items")
     out = _cpu.scan(comm, x, op_code)
+    if done:
+        done()
+    return out
+
+
+def reduce_scatter(comm: Comm, x: torch.Tensor, op_code: int) -> torch.Tensor:
+    _plain(x)
+    if x.is_cuda:
+        return comm._native_comm().reduce_scatter(x, op_code)
+    done = _log(comm, "Reduce_scatter_block", f"with {x.numel() // x.shape[0]} items per block")
+    out = _cpu.reduce_scatter(comm, x, op_code)
     if done:
         done()
     return out

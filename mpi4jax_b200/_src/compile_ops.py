@@ -1,4 +1,4 @@
-"""``torch.library`` registration of the 12 ops -- the traceable frontend.
+"""``torch.library`` registration of the 13 ops -- the traceable frontend.
 
 The reference's ops are JAX *primitives*: abstract-eval rules give shapes, an ordered effect
 threads a token through every custom call so XLA keeps them in program order
@@ -81,6 +81,30 @@ def _allreduce_backward(ctx, g):
 
 
 _allreduce.register_autograd(_allreduce_backward, setup_context=_allreduce_setup)
+
+
+@custom_op("mpi4jax_b200::reduce_scatter", mutates_args=())
+def _reduce_scatter(x: torch.Tensor, op: int, comm_id: int) -> torch.Tensor:
+    return _dispatch.reduce_scatter(_c(comm_id), x.contiguous(), op)
+
+
+@_reduce_scatter.register_fake
+def _(x, op, comm_id):
+    return x.new_empty(x.shape[1:])
+
+
+def _reduce_scatter_setup(ctx, inputs, output):
+    _, ctx.op, ctx.comm_id = inputs
+
+
+def _reduce_scatter_backward(ctx, g):
+    if ctx.op != SUM.code:
+        raise NotImplementedError("The adjoint of reduce_scatter is only defined for SUM")
+    size = _c(ctx.comm_id).Get_size()
+    return torch.ops.mpi4jax_b200.allgather(g.contiguous(), ctx.comm_id, size), None, None
+
+
+_reduce_scatter.register_autograd(_reduce_scatter_backward, setup_context=_reduce_scatter_setup)
 
 
 @custom_op("mpi4jax_b200::allgather", mutates_args=())
@@ -268,7 +292,7 @@ _sendrecv.register_autograd(_sendrecv_backward, setup_context=_sendrecv_setup)
 
 
 ALL_OPS = ("allreduce", "allgather", "alltoall", "bcast", "scan", "reduce", "gather_root", "gather_leaf",
-           "scatter", "barrier", "send", "recv", "sendrecv")
+           "scatter", "barrier", "send", "recv", "sendrecv", "reduce_scatter")
 ORDERED_EFFECT = False
 try:  # the ordered effect: AOTAutograd threads a token through these ops in program order
     from torch._higher_order_ops.effects import _EffectType, _register_effectful_op
@@ -287,6 +311,13 @@ class compiled:
     @staticmethod
     def allreduce(x, op, *, comm=None):
         return torch.ops.mpi4jax_b200.allreduce(x, as_op(op).code, _register(comm))
+
+    @staticmethod
+    def reduce_scatter(x, op, *, comm=None):
+        comm = comm or get_default_comm()
+        if x.dim() == 0 or x.shape[0] != comm.Get_size():
+            raise ValueError("Reduce_scatter input must have shape (nproc, ...)")
+        return torch.ops.mpi4jax_b200.reduce_scatter(x, as_op(op).code, comm._id)
 
     @staticmethod
     def allgather(x, *, comm=None):
