@@ -4,6 +4,9 @@
   next to NCCL on the same box                                   (configs 2)
 * allgather and alltoall 1 KB - 1 GB per-rank payload vs NCCL     (config 4)
 * reduce_scatter (P, n) fp32 + bf16, 1 KB - 1 GB per-rank input, vs NCCL and vs allreduce
+* alltoallv bf16 token rows, balanced and skewed counts, 64 KiB - 256 MiB per rank, vs NCCL
+  all_to_all_single (with its counts exchange and host read-back) and vs the equal-split alltoall;
+  plus balanced rows of 8190 bytes (the byte-wise path for rows that are not a multiple of 16 bytes)
 * bcast, reduce, gather, scatter (root = last rank) vs NCCL, scan (no NCCL counterpart)
 * sendrecv ring, halo exchange latency
 
@@ -232,6 +235,53 @@ for dtype, dname in ((torch.float32, "fp32"), (torch.bfloat16, "bf16")):
             print("reduce_scatter", dname, nbytes, {k: (v["us"], v["busbw"]) for k, v in row.items()}, flush=True)
         del x
     result["reduce_scatter"][dname] = table
+
+# ---------------------------------------------------------------- alltoallv (per-rank input |x| = nbytes, 64 KiB - 256 MiB)
+# bf16 token rows of hidden size 4096 (8 KiB), the layout of an expert-parallel MoE dispatch.  Balanced:
+# N / P rows to every rank; skewed: half of every rank's rows to rank 0, the rest spread evenly.  Next to
+# the equal-split alltoall at the same bytes, and to what an NCCL-based MoE layer does: exchange the
+# counts, read them back to the host (.tolist(), a device synchronisation), then all_to_all_single with
+# split lists -- which cannot be captured into a CUDA graph, so it is timed eagerly.
+# "odd_rows": balanced again with hidden size 4095 (8190-byte rows), which takes the byte-wise path of the
+# kernel (rows that are not a multiple of 16 bytes).
+result["alltoallv"] = {"balanced": {}, "skewed": {}, "odd_rows": {}}
+
+
+def alltoallv_counts(kind, n):
+    rest = (n - n // 2) // max(size - 1, 1)
+    if kind == "skewed":
+        return [n // 2 + (rest if size == 1 else 0)] + [rest] * (size - 1)
+    return [n // size] * size
+
+
+for nbytes in [b for b in sizes if (64 << 10) <= b <= (256 << 20)]:
+    for kind, hidden in (("balanced", 4096), ("skewed", 4096), ("odd_rows", 4095)):
+        n = nbytes // (hidden * 2)
+        if n < size:
+            continue
+        x = torch.ones(n, hidden, dtype=torch.bfloat16, device=dev)
+        counts = torch.tensor(alltoallv_counts(kind, n), dtype=torch.int64, device=dev)
+        reps = reps_for(nbytes)
+        bw = lambda us: round(n * hidden * 2 * (size - 1) / size / us / 1e3, 1)
+        row = {}
+        us = time_graph(lambda: m.alltoallv(x, counts, comm=comm), reps)
+        row["ours"] = {"us": round(us, 2), "busbw": bw(us)}
+        y = x[: n // size * size].view(size, n // size, hidden)
+        us = time_graph(lambda: m.alltoall(y, comm=comm), reps)
+        row["alltoall"] = {"us": round(us, 2), "busbw": bw(us)}
+        if nccl is not None:
+            def nccl_alltoallv():
+                recv = torch.empty_like(counts)
+                dist.all_to_all_single(recv, counts, group=nccl)
+                send_split, recv_split = counts.tolist(), recv.tolist()
+                out = torch.empty(sum(recv_split), hidden, dtype=x.dtype, device=dev)
+                dist.all_to_all_single(out, x[: sum(send_split)], recv_split, send_split, group=nccl)
+            us = time_eager(nccl_alltoallv, max(reps, 5))
+            row["nccl"] = {"us": round(us, 2), "busbw": bw(us)}
+        result["alltoallv"][kind][str(nbytes)] = row
+        if rank == 0:
+            print("alltoallv", kind, nbytes, {k: (v["us"], v["busbw"]) for k, v in row.items()}, flush=True)
+        del x, y
 
 # ---------------------------------------------------------------- rooted ops + scan (per-rank payload = nbytes)
 result.update({"bcast": {}, "reduce": {}, "gather": {}, "scatter": {}, "scan": {}})

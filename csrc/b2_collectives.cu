@@ -261,6 +261,148 @@ b2_k_move(const __grid_constant__ B2DevComm c, const __grid_constant__ B2MoveArg
 }
 
 // ---------------------------------------------------------------------------
+// alltoallv: row counts that exist only on the device
+//
+// Staging parity of every rank: [header: this rank's clamped send counts, int64 x B2_MAX_RANKS]
+// [the rows it sends, in destination order].  Every CTA writes the header (identical values) before
+// its first arrive, so after the first wait each CTA reads the P x P count matrix from the peers and
+// derives the whole schedule locally -- the same on every rank.  Chunk k indexes bytes of every rank's
+// staged rows and belongs to CTA k mod grid everywhere, as in b2_k_move; the pull of chunk k from
+// peer q is its intersection with q's segment for this rank.
+// ---------------------------------------------------------------------------
+#define B2_A2AV_HDR ((size_t)B2_MAX_RANKS * sizeof(long long))
+
+struct B2AlltoallvArgs {
+  const void* in;
+  void* out;
+  const long long* send_counts;    // [P] rows to each rank (any value: clamped here)
+  const long long* place_counts;   // [P] reverse mode: where the segments land (null: packed, forward)
+  long long* recv_counts;          // [P] rows written from each rank
+  size_t row_bytes;
+  size_t in_rows;
+  size_t out_rows;
+  size_t max_rows;                 // rows a rank may stage, the same on every rank (sizes the staging)
+  size_t chunk;
+  int opcode;
+};
+
+// zero bytes [lo, hi) of `out`, spread over every thread of the grid
+__device__ __forceinline__ void a2av_zero(char* out, size_t lo, size_t hi) {
+  const size_t gt = (size_t)blockIdx.x * blockDim.x + threadIdx.x, gs = (size_t)gridDim.x * blockDim.x;
+  if (lo >= hi) return;
+  const size_t v0 = lo + ((16 - ((uintptr_t)(out + lo) & 15)) & 15);     // first 16-byte aligned byte
+  const size_t tail = (uintptr_t)(out + hi) & 15;
+  const size_t v1 = hi - tail;                                           // end of the aligned vectors
+  if (hi - lo < 32 || v0 >= v1) {
+    for (size_t i = lo + gt; i < hi; i += gs) out[i] = 0;
+    return;
+  }
+  for (size_t i = lo + gt; i < v0; i += gs) out[i] = 0;
+  for (size_t i = v0 + (gt << 4); i < v1; i += gs << 4) b2_st16(out + i, make_uint4(0, 0, 0, 0));
+  for (size_t i = v1 + gt; i < hi; i += gs) out[i] = 0;
+}
+
+__global__ void __launch_bounds__(B2_THREADS, 1)
+b2_k_alltoallv(const __grid_constant__ B2DevComm c, const __grid_constant__ B2AlltoallvArgs a) {
+  __shared__ unsigned long long s_cnt[B2_MAX_RANKS][B2_MAX_RANKS];   // [q][p]: rows rank q sends to p
+  __shared__ size_t s_src[B2_MAX_RANKS], s_dst[B2_MAX_RANKS], s_len[B2_MAX_RANKS];   // bytes
+  __shared__ size_t s_gap[B2_MAX_RANKS + 1][2];                    // output bytes nobody writes
+  __shared__ size_t s_mine, s_nch;
+  const unsigned ticket = b2_ticket_read(c.ticket);
+  const size_t par = (size_t)(ticket & 1u) * c.stage_half;
+  unsigned e = b2_ld_volatile(c.epoch + blockIdx.x);
+  const int t = threadIdx.x, P = c.size, r = c.rank;
+  const char* in = (const char*)a.in;
+  char* out = (char*)a.out;
+  char* mine = c.stage[r] + par;
+  const size_t rb = a.row_bytes;
+  // 1. this rank's send counts, clamped in rank order to the rows that exist -> header
+  if (t == 0) {
+    const size_t n = a.in_rows < a.max_rows ? a.in_rows : a.max_rows;
+    size_t used = 0;
+    for (int q = 0; q < P; ++q) {
+      const long long want = a.send_counts[q];
+      size_t s = want > 0 ? (size_t)want : 0;
+      if (s > n - used) s = n - used;
+      used += s;
+      ((volatile unsigned long long*)mine)[q] = s;
+    }
+    s_mine = used * rb;
+  }
+  __syncthreads();
+  const size_t mine_bytes = s_mine;
+  char* mine_rows = mine + B2_A2AV_HDR;
+#define CH_LEN(ch) ((ch) * a.chunk < mine_bytes                                                         \
+                        ? (mine_bytes - (ch) * a.chunk < a.chunk ? mine_bytes - (ch) * a.chunk : a.chunk) \
+                        : (size_t)0)
+  size_t ch = blockIdx.x;
+  b2_copy_bytes<false>(mine_rows + ch * a.chunk, in + ch * a.chunk, CH_LEN(ch));
+  b2_barrier_arrive(c, ++e);
+  unsigned e_cur = e;
+  b2_barrier_wait(c, e_cur, a.opcode);              // every rank's header and chunk blockIdx.x are staged
+  // 2. the count matrix and this rank's receive schedule
+  if (t < P * P) s_cnt[t / P][t % P] = ((const volatile unsigned long long*)(c.stage[t / P] + par))[t % P];
+  __syncthreads();
+  if (t == 0) {
+    size_t smax = 0, filled = 0;
+    for (int q = 0; q < P; ++q) {
+      size_t tot = 0, d = 0;
+      for (int p = 0; p < P; ++p) {
+        if (p == r) d = tot;
+        tot += s_cnt[q][p];
+      }
+      if (tot > smax) smax = tot;
+      // forward: packed in source order, clipped to the output rows; reverse: at the sum of the
+      // (clamped) place counts of the lower ranks, at most place_counts[q] rows
+      size_t k = s_cnt[q][r], slot = a.out_rows - filled;
+      if (a.place_counts != nullptr) {
+        const long long w = a.place_counts[q];
+        if (w < 0) slot = 0;
+        else if ((size_t)w < slot) slot = (size_t)w;
+      }
+      if (k > slot) k = slot;
+      if (a.place_counts == nullptr) slot = k;
+      s_src[q] = d * rb;
+      s_dst[q] = filled * rb;
+      s_len[q] = k * rb;
+      s_gap[q][0] = (filled + k) * rb;
+      s_gap[q][1] = (filled + slot) * rb;
+      if (blockIdx.x == 0) a.recv_counts[q] = (long long)k;
+      filled += slot;
+    }
+    s_gap[P][0] = filled * rb;
+    s_gap[P][1] = a.out_rows * rb;
+    s_nch = (smax * rb + a.chunk - 1) / a.chunk;     // the same on every rank
+  }
+  __syncthreads();
+  // 3. stage -> arrive -> wait -> pull, software-pipelined over the chunks of this CTA
+  const size_t nch = s_nch;
+  for (; ch < nch; ch += gridDim.x) {
+    if (ch != blockIdx.x) b2_barrier_wait(c, e_cur, a.opcode);
+    const size_t off = ch * a.chunk, end = off + a.chunk;
+    for (int s2 = 0; s2 < P; ++s2) {
+      const int q = (s2 + r) % P;                    // stagger peers across ranks
+      const size_t lo = off > s_src[q] ? off : s_src[q];
+      const size_t hi = end < s_src[q] + s_len[q] ? end : s_src[q] + s_len[q];
+      if (lo < hi)
+        b2_copy_bytes<true>(out + s_dst[q] + (lo - s_src[q]), c.stage[q] + par + B2_A2AV_HDR + lo, hi - lo);
+    }
+    const size_t nxt = ch + gridDim.x;
+    if (nxt < nch) {
+      b2_copy_bytes<false>(mine_rows + nxt * a.chunk, in + nxt * a.chunk, CH_LEN(nxt));
+      b2_barrier_arrive(c, ++e);
+      e_cur = e;
+    }
+  }
+#undef CH_LEN
+  // 4. rows nobody sends are zero: the output is fully written on every call
+  for (int q = 0; q <= P; ++q) a2av_zero(out, s_gap[q][0], s_gap[q][1]);
+  __syncthreads();
+  if (t == 0) b2_st_volatile(c.epoch + blockIdx.x, e);
+  b2_finish_bump(c.ticket, c.ticket + 1, 1u, gridDim.x);
+}
+
+// ---------------------------------------------------------------------------
 // NVLS allreduce (SUM; f32 / bf16 / f16 with fp32 accumulation in the switch)
 // ---------------------------------------------------------------------------
 template <int DT>
@@ -601,6 +743,8 @@ extern "C" size_t b2_stage_need(int opcode, int nranks, size_t blk_bytes) {
     case B2_OPC_SCATTER:
     case B2_OPC_REDUCE_SCATTER:
       return stride * (size_t)nranks + 4096;
+    case B2_OPC_ALLTOALLV:                       // blk_bytes: the most bytes of rows a rank stages
+      return B2_A2AV_HDR + stride + 4096;
     default:
       return stride + 4096;
   }
@@ -930,6 +1074,34 @@ extern "C" int b2_scatter(B2Comm* c, const void* in, void* out, size_t blk_bytes
     a.src_rank[0] = root; a.src_blk[0] = c->dev.rank; a.dst_blk[0] = 0;
     rc = set_layout(a, c->dev.rank == root ? lay : nullptr, "scatter");
     if (rc == 0) rc = move_common(c, a, "scatter", stream);
+  }
+  b2_debug_end(dbg, rc);
+  return rc;
+}
+
+// The launch geometry depends only on sizes every rank agrees on: the forward's input rows (the same
+// everywhere) or, in reverse mode, nranks x its output rows (the forward's input rows again).  The
+// counts are read on the device, so the host never waits for them.
+extern "C" int b2_alltoallv(B2Comm* c, const void* in, void* out, size_t row_bytes, size_t in_rows, size_t out_rows,
+                            const long long* send_counts, long long* recv_counts, const long long* place_counts,
+                            cudaStream_t stream) {
+  B2DebugScope* dbg = b2_debug_begin(c, "Alltoallv", stream, "with %zu rows of %zu bytes", in_rows, row_bytes);
+  B2AlltoallvArgs a;
+  memset(&a, 0, sizeof a);
+  a.in = in; a.out = out; a.send_counts = send_counts; a.place_counts = place_counts; a.recv_counts = recv_counts;
+  a.row_bytes = row_bytes; a.in_rows = in_rows; a.out_rows = out_rows; a.opcode = B2_OPC_ALLTOALLV;
+  a.max_rows = place_counts == nullptr ? in_rows : (size_t)c->dev.size * out_rows;
+  int rc = 0;
+  if (send_counts == nullptr || recv_counts == nullptr) {
+    b2_set_error("alltoallv: send_counts and recv_counts must be device arrays of %d int64", c->dev.size);
+    rc = B2_ERR_BAD_ARG;
+  }
+  if (rc == 0) rc = check_stage(c, a.opcode, a.max_rows * row_bytes, "alltoallv");
+  if (rc == 0) {
+    int grid;
+    pick_chunks(c, a.max_rows * row_bytes, coresident_blocks(c, (const void*)b2_k_alltoallv), &a.chunk, &grid);
+    b2_k_alltoallv<<<grid, B2_THREADS, 0, stream>>>(c->dev, a);
+    rc = b2_launched(c, "alltoallv");
   }
   b2_debug_end(dbg, rc);
   return rc;

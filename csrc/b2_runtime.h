@@ -150,6 +150,15 @@ int b2_gather(B2Comm* c, const void* in, void* out, size_t blk_bytes, int root, 
               cudaStream_t stream);
 int b2_scatter(B2Comm* c, const void* in, void* out, size_t blk_bytes, int root, const B2Strided* lay,
                cudaStream_t stream);
+// Variable-count all-to-all whose counts stay on the device.  `in`: in_rows rows of row_bytes bytes
+// (contiguous); `send_counts`, `recv_counts`: [nranks] int64 device arrays.  Forward (place_counts
+// null): rows sent to each rank are clamped in rank order to the rows that exist, received segments
+// are packed in source order and clipped to out_rows.  Reverse (place_counts = the send counts of a
+// forward call, out_rows = its in_rows): the segment from rank q lands at the sum of place_counts[p]
+// over p < q.  Output rows that receive nothing are zeroed; recv_counts holds the rows written.
+int b2_alltoallv(B2Comm* c, const void* in, void* out, size_t row_bytes, size_t in_rows, size_t out_rows,
+                 const long long* send_counts, long long* recv_counts, const long long* place_counts,
+                 cudaStream_t stream);
 
 // --- point to point ----------------------------------------------------------
 // source/tag may be -1 (ANY).  `status` is a host-mapped B2StatusRecord or null.

@@ -1,4 +1,4 @@
-"""CPU backend: the 13 ops on host tensors over ``torch.distributed`` (gloo).
+"""CPU backend: the 14 ops on host tensors over ``torch.distributed`` (gloo).
 
 Role: what the reference's CPU bridge (mpi_xla_bridge_cpu.cpp, one blocking MPI call
 per op) is to its GPU bridge -- the correctness path that runs anywhere, including the
@@ -151,6 +151,42 @@ def alltoall(comm: Comm, x: torch.Tensor) -> torch.Tensor:
     # x: (P, *S).  Everybody gathers everything and keeps its column (correctness path).
     stack = _gather_stack(comm, x)            # (P_src, P_dst, *S)
     return stack[:, comm.rank].clone()
+
+
+def _clamp_in_order(counts, n: int) -> list:
+    """Counts clamped in rank order to ``n`` rows: negative -> 0, nothing past row ``n``."""
+    out, used = [], 0
+    for c in counts:
+        k = min(max(int(c), 0), n - used)
+        out.append(k)
+        used += k
+    return out
+
+
+def alltoallv(comm: Comm, x: torch.Tensor, send_counts: torch.Tensor, out_rows: int,
+              place_counts: Optional[torch.Tensor] = None):
+    """Same rules as the kernel (csrc/b2_collectives.cu: b2_k_alltoallv): everybody gathers every
+    rank's clamped counts and sent rows, then assembles its own output (correctness path)."""
+    P, r = comm.size, comm.rank
+    rows = x.shape[0]
+    max_rows = rows if place_counts is None else P * out_rows
+    sent = _clamp_in_order(send_counts.tolist(), min(rows, max_rows))
+    counts = _gather_stack(comm, torch.tensor(sent, dtype=torch.int64)).tolist()      # [q][p]
+    width = max(sum(row) for row in counts)
+    mine = torch.zeros((width, *x.shape[1:]), dtype=x.dtype)
+    mine[: sum(sent)] = x[: sum(sent)]
+    stack = _gather_stack(comm, mine)                                                   # (P, width, *S)
+    out = torch.zeros((out_rows, *x.shape[1:]), dtype=x.dtype)
+    place = None if place_counts is None else _clamp_in_order(place_counts.tolist(), out_rows)
+    recv, filled = [], 0
+    for q in range(P):
+        d = sum(counts[q][:r])
+        slot = out_rows - filled if place is None else place[q]
+        k = min(counts[q][r], slot)
+        out[filled: filled + k] = stack[q, d: d + k]
+        recv.append(k)
+        filled += k if place is None else slot
+    return out, torch.tensor(recv, dtype=torch.int64)
 
 
 def bcast(comm: Comm, x: torch.Tensor, root: int) -> torch.Tensor:

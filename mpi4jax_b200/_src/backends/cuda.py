@@ -18,6 +18,7 @@ from __future__ import annotations
 
 import ctypes
 import functools
+import math
 import os
 import socket
 import sys
@@ -60,8 +61,15 @@ def stage_need(opcode: int, nranks: int, blk_bytes: int) -> int:
     """Staging bytes per parity that an op with ``blk_bytes`` per block needs: the Python twin of
     ``b2_stage_need`` (csrc/b2_collectives.cu), which validates every launch with the same formula."""
     stride = (blk_bytes + 15) & ~15
+    if opcode == codes.OPC_ALLTOALLV:         # a header of the send counts in front of the rows
+        return ALLTOALLV_HEADER + stride + 4096
     mult = nranks if opcode in (codes.OPC_ALLTOALL, codes.OPC_SCATTER, codes.OPC_REDUCE_SCATTER) else 1
     return stride * mult + 4096
+
+
+#: bytes in front of the rows an alltoallv stages: the rank's clamped send counts, one int64 per possible
+#: rank (B2_A2AV_HDR; MAX_RANKS is checked against the library at import)
+ALLTOALLV_HEADER = native.MAX_RANKS * 8
 
 
 def abort_or_raise(message: str, code: int = 1):
@@ -541,6 +549,26 @@ class NativeComm:
         self._check(rc, "Scatter")
         return out
 
+    def alltoallv(self, x: torch.Tensor, send_counts: torch.Tensor, out_rows: int,
+                  place_counts: Optional[torch.Tensor] = None):
+        """``(out, recv_counts)``: rows of ``x`` exchanged by the device-resident ``send_counts``
+        (``collective_ops/alltoallv.py`` states the rules).  ``place_counts``: the reverse mode, which
+        puts the rows from rank q where a forward call with these send counts took them from."""
+        x = _prep(x)
+        row_bytes = math.prod(x.shape[1:]) * x.element_size()
+        max_rows = x.shape[0] if place_counts is None else self.comm.size * out_rows
+        out = torch.empty((out_rows, *x.shape[1:]), dtype=x.dtype, device=x.device)
+        recv_counts = torch.empty(self.comm.size, dtype=torch.int64, device=x.device)
+        send_counts = send_counts.to(torch.int64).contiguous()
+        if place_counts is not None:
+            place_counts = place_counts.to(torch.int64).contiguous()
+        self.ensure_stage(codes.OPC_ALLTOALLV, max_rows * row_bytes)
+        rc = _lib().b2_alltoallv(self.handle, x.data_ptr(), out.data_ptr(), row_bytes, x.shape[0], out_rows,
+                                 send_counts.data_ptr(), recv_counts.data_ptr(),
+                                 None if place_counts is None else place_counts.data_ptr(), self._stream())
+        self._check(rc, "Alltoallv")
+        return out, recv_counts
+
     # -- point to point ------------------------------------------------------------
     def _status_record(self, status: Optional[Status], itemsize: int):
         if status is None:
@@ -651,7 +679,7 @@ def _nvtx_wrap(name: str, fn):
 #: ``MPI4JAX_B200_NVTX=1``: one NVTX range per op (visible in Nsight Systems timelines); the
 #: methods are left untouched otherwise, so the fast path pays nothing (SURVEY 5.1)
 NVTX_OPS = ("barrier", "allreduce", "reduce", "scan", "allgather", "alltoall", "bcast", "gather", "scatter",
-            "send", "recv", "sendrecv", "reduce_scatter", "gemm_allreduce", "halo_exchange")
+            "send", "recv", "sendrecv", "reduce_scatter", "alltoallv", "gemm_allreduce", "halo_exchange")
 if env_flag("MPI4JAX_B200_NVTX", False):
     for _name in NVTX_OPS:
         setattr(NativeComm, _name, _nvtx_wrap(_name, getattr(NativeComm, _name)))

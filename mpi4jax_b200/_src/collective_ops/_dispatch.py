@@ -1,4 +1,4 @@
-"""Backend dispatch for the 13 ops: CUDA tensors -> native kernels, CPU tensors -> gloo.
+"""Backend dispatch for the 14 ops: CUDA tensors -> native kernels, CPU tensors -> gloo.
 
 This is the analogue of the per-platform lowering registration each reference op does
 (``register_lowering(..., platform="cpu"|"cuda"|"xpu")``, e.g.
@@ -8,6 +8,7 @@ device back ends, chosen by where the operand lives.
 
 from __future__ import annotations
 
+import math
 from typing import Optional
 
 import torch
@@ -142,6 +143,41 @@ def alltoall(comm: Comm, x: torch.Tensor) -> torch.Tensor:
         return comm._native_comm().alltoall(x)
     done = _log(comm, "Alltoall", f"with {x.numel()} items")
     out = _cpu.alltoall(comm, x)
+    if done:
+        done()
+    return out
+
+
+def check_alltoallv_args(comm: Comm, x: torch.Tensor, counts: torch.Tensor, out_rows: int,
+                         name: str = "send_counts") -> None:
+    """Host-side checks of an alltoallv call.  Every entry point (the op, ``compiled.alltoallv``, the raw
+    ``torch.ops`` op, the backends) passes through them: the kernel dereferences the counts as ``nproc``
+    int64 values in x's device memory, so anything else must be refused before the launch."""
+    if x.dim() == 0:
+        raise ValueError("Alltoallv input must have shape (rows, ...)")
+    if not isinstance(counts, torch.Tensor):
+        raise TypeError(f"Alltoallv {name} must be an integer tensor (got {type(counts).__name__})")
+    if counts.dtype.is_floating_point or counts.dtype.is_complex or counts.dtype == torch.bool:
+        raise TypeError(f"Alltoallv {name} must be an integer tensor (got {counts.dtype})")
+    if tuple(counts.shape) != (comm.Get_size(),):
+        raise ValueError(f"Alltoallv {name} must have shape (nproc,) (got {tuple(counts.shape)})")
+    if counts.device != x.device:
+        raise ValueError(f"Alltoallv {name} must live on the device of x ({x.device}, got {counts.device})")
+    if out_rows < 0:
+        raise ValueError(f"Alltoallv recv_capacity must be >= 0 (got {out_rows})")
+
+
+def alltoallv(comm: Comm, x: torch.Tensor, send_counts: torch.Tensor, out_rows: int,
+              place_counts: Optional[torch.Tensor] = None):
+    _plain(x)
+    check_alltoallv_args(comm, x, send_counts, out_rows)
+    if place_counts is not None:
+        check_alltoallv_args(comm, x, place_counts, out_rows, "place_counts")
+    if x.is_cuda:
+        return comm._native_comm().alltoallv(x, send_counts, out_rows, place_counts)
+    row_bytes = math.prod(x.shape[1:]) * x.element_size()
+    done = _log(comm, "Alltoallv", f"with {x.shape[0]} rows of {row_bytes} bytes")
+    out = _cpu.alltoallv(comm, x, send_counts, out_rows, place_counts)
     if done:
         done()
     return out

@@ -1,4 +1,4 @@
-"""``torch.library`` registration of the 13 ops -- the traceable frontend.
+"""``torch.library`` registration of the 14 ops -- the traceable frontend.
 
 The reference's ops are JAX *primitives*: abstract-eval rules give shapes, an ordered effect
 threads a token through every custom call so XLA keeps them in program order
@@ -151,6 +151,39 @@ def _alltoall_backward(ctx, g):
 _alltoall.register_autograd(_alltoall_backward, setup_context=_alltoall_setup)
 
 
+@custom_op("mpi4jax_b200::alltoallv", mutates_args=())
+def _alltoallv(x: torch.Tensor, send_counts: torch.Tensor, out_rows: int, place_counts: Optional[torch.Tensor],
+               comm_id: int) -> tuple[torch.Tensor, torch.Tensor]:
+    return _dispatch.alltoallv(_c(comm_id), x.contiguous(), send_counts, out_rows, place_counts)
+
+
+@_alltoallv.register_fake
+def _(x, send_counts, out_rows, place_counts, comm_id):
+    comm = _c(comm_id)
+    _dispatch.check_alltoallv_args(comm, x, send_counts, out_rows)
+    return x.new_empty((out_rows, *x.shape[1:])), x.new_empty((comm.Get_size(),), dtype=torch.int64)
+
+
+def _alltoallv_setup(ctx, inputs, output):
+    x, send_counts, _, place_counts, ctx.comm_id = inputs
+    ctx.in_rows = x.shape[0]
+    ctx.reverse = place_counts is not None
+    ctx.save_for_backward(send_counts, place_counts, output[1])
+
+
+def _alltoallv_backward(ctx, g, _g_counts):
+    # forward <-> reverse mode (collective_ops/alltoallv.py): the rows travel back the way they came
+    send_counts, place_counts, recv_counts = ctx.saved_tensors
+    if ctx.reverse:
+        back = torch.ops.mpi4jax_b200.alltoallv(g.contiguous(), place_counts, ctx.in_rows, None, ctx.comm_id)
+    else:
+        back = torch.ops.mpi4jax_b200.alltoallv(g.contiguous(), recv_counts, ctx.in_rows, send_counts, ctx.comm_id)
+    return back[0], None, None, None, None
+
+
+_alltoallv.register_autograd(_alltoallv_backward, setup_context=_alltoallv_setup)
+
+
 @custom_op("mpi4jax_b200::bcast", mutates_args=())
 def _bcast(x: torch.Tensor, root: int, comm_id: int) -> torch.Tensor:
     out = _dispatch.bcast(_c(comm_id), x.contiguous(), root)
@@ -292,7 +325,7 @@ _sendrecv.register_autograd(_sendrecv_backward, setup_context=_sendrecv_setup)
 
 
 ALL_OPS = ("allreduce", "allgather", "alltoall", "bcast", "scan", "reduce", "gather_root", "gather_leaf",
-           "scatter", "barrier", "send", "recv", "sendrecv", "reduce_scatter")
+           "scatter", "barrier", "send", "recv", "sendrecv", "reduce_scatter", "alltoallv")
 ORDERED_EFFECT = False
 try:  # the ordered effect: AOTAutograd threads a token through these ops in program order
     from torch._higher_order_ops.effects import _EffectType, _register_effectful_op
@@ -327,6 +360,17 @@ class compiled:
     @staticmethod
     def alltoall(x, *, comm=None):
         return torch.ops.mpi4jax_b200.alltoall(x, _register(comm))
+
+    @staticmethod
+    def alltoallv(x, send_counts, *, recv_capacity=None, comm=None):
+        """``(out, recv_counts)`` of :func:`mpi4jax_b200.alltoallv`; ``send_counts`` must be a device
+        tensor of shape ``(nproc,)``."""
+        comm = comm or get_default_comm()
+        if x.dim() == 0:
+            raise ValueError("Alltoallv input must have shape (rows, ...)")
+        cap = x.shape[0] * comm.Get_size() if recv_capacity is None else recv_capacity
+        _dispatch.check_alltoallv_args(comm, x, send_counts, cap)
+        return torch.ops.mpi4jax_b200.alltoallv(x, send_counts, cap, None, comm._id)
 
     @staticmethod
     def bcast(x, root, *, comm=None):

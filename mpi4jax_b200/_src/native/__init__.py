@@ -176,6 +176,10 @@ _SIGNATURES = {
     "b2_bcast": (c_int, [c_void_p, c_void_p, c_void_p, c_size_t, c_int, POINTER(B2Strided), c_void_p]),
     "b2_gather": (c_int, [c_void_p, c_void_p, c_void_p, c_size_t, c_int, POINTER(B2Strided), c_void_p]),
     "b2_scatter": (c_int, [c_void_p, c_void_p, c_void_p, c_size_t, c_int, POINTER(B2Strided), c_void_p]),
+    "b2_alltoallv": (
+        c_int,
+        [c_void_p, c_void_p, c_void_p, c_size_t, c_size_t, c_size_t, c_void_p, c_void_p, c_void_p, c_void_p],
+    ),
     "b2_status_alloc": (POINTER(B2StatusRecord), []),
     "b2_status_free": (None, [POINTER(B2StatusRecord)]),
     "b2_send": (c_int, [c_void_p, c_void_p, c_size_t, c_int, c_int, c_void_p]),
@@ -208,13 +212,15 @@ _SIGNATURES = {
 
 
 #: must equal B2_ABI_VERSION in csrc/b2_common.h
-ABI_VERSION = 13
+ABI_VERSION = 14
+#: must equal B2_MAX_RANKS in csrc/b2_common.h (ranks per communicator; sizes the alltoallv count header)
+MAX_RANKS = 16
 _ABI_FIELDS = ("abi_version", "sizeof_status_record", "sizeof_halo_desc", "sizeof_swe_params",
                "sizeof_swe_state", "sizeof_error_record", "max_ranks", "p2p_nslot", "sizeof_swe_ca")
 
 
 def _abi_expected() -> dict:
-    return {"abi_version": ABI_VERSION, "sizeof_status_record": ctypes.sizeof(B2StatusRecord),
+    return {"abi_version": ABI_VERSION, "max_ranks": MAX_RANKS, "sizeof_status_record": ctypes.sizeof(B2StatusRecord),
             "sizeof_halo_desc": ctypes.sizeof(B2HaloDesc), "sizeof_swe_params": ctypes.sizeof(B2SweParams),
             "sizeof_swe_state": ctypes.sizeof(B2SweState), "sizeof_swe_ca": ctypes.sizeof(B2SweCA)}
 

@@ -42,5 +42,6 @@ ALGO_BY_NAME = {
 OPC_ALLREDUCE, OPC_REDUCE, OPC_SCAN, OPC_ALLGATHER, OPC_ALLTOALL = 1, 2, 3, 4, 5
 OPC_BCAST, OPC_GATHER, OPC_SCATTER = 6, 7, 8
 OPC_REDUCE_SCATTER = 13
+OPC_ALLTOALLV = 14
 
 ANY = -1  # ANY_SOURCE / ANY_TAG on the wire

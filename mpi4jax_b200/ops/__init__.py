@@ -1,8 +1,8 @@
-"""Functional op namespace: the 13 primitives plus the fused ops that go beyond the
+"""Functional op namespace: the 14 primitives plus the fused ops that go beyond the
 reference's one-MPI-call-per-op model (fused multi-field halo exchange)."""
 
 from .._src import (  # noqa: F401
-    allgather, allreduce, alltoall, barrier, bcast, gather, recv, reduce, reduce_scatter, scan, scatter,
+    allgather, allreduce, alltoall, alltoallv, barrier, bcast, gather, recv, reduce, reduce_scatter, scan, scatter,
     send, send_with_grad, sendrecv,
 )
 from .halo import halo_exchange  # noqa: F401

@@ -8,6 +8,7 @@ They are provided here as small, tested helpers:
 * ``column_parallel_matvec`` / ``row_parallel_matvec`` tensor parallel (test_allreduce_matvec.py:41-65)
 * ``ring_shift``                                      sequence/context-parallel building block
 * ``alltoall_reshard``                                Ulysses-style head<->sequence reshard
+* ``expert_dispatch`` / ``expert_combine``            mixture-of-experts token routing (alltoallv)
 * ``pipeline_send`` / ``pipeline_recv``               differentiable stage boundary (extension)
 * ``cartesian_neighbors``                             2-D domain decomposition (shallow_water.py:64-107)
 """
@@ -18,6 +19,8 @@ from .patterns import (  # noqa: F401
     broadcast_parameters,
     cartesian_neighbors,
     column_parallel_matvec,
+    expert_combine,
+    expert_dispatch,
     pipeline_recv,
     pipeline_send,
     ring_shift,

@@ -2,12 +2,13 @@
 
 from __future__ import annotations
 
-from typing import Iterable, Optional
+from typing import Iterable, NamedTuple, Optional
 
 import numpy as np
 import torch
 
 from .. import _src as ops
+from .._src.collective_ops.alltoallv import alltoallv_reverse
 from .._src.comm import SUM, Comm
 from .._src.utils import get_default_comm
 
@@ -58,6 +59,45 @@ def alltoall_reshard(x: torch.Tensor, scatter_dim: int, gather_dim: int,
     parts = torch.stack(torch.chunk(x, n, dim=scatter_dim), dim=0)      # (n, ...)
     recv = ops.alltoall(parts, comm=comm)                               # recv[q] = peer q's chunk
     return torch.cat(list(recv.unbind(0)), dim=gather_dim)
+
+
+class ExpertPlan(NamedTuple):
+    """What :func:`expert_combine` needs to undo an :func:`expert_dispatch` (all on the device)."""
+
+    order: torch.Tensor          # (N,) token index of each sorted row
+    send_counts: torch.Tensor    # (nproc,) int64 tokens sent to each rank
+    recv_counts: torch.Tensor    # (nproc,) int64 rows received from each rank
+    comm: Comm
+
+
+def expert_dispatch(x: torch.Tensor, dest_rank: torch.Tensor, capacity: Optional[int] = None,
+                    comm: Optional[Comm] = None):
+    """Send every token (row of ``x``) to the rank ``dest_rank`` names -- the dispatch of an
+    expert-parallel mixture-of-experts layer.  Returns ``(rows, recv_counts, plan)``: the received
+    tokens packed by source rank in a ``(capacity, ...)`` tensor (default capacity ``N * nproc``),
+    the rows received from each rank, and the plan :func:`expert_combine` uses to bring results back.
+    Tokens that do not fit the receiver's capacity are dropped, as are tokens whose destination is not
+    a rank.  Differentiable; the counts never leave the device (no host synchronisation)."""
+    comm = comm or get_default_comm()
+    n = comm.Get_size()
+    if dest_rank.shape != x.shape[:1]:
+        raise ValueError(f"expert_dispatch: dest_rank must have shape ({x.shape[0]},) (got {tuple(dest_rank.shape)})")
+    # invalid destinations sort last and are counted for no rank, so they are never sent
+    key = torch.where((dest_rank >= 0) & (dest_rank < n), dest_rank, n).to(torch.int64)
+    order = torch.argsort(key, stable=True)
+    # counts from the sorted keys: torch.bincount would read its maximum back to the host
+    bounds = torch.searchsorted(key[order], torch.arange(n + 1, device=key.device))
+    send_counts = bounds.diff()
+    rows, recv_counts = ops.alltoallv(x[order], send_counts, recv_capacity=capacity, comm=comm)
+    return rows, recv_counts, ExpertPlan(order, send_counts, recv_counts, comm)
+
+
+def expert_combine(y: torch.Tensor, plan: ExpertPlan) -> torch.Tensor:
+    """Return the rows of ``y`` (laid out like :func:`expert_dispatch`'s output, e.g. the experts'
+    results) to the ranks and token positions they came from.  Dropped tokens come back as zeros.
+    Differentiable; no host synchronisation."""
+    back = alltoallv_reverse(y, plan.recv_counts, plan.send_counts, plan.order.shape[0], plan.comm)
+    return torch.zeros_like(back).index_copy(0, plan.order, back)
 
 
 def pipeline_send(x: torch.Tensor, dest: int, tag: int = 0, comm: Optional[Comm] = None):
