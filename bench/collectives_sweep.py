@@ -7,6 +7,8 @@
 * alltoallv bf16 token rows, balanced and skewed counts, 64 KiB - 256 MiB per rank, vs NCCL
   all_to_all_single (with its counts exchange and host read-back) and vs the equal-split alltoall;
   plus balanced rows of 8190 bytes (the byte-wise path for rows that are not a multiple of 16 bytes)
+* allgatherv bf16 rows, full / half / skewed counts, 64 KiB - 256 MiB per rank, vs the allgather of the
+  padded rows (alone and followed by a device-side compaction) and vs NCCL all_gather_into_tensor
 * bcast, reduce, gather, scatter (root = last rank) vs NCCL, scan (no NCCL counterpart)
 * sendrecv ring, halo exchange latency
 
@@ -40,6 +42,7 @@ ap.add_argument("--quick", action="store_true", help="every fourth size")
 ap.add_argument("--skip-allreduce-algos", action="store_true", help="time only the automatic choice")
 ap.add_argument("--only-allreduce", action="store_true", help="stop after the allreduce tables")
 ap.add_argument("--only-p2p", action="store_true", help="only the p2p ring, barrier and halo lines")
+ap.add_argument("--only-allgatherv", action="store_true", help="only the allgatherv rows")
 ap.add_argument("--max-blocks", type=int, default=0, help="override the collective grid cap")
 ap.add_argument("--nvls-pipeline", type=int, default=-1, help="0 / 1: software pipelining of the NVLS allreduce")
 ap.add_argument("--min-bytes", type=int, default=1 << 10)
@@ -126,6 +129,64 @@ def time_nccl(fn, reps):
 
 sizes = [] if ns.only_p2p else [1 << k for k in range(10, 31, 2 if ns.quick else 1) if ns.min_bytes <= (1 << k) <= ns.max_bytes]
 result = {"world": size, "nvls": has_nvls, "allreduce": {}, "allgather": {}, "alltoall": {}, "p2p": {}}
+
+
+# ---------------------------------------------------------------- allgatherv (per-rank |x| = nbytes, 64 KiB - 256 MiB)
+# bf16 rows of hidden size 4096 (8 KiB), every rank contributing count_r of its N rows: "full" (N), "half"
+# (N / 2) and "skewed" (rank r contributes N * (r + 1) / P).  Next to the allgather of the padded N rows,
+# to that allgather followed by the device-side compaction a user would write without allgatherv (gather
+# the counts too, scatter the valid rows to their packed positions: capturable, no host read), and to
+# NCCL's all_gather_into_tensor of the padded rows.  Bandwidth: the bytes a rank receives from its peers,
+# sum_{q != r} count_q * row_bytes (the most over ranks), divided by the time -- the same numerator for
+# every column, so the columns compare as times do.
+def allgatherv_rows():
+    result["allgatherv"] = {"full": {}, "half": {}, "skewed": {}}
+    hidden = 4096
+    for nbytes in [b for b in sizes if (64 << 10) <= b <= (256 << 20)]:
+        n = nbytes // (hidden * 2)
+        for kind in ("full", "half", "skewed"):
+            counts = [n if kind == "full" else n // 2 if kind == "half" else n * (q + 1) // size
+                      for q in range(size)]
+            useful = max(sum(counts) - counts[q] for q in range(size)) * hidden * 2
+            bw = lambda us: round(useful / us / 1e3, 1)
+            x = torch.ones(n, hidden, dtype=torch.bfloat16, device=dev)
+            count = torch.tensor(counts[rank], dtype=torch.int64, device=dev)
+            reps = reps_for(nbytes * size // 2)
+            row = {}
+            us = time_graph(lambda: m.allgatherv(x, count, comm=comm), reps)
+            row["ours"] = {"us": round(us, 2), "busbw": bw(us)}
+            us = time_graph(lambda: m.allgather(x, comm=comm), reps)
+            row["allgather"] = {"us": round(us, 2), "busbw": bw(us)}
+            rows = torch.arange(n, device=dev)
+
+            def allgather_compact():
+                xs = m.allgather(x, comm=comm)                                      # (P, N, hidden)
+                cs = m.allgather(count.view(1), comm=comm).view(size, 1)
+                dest = torch.where(rows < cs, torch.cumsum(cs, 0) - cs + rows, n * size)   # invalid -> pad row
+                out = torch.zeros(n * size + 1, hidden, dtype=x.dtype, device=dev)
+                return out.index_copy_(0, dest.view(-1), xs.view(-1, hidden))[: n * size]
+
+            us = time_graph(allgather_compact, reps)
+            row["allgather_compact"] = {"us": round(us, 2), "busbw": bw(us)}
+            if nccl is not None:
+                out = torch.empty(size * n, hidden, dtype=x.dtype, device=dev)
+                us = time_nccl(lambda: dist.all_gather_into_tensor(out, x, group=nccl), reps)
+                row["nccl"] = {"us": round(us, 2), "busbw": bw(us)}
+                del out
+            result["allgatherv"][kind][str(nbytes)] = row
+            if rank == 0:
+                print("allgatherv", kind, nbytes, {k: (v["us"], v["busbw"]) for k, v in row.items()}, flush=True)
+            del x
+
+
+if ns.only_allgatherv:
+    allgatherv_rows()
+    if rank == 0:
+        os.makedirs(os.path.dirname(ns.out) or ".", exist_ok=True)
+        with open(ns.out, "w") as f:
+            json.dump(result, f, indent=1)
+    m.flush()
+    sys.exit(0)
 
 # ---------------------------------------------------------------- allreduce
 sym_pool = None
@@ -282,6 +343,8 @@ for nbytes in [b for b in sizes if (64 << 10) <= b <= (256 << 20)]:
         if rank == 0:
             print("alltoallv", kind, nbytes, {k: (v["us"], v["busbw"]) for k, v in row.items()}, flush=True)
         del x, y
+
+allgatherv_rows()
 
 # ---------------------------------------------------------------- rooted ops + scan (per-rank payload = nbytes)
 result.update({"bcast": {}, "reduce": {}, "gather": {}, "scatter": {}, "scan": {}})

@@ -403,6 +403,103 @@ b2_k_alltoallv(const __grid_constant__ B2DevComm c, const __grid_constant__ B2Al
 }
 
 // ---------------------------------------------------------------------------
+// allgatherv: every rank contributes a row count that exists only on the device
+//
+// Staging parity of every rank: [header: this rank's clamped row count, in a B2_A2AV_HDR-sized slot so
+// the rows stay 16-byte aligned] [its first n_r rows].  Unlike alltoallv the rows are staged once and
+// every peer reads the same segment from offset 0, so the header holds one count, not P.  After the
+// first wait each CTA reads the P headers and derives the packed offsets, the clipped counts and the
+// loop bound (the largest n_q) -- the same on every rank.
+// ---------------------------------------------------------------------------
+struct B2AllgathervArgs {
+  const void* in;
+  void* out;
+  const long long* count;          // this rank's rows (any value: clamped here)
+  long long* recv_counts;          // [P] rows written from each rank
+  size_t row_bytes;
+  size_t in_rows;                  // N, the same on every rank (sizes the staging and the chunks)
+  size_t out_rows;
+  size_t chunk;
+  int opcode;
+};
+
+__global__ void __launch_bounds__(B2_THREADS, 1)
+b2_k_allgatherv(const __grid_constant__ B2DevComm c, const __grid_constant__ B2AllgathervArgs a) {
+  __shared__ unsigned long long s_cnt[B2_MAX_RANKS];              // n_q: rows rank q staged
+  __shared__ size_t s_dst[B2_MAX_RANKS], s_len[B2_MAX_RANKS];      // bytes
+  __shared__ size_t s_mine, s_nch, s_fill;
+  const unsigned ticket = b2_ticket_read(c.ticket);
+  const size_t par = (size_t)(ticket & 1u) * c.stage_half;
+  unsigned e = b2_ld_volatile(c.epoch + blockIdx.x);
+  const int t = threadIdx.x, P = c.size, r = c.rank;
+  const char* in = (const char*)a.in;
+  char* out = (char*)a.out;
+  char* mine = c.stage[r] + par;
+  const size_t rb = a.row_bytes;
+  // 1. this rank's count, clamped to the rows that exist -> header
+  if (t == 0) {
+    const long long want = *a.count;
+    size_t n = want > 0 ? (size_t)want : 0;
+    if (n > a.in_rows) n = a.in_rows;
+    ((volatile unsigned long long*)mine)[0] = n;
+    s_mine = n * rb;
+  }
+  __syncthreads();
+  const size_t mine_bytes = s_mine;
+  char* mine_rows = mine + B2_A2AV_HDR;
+#define CH_LEN(ch) ((ch) * a.chunk < mine_bytes                                                         \
+                        ? (mine_bytes - (ch) * a.chunk < a.chunk ? mine_bytes - (ch) * a.chunk : a.chunk) \
+                        : (size_t)0)
+  size_t ch = blockIdx.x;
+  b2_copy_bytes<false>(mine_rows + ch * a.chunk, in + ch * a.chunk, CH_LEN(ch));
+  b2_barrier_arrive(c, ++e);
+  unsigned e_cur = e;
+  b2_barrier_wait(c, e_cur, a.opcode);              // every rank's header and chunk blockIdx.x are staged
+  // 2. the P counts (one remote load per thread) and this rank's packed schedule
+  if (t < P) s_cnt[t] = ((const volatile unsigned long long*)(c.stage[t] + par))[0];
+  __syncthreads();
+  if (t == 0) {
+    size_t nmax = 0, filled = 0;
+    for (int q = 0; q < P; ++q) {
+      const size_t n = s_cnt[q];
+      if (n > nmax) nmax = n;
+      const size_t k = n < a.out_rows - filled ? n : a.out_rows - filled;   // clipped to the output rows
+      s_dst[q] = filled * rb;
+      s_len[q] = k * rb;
+      if (blockIdx.x == 0) a.recv_counts[q] = (long long)k;
+      filled += k;
+    }
+    s_fill = filled * rb;
+    s_nch = (nmax * rb + a.chunk - 1) / a.chunk;     // the same on every rank
+  }
+  __syncthreads();
+  // 3. stage -> arrive -> wait -> pull, software-pipelined over the chunks of this CTA; the pull from
+  // peer q is the part of the chunk below c[q] rows, written at q's packed offset
+  const size_t nch = s_nch;
+  for (; ch < nch; ch += gridDim.x) {
+    if (ch != blockIdx.x) b2_barrier_wait(c, e_cur, a.opcode);
+    const size_t off = ch * a.chunk, end = off + a.chunk;
+    for (int s2 = 0; s2 < P; ++s2) {
+      const int q = (s2 + r) % P;                    // stagger peers across ranks
+      const size_t hi = end < s_len[q] ? end : s_len[q];
+      if (off < hi) b2_copy_bytes<true>(out + s_dst[q] + off, c.stage[q] + par + B2_A2AV_HDR + off, hi - off);
+    }
+    const size_t nxt = ch + gridDim.x;
+    if (nxt < nch) {
+      b2_copy_bytes<false>(mine_rows + nxt * a.chunk, in + nxt * a.chunk, CH_LEN(nxt));
+      b2_barrier_arrive(c, ++e);
+      e_cur = e;
+    }
+  }
+#undef CH_LEN
+  // 4. rows past the last received one are zero: the output is fully written on every call
+  a2av_zero(out, s_fill, a.out_rows * rb);
+  __syncthreads();
+  if (t == 0) b2_st_volatile(c.epoch + blockIdx.x, e);
+  b2_finish_bump(c.ticket, c.ticket + 1, 1u, gridDim.x);
+}
+
+// ---------------------------------------------------------------------------
 // NVLS allreduce (SUM; f32 / bf16 / f16 with fp32 accumulation in the switch)
 // ---------------------------------------------------------------------------
 template <int DT>
@@ -744,6 +841,7 @@ extern "C" size_t b2_stage_need(int opcode, int nranks, size_t blk_bytes) {
     case B2_OPC_REDUCE_SCATTER:
       return stride * (size_t)nranks + 4096;
     case B2_OPC_ALLTOALLV:                       // blk_bytes: the most bytes of rows a rank stages
+    case B2_OPC_ALLGATHERV:
       return B2_A2AV_HDR + stride + 4096;
     default:
       return stride + 4096;
@@ -1102,6 +1200,31 @@ extern "C" int b2_alltoallv(B2Comm* c, const void* in, void* out, size_t row_byt
     pick_chunks(c, a.max_rows * row_bytes, coresident_blocks(c, (const void*)b2_k_alltoallv), &a.chunk, &grid);
     b2_k_alltoallv<<<grid, B2_THREADS, 0, stream>>>(c->dev, a);
     rc = b2_launched(c, "alltoallv");
+  }
+  b2_debug_end(dbg, rc);
+  return rc;
+}
+
+// The staging and the chunk geometry come from in_rows, which every rank agrees on; the count is read
+// on the device, so the host never waits for it.
+extern "C" int b2_allgatherv(B2Comm* c, const void* in, void* out, size_t row_bytes, size_t in_rows, size_t out_rows,
+                             const long long* count, long long* recv_counts, cudaStream_t stream) {
+  B2DebugScope* dbg = b2_debug_begin(c, "Allgatherv", stream, "with %zu rows of %zu bytes", in_rows, row_bytes);
+  B2AllgathervArgs a;
+  memset(&a, 0, sizeof a);
+  a.in = in; a.out = out; a.count = count; a.recv_counts = recv_counts;
+  a.row_bytes = row_bytes; a.in_rows = in_rows; a.out_rows = out_rows; a.opcode = B2_OPC_ALLGATHERV;
+  int rc = 0;
+  if (count == nullptr || recv_counts == nullptr) {
+    b2_set_error("allgatherv: count and recv_counts must be device arrays of 1 and %d int64", c->dev.size);
+    rc = B2_ERR_BAD_ARG;
+  }
+  if (rc == 0) rc = check_stage(c, a.opcode, in_rows * row_bytes, "allgatherv");
+  if (rc == 0) {
+    int grid;
+    pick_chunks(c, in_rows * row_bytes, coresident_blocks(c, (const void*)b2_k_allgatherv), &a.chunk, &grid);
+    b2_k_allgatherv<<<grid, B2_THREADS, 0, stream>>>(c->dev, a);
+    rc = b2_launched(c, "allgatherv");
   }
   b2_debug_end(dbg, rc);
   return rc;

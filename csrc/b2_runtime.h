@@ -159,6 +159,13 @@ int b2_scatter(B2Comm* c, const void* in, void* out, size_t blk_bytes, int root,
 int b2_alltoallv(B2Comm* c, const void* in, void* out, size_t row_bytes, size_t in_rows, size_t out_rows,
                  const long long* send_counts, long long* recv_counts, const long long* place_counts,
                  cudaStream_t stream);
+// Variable-count allgather whose counts stay on the device.  `in`: in_rows rows of row_bytes bytes
+// (contiguous, in_rows the same on every rank); `count`: one int64 on the device, clamped to
+// [0, in_rows]; `recv_counts`: [nranks] int64.  The segments of all ranks are packed in rank order and
+// clipped to out_rows; output rows past the last one received are zeroed; recv_counts holds the rows
+// written from each rank.
+int b2_allgatherv(B2Comm* c, const void* in, void* out, size_t row_bytes, size_t in_rows, size_t out_rows,
+                  const long long* count, long long* recv_counts, cudaStream_t stream);
 
 // --- point to point ----------------------------------------------------------
 // source/tag may be -1 (ANY).  `status` is a host-mapped B2StatusRecord or null.

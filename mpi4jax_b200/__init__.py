@@ -1,6 +1,6 @@
 """mpi4jax_b200 -- Hopper-native communication primitives with the API of mpi4jax.
 
-Public namespace (reference: /root/reference/mpi4jax/__init__.py:9-41): the 14 ops and the
+Public namespace (reference: /root/reference/mpi4jax/__init__.py:9-41): the 15 ops and the
 two capability probes, plus what replaces the pieces JAX/mpi4py provided there:
 
 * ``MPI``      communicators, reduction ops, Status, ANY_SOURCE/ANY_TAG (``mpi4py.MPI`` stand-in)
@@ -12,6 +12,7 @@ two capability probes, plus what replaces the pieces JAX/mpi4py provided there:
 from ._version import __version__  # noqa: F401
 from ._src import (  # noqa: F401
     allgather,
+    allgatherv,
     allreduce,
     alltoall,
     alltoallv,
@@ -40,7 +41,7 @@ from ._src.compile_ops import compiled  # noqa: F401  (torch.library / torch.com
 effects_barrier = flush
 
 __all__ = [
-    "allgather", "allreduce", "alltoall", "alltoallv", "barrier", "bcast", "gather", "recv", "reduce",
+    "allgather", "allgatherv", "allreduce", "alltoall", "alltoallv", "barrier", "bcast", "gather", "recv", "reduce",
     "reduce_scatter", "scan", "scatter", "send", "sendrecv", "has_cuda_support", "has_sycl_support",
     "MPI", "jit", "compiled", "flush", "effects_barrier", "linear_transpose", "send_with_grad", "comm_reserve",
     "symmetric_empty", "allreduce_",

@@ -3,7 +3,7 @@
 The reference imports mpi4py first (MPI_Init + finalize-atexit), gates on the JAX version,
 registers the FFI targets and installs an atexit ``flush`` so that pending asynchronous
 custom calls finish before MPI_Finalize.  Here: gate on the torch version, load the native
-library (``native``), import the 14 ops; ``comm`` registers an atexit hook that drains
+library (``native``), import the 15 ops; ``comm`` registers an atexit hook that drains
 every stream / pending isend and tears the symmetric heaps down *before* the process group
 is destroyed (same purpose: no deadlock or crash at interpreter exit,
 tests/collective_ops/test_common.py:91-115 in the reference).
@@ -18,6 +18,7 @@ from . import native  # noqa: E402,F401  (loads libb2mpi.so, applies MPI4JAX_B20
 from . import comm  # noqa: E402,F401   (atexit flush + teardown)
 
 from .collective_ops.allgather import allgather  # noqa: E402,F401
+from .collective_ops.allgatherv import allgatherv  # noqa: E402,F401
 from .collective_ops.allreduce import allreduce  # noqa: E402,F401
 from .collective_ops.alltoall import alltoall  # noqa: E402,F401
 from .collective_ops.alltoallv import alltoallv  # noqa: E402,F401

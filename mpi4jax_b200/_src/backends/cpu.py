@@ -1,4 +1,4 @@
-"""CPU backend: the 14 ops on host tensors over ``torch.distributed`` (gloo).
+"""CPU backend: the 15 ops on host tensors over ``torch.distributed`` (gloo).
 
 Role: what the reference's CPU bridge (mpi_xla_bridge_cpu.cpp, one blocking MPI call
 per op) is to its GPU bridge -- the correctness path that runs anywhere, including the
@@ -186,6 +186,22 @@ def alltoallv(comm: Comm, x: torch.Tensor, send_counts: torch.Tensor, out_rows: 
         out[filled: filled + k] = stack[q, d: d + k]
         recv.append(k)
         filled += k if place is None else slot
+    return out, torch.tensor(recv, dtype=torch.int64)
+
+
+def allgatherv(comm: Comm, x: torch.Tensor, count: torch.Tensor, out_rows: int):
+    """Same rules as the kernel (csrc/b2_collectives.cu: b2_k_allgatherv): everybody gathers every
+    rank's rows and clamped count, then packs the segments in rank order (correctness path)."""
+    n = min(max(int(count), 0), x.shape[0])
+    counts = _gather_stack(comm, torch.tensor(n, dtype=torch.int64)).tolist()
+    stack = _gather_stack(comm, x)                                                      # (P, N, *S)
+    out = torch.zeros((out_rows, *x.shape[1:]), dtype=x.dtype)
+    recv, filled = [], 0
+    for q in range(comm.size):
+        k = min(counts[q], out_rows - filled)
+        out[filled: filled + k] = stack[q, :k]
+        recv.append(k)
+        filled += k
     return out, torch.tensor(recv, dtype=torch.int64)
 
 

@@ -61,14 +61,15 @@ def stage_need(opcode: int, nranks: int, blk_bytes: int) -> int:
     """Staging bytes per parity that an op with ``blk_bytes`` per block needs: the Python twin of
     ``b2_stage_need`` (csrc/b2_collectives.cu), which validates every launch with the same formula."""
     stride = (blk_bytes + 15) & ~15
-    if opcode == codes.OPC_ALLTOALLV:         # a header of the send counts in front of the rows
+    if opcode in (codes.OPC_ALLTOALLV, codes.OPC_ALLGATHERV):    # a header of the counts in front of the rows
         return ALLTOALLV_HEADER + stride + 4096
     mult = nranks if opcode in (codes.OPC_ALLTOALL, codes.OPC_SCATTER, codes.OPC_REDUCE_SCATTER) else 1
     return stride * mult + 4096
 
 
 #: bytes in front of the rows an alltoallv stages: the rank's clamped send counts, one int64 per possible
-#: rank (B2_A2AV_HDR; MAX_RANKS is checked against the library at import)
+#: rank (B2_A2AV_HDR; MAX_RANKS is checked against the library at import).  allgatherv reuses the slot
+#: for its one count, which keeps the rows 16-byte aligned
 ALLTOALLV_HEADER = native.MAX_RANKS * 8
 
 
@@ -569,6 +570,20 @@ class NativeComm:
         self._check(rc, "Alltoallv")
         return out, recv_counts
 
+    def allgatherv(self, x: torch.Tensor, count: torch.Tensor, out_rows: int):
+        """``(out, recv_counts)``: the first ``count`` rows of every rank's ``x``, packed in rank order
+        (``collective_ops/allgatherv.py`` states the rules); the count is read on the device."""
+        x = _prep(x)
+        row_bytes = math.prod(x.shape[1:]) * x.element_size()
+        out = torch.empty((out_rows, *x.shape[1:]), dtype=x.dtype, device=x.device)
+        recv_counts = torch.empty(self.comm.size, dtype=torch.int64, device=x.device)
+        count = count.to(torch.int64).contiguous()
+        self.ensure_stage(codes.OPC_ALLGATHERV, x.shape[0] * row_bytes)
+        rc = _lib().b2_allgatherv(self.handle, x.data_ptr(), out.data_ptr(), row_bytes, x.shape[0], out_rows,
+                                  count.data_ptr(), recv_counts.data_ptr(), self._stream())
+        self._check(rc, "Allgatherv")
+        return out, recv_counts
+
     # -- point to point ------------------------------------------------------------
     def _status_record(self, status: Optional[Status], itemsize: int):
         if status is None:
@@ -679,7 +694,8 @@ def _nvtx_wrap(name: str, fn):
 #: ``MPI4JAX_B200_NVTX=1``: one NVTX range per op (visible in Nsight Systems timelines); the
 #: methods are left untouched otherwise, so the fast path pays nothing (SURVEY 5.1)
 NVTX_OPS = ("barrier", "allreduce", "reduce", "scan", "allgather", "alltoall", "bcast", "gather", "scatter",
-            "send", "recv", "sendrecv", "reduce_scatter", "alltoallv", "gemm_allreduce", "halo_exchange")
+            "send", "recv", "sendrecv", "reduce_scatter", "alltoallv", "allgatherv", "gemm_allreduce",
+            "halo_exchange")
 if env_flag("MPI4JAX_B200_NVTX", False):
     for _name in NVTX_OPS:
         setattr(NativeComm, _name, _nvtx_wrap(_name, getattr(NativeComm, _name)))

@@ -9,7 +9,7 @@ fallback, never the default on one node:
   needs peer-mapped HBM, i.e. one NVLink domain), with a one-time warning;
 * forced by ``MPI4JAX_B200_TRANSPORT=host`` or the reference's ``MPI4JAX_USE_CUDA_MPI=0``.
 
-Same method surface as ``backends.cuda.NativeComm`` for the 14 ops; the fused / H100-only entry
+Same method surface as ``backends.cuda.NativeComm`` for the 15 ops; the fused / H100-only entry
 points (halo exchange, GEMM+allreduce) raise.  Ops synchronise the stream and block the host, so
 they cannot be captured into CUDA graphs: ``mpi4jax_b200.jit`` runs such functions eagerly.
 """
@@ -53,7 +53,7 @@ class HostStagedComm:
 
     def _unsupported(self, what: str):
         raise MPIError(f"{what} needs the native NVLink transport, but this communicator uses host "
-                       f"staging ({self.reason or 'requested'}); use the 14 primitives instead")
+                       f"staging ({self.reason or 'requested'}); use the 15 primitives instead")
 
     # -- lifecycle (NativeComm surface) ---------------------------------------------
     def flush(self) -> None:
@@ -66,7 +66,7 @@ class HostStagedComm:
     def destroy(self) -> None:
         pass
 
-    # -- the 14 ops ------------------------------------------------------------------
+    # -- the 15 ops ------------------------------------------------------------------
     def barrier(self) -> None:
         self.flush()                      # the reference: stream sync, then MPI_Barrier (cuda.cpp:75-86)
         _cpu.barrier(self.comm)
@@ -92,6 +92,10 @@ class HostStagedComm:
     def alltoallv(self, x, send_counts, out_rows: int, place_counts=None):
         out, recv_counts = _cpu.alltoallv(self.comm, self._down(x), self._down(send_counts), out_rows,
                                           None if place_counts is None else self._down(place_counts))
+        return self._up(out, x), self._up(recv_counts, x)
+
+    def allgatherv(self, x, count, out_rows: int):
+        out, recv_counts = _cpu.allgatherv(self.comm, self._down(x), self._down(count), out_rows)
         return self._up(out, x), self._up(recv_counts, x)
 
     def bcast(self, x, root: int):

@@ -1,4 +1,4 @@
-"""Backend dispatch for the 14 ops: CUDA tensors -> native kernels, CPU tensors -> gloo.
+"""Backend dispatch for the 15 ops: CUDA tensors -> native kernels, CPU tensors -> gloo.
 
 This is the analogue of the per-platform lowering registration each reference op does
 (``register_lowering(..., platform="cpu"|"cuda"|"xpu")``, e.g.
@@ -178,6 +178,37 @@ def alltoallv(comm: Comm, x: torch.Tensor, send_counts: torch.Tensor, out_rows: 
     row_bytes = math.prod(x.shape[1:]) * x.element_size()
     done = _log(comm, "Alltoallv", f"with {x.shape[0]} rows of {row_bytes} bytes")
     out = _cpu.alltoallv(comm, x, send_counts, out_rows, place_counts)
+    if done:
+        done()
+    return out
+
+
+def check_allgatherv_args(x: torch.Tensor, count: torch.Tensor, out_rows: int) -> None:
+    """Host-side checks of an allgatherv call.  Every entry point (the op, ``compiled.allgatherv``, the raw
+    ``torch.ops`` op and its fake kernel, the backends) passes through them: the kernel dereferences the
+    count as one int64 value in x's device memory, so anything else must be refused before the launch."""
+    if x.dim() == 0:
+        raise ValueError("Allgatherv input must have shape (rows, ...)")
+    if not isinstance(count, torch.Tensor):
+        raise TypeError(f"Allgatherv count must be an integer tensor (got {type(count).__name__})")
+    if count.dtype.is_floating_point or count.dtype.is_complex or count.dtype == torch.bool:
+        raise TypeError(f"Allgatherv count must be an integer tensor (got {count.dtype})")
+    if count.dim() != 0:
+        raise ValueError(f"Allgatherv count must have shape () (got {tuple(count.shape)})")
+    if count.device != x.device:
+        raise ValueError(f"Allgatherv count must live on the device of x ({x.device}, got {count.device})")
+    if out_rows < 0:
+        raise ValueError(f"Allgatherv recv_capacity must be >= 0 (got {out_rows})")
+
+
+def allgatherv(comm: Comm, x: torch.Tensor, count: torch.Tensor, out_rows: int):
+    _plain(x)
+    check_allgatherv_args(x, count, out_rows)
+    if x.is_cuda:
+        return comm._native_comm().allgatherv(x, count, out_rows)
+    row_bytes = math.prod(x.shape[1:]) * x.element_size()
+    done = _log(comm, "Allgatherv", f"with {x.shape[0]} rows of {row_bytes} bytes")
+    out = _cpu.allgatherv(comm, x, count, out_rows)
     if done:
         done()
     return out

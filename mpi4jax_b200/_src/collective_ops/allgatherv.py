@@ -1,0 +1,127 @@
+"""allgatherv -- a variable-count allgather whose counts stay on the device.
+
+``MPI_Allgatherv`` for rows whose number is known only on the GPU (top-k gradients, tokens or particles
+that survive a device-side filter): every rank contributes the first ``count`` rows of its input and
+every rank receives all of them, packed in rank order into an output of static capacity.  The count
+is a device tensor, so the host never waits for it and the call can be captured into a CUDA graph and
+replayed with other counts.  Extension: the reference has no allgatherv.
+
+Rules, on rank r of P (``x_r`` has shape ``(N, *S)``; ``N``, ``S`` and the dtype are the same on every
+rank; capacity ``C_r``, which may differ between ranks):
+
+* contributed: ``n_r = clamp(count_r, 0, N)`` rows, rows ``[0, n_r)`` of ``x_r``;
+* received: ``c[q] = clamp(C_r - sum_{p<q} c[p], 0, n_q)`` rows from rank q land at row
+  ``sum_{p<q} c[p]`` -- segments packed in source-rank order, a segment that does not fit loses its
+  tail; rows past ``sum_q c[q]`` are zero.  ``recv_counts`` = ``c`` (int64, on x's device).
+
+An invalid count is never an error and never makes the kernel read or write out of bounds.
+
+GPU: every rank stages its ``n_r`` rows once, behind a header holding ``n_r``; after one barrier each
+CTA reads the P headers, derives the packed offsets itself and pulls its chunks of every peer's segment
+straight into the output (csrc/b2_collectives.cu: b2_k_allgatherv).  Differentiable: the adjoint (SUM)
+cuts every received segment out of the cotangent into a ``(P, N, *S)`` tensor, zero-padded, and
+reduce-scatters it, so rank r gets the rank-order sum of what the receivers kept of its rows.
+"""
+
+from __future__ import annotations
+
+import operator
+
+import numpy as np
+import torch
+
+from ..comm import SUM, Comm
+from ..utils import (NOTSET, as_tensor, check_dtype, get_default_comm, needs_autograd,
+                     raise_if_token_is_set)
+from ..validation import enforce_types
+from . import _dispatch
+
+
+def segments(g: torch.Tensor, recv_counts: torch.Tensor, rows: int) -> torch.Tensor:
+    """``G`` of shape ``(P, rows, *S)`` with ``G[q, i] = g[o[q] + i]`` for ``i < recv_counts[q]`` and 0
+    otherwise, where ``o`` is the exclusive prefix sum of ``recv_counts``: the segments of an allgatherv
+    output, each back at the start of its source's rows.  Device ops only (no host read of the counts);
+    differentiable in ``g``."""
+    P = recv_counts.shape[0]
+    offsets = torch.cumsum(recv_counts, 0) - recv_counts
+    i = torch.arange(rows, device=g.device)
+    # entries past a segment read a zero row appended to g (index g.shape[0])
+    idx = torch.where(i < recv_counts.view(P, 1), offsets.view(P, 1) + i, g.shape[0])
+    padded = torch.cat([g, g.new_zeros((1, *g.shape[1:]))])
+    return padded[idx]
+
+
+class _Allgatherv(torch.autograd.Function):
+    @staticmethod
+    def forward(x, count, out_rows, comm):
+        return _dispatch.allgatherv(comm, x, count, out_rows)
+
+    @staticmethod
+    def setup_context(ctx, inputs, output):
+        x, ctx.count, ctx.out_rows, ctx.comm = inputs
+        ctx.in_rows = x.shape[0]
+        ctx.mark_non_differentiable(output[1])
+        ctx.save_for_backward(output[1])
+
+    @staticmethod
+    def backward(ctx, g, _g_counts):
+        from .reduce_scatter import reduce_scatter      # the differentiable op: double backward works
+
+        (recv_counts,) = ctx.saved_tensors
+        return reduce_scatter(segments(g, recv_counts, ctx.in_rows), SUM, comm=ctx.comm), None, None, None
+
+    @staticmethod
+    def jvp(ctx, x_t, *_):
+        out_t, _counts = _Allgatherv.apply(x_t, ctx.count, ctx.out_rows, ctx.comm)
+        return out_t, None
+
+    @staticmethod
+    def vmap(info, in_dims, x, count, out_rows, comm):
+        if in_dims[1] is not None:
+            raise ValueError("allgatherv under vmap: the count must not be batched (one exchange moves every "
+                             "batch entry)")
+        if in_dims[0] is None:
+            return _Allgatherv.apply(x, count, out_rows, comm), (None, None)
+        # keep the row axis in front: (B, N, *S) -> (N, B, *S), gathered as one message of B-times larger rows
+        out, counts = _Allgatherv.apply(x.movedim(in_dims[0], 1).contiguous(), count, out_rows, comm)
+        return (out, counts), (1, None)
+
+
+def _as_count(count, x: torch.Tensor) -> torch.Tensor:
+    """A Python int becomes an int64 scalar tensor on x's device; tensors are checked, not moved."""
+    if isinstance(count, torch.Tensor):
+        return count
+    return torch.tensor(operator.index(count), dtype=torch.int64, device=x.device)
+
+
+@enforce_types(recv_capacity=(type(None), np.integer), comm=(type(None), Comm))
+def allgatherv(x, count, *, recv_capacity=None, comm=None, token=NOTSET):
+    """Perform a variable-count allgather operation (``MPI_Allgatherv``) with a device-resident count.
+
+    Arguments:
+        x: input of shape ``(N, ...)``; ``N``, the row shape and the dtype must be the same on every rank.
+        count: rows this rank contributes, taken from the start of ``x``: a Python int or an integer
+            tensor of shape ``()`` on ``x``'s device.  Negative counts contribute nothing, counts past
+            ``N`` are cut at ``N``.
+        recv_capacity: rows of the output (default ``N * nproc``, which never drops a row; may differ
+            between ranks).  A segment that does not fit loses its last rows.
+        comm: the communicator (defaults to a clone of ``COMM_WORLD``).
+
+    Returns:
+        Tuple[Tensor, Tensor]: every rank's rows, shape ``(recv_capacity, ...)``, packed in rank order
+        and zero past the last one, and ``recv_counts``, int64 ``(nproc,)`` on the device: the rows
+        written from each rank.
+    """
+    raise_if_token_is_set(token)
+    if comm is None:
+        comm = get_default_comm()
+    x = as_tensor(x, comm)
+    check_dtype(x)
+    if x.dim() == 0:
+        raise ValueError("Allgatherv input must have shape (rows, ...)")
+    count = _as_count(count, x)
+    cap = x.shape[0] * comm.Get_size() if recv_capacity is None else int(recv_capacity)
+    _dispatch.check_allgatherv_args(x, count, cap)
+    if not needs_autograd(x):
+        return _dispatch.allgatherv(comm, x, count, cap)
+    return _Allgatherv.apply(x, count, cap, comm)

@@ -1,4 +1,4 @@
-"""``torch.library`` registration of the 14 ops -- the traceable frontend.
+"""``torch.library`` registration of the 15 ops -- the traceable frontend.
 
 The reference's ops are JAX *primitives*: abstract-eval rules give shapes, an ordered effect
 threads a token through every custom call so XLA keeps them in program order
@@ -28,6 +28,7 @@ from torch.library import custom_op
 
 from . import comm as _comm_mod
 from .collective_ops import _dispatch
+from .collective_ops.allgatherv import segments
 from .comm import ANY_SOURCE, ANY_TAG, SUM, Comm, as_op
 from .native import codes
 from .utils import get_default_comm
@@ -184,6 +185,33 @@ def _alltoallv_backward(ctx, g, _g_counts):
 _alltoallv.register_autograd(_alltoallv_backward, setup_context=_alltoallv_setup)
 
 
+@custom_op("mpi4jax_b200::allgatherv", mutates_args=())
+def _allgatherv(x: torch.Tensor, count: torch.Tensor, out_rows: int, comm_id: int) -> tuple[torch.Tensor, torch.Tensor]:
+    return _dispatch.allgatherv(_c(comm_id), x.contiguous(), count, out_rows)
+
+
+@_allgatherv.register_fake
+def _(x, count, out_rows, comm_id):
+    _dispatch.check_allgatherv_args(x, count, out_rows)
+    return x.new_empty((out_rows, *x.shape[1:])), x.new_empty((_c(comm_id).Get_size(),), dtype=torch.int64)
+
+
+def _allgatherv_setup(ctx, inputs, output):
+    x, _, _, ctx.comm_id = inputs
+    ctx.in_rows = x.shape[0]
+    ctx.save_for_backward(output[1])
+
+
+def _allgatherv_backward(ctx, g, _g_counts):
+    # SUM adjoint (collective_ops/allgatherv.py): the received segments, zero-padded to (P, N, ...), reduce-scattered
+    (recv_counts,) = ctx.saved_tensors
+    G = segments(g.contiguous(), recv_counts, ctx.in_rows)
+    return torch.ops.mpi4jax_b200.reduce_scatter(G, SUM.code, ctx.comm_id), None, None, None
+
+
+_allgatherv.register_autograd(_allgatherv_backward, setup_context=_allgatherv_setup)
+
+
 @custom_op("mpi4jax_b200::bcast", mutates_args=())
 def _bcast(x: torch.Tensor, root: int, comm_id: int) -> torch.Tensor:
     out = _dispatch.bcast(_c(comm_id), x.contiguous(), root)
@@ -325,7 +353,7 @@ _sendrecv.register_autograd(_sendrecv_backward, setup_context=_sendrecv_setup)
 
 
 ALL_OPS = ("allreduce", "allgather", "alltoall", "bcast", "scan", "reduce", "gather_root", "gather_leaf",
-           "scatter", "barrier", "send", "recv", "sendrecv", "reduce_scatter", "alltoallv")
+           "scatter", "barrier", "send", "recv", "sendrecv", "reduce_scatter", "alltoallv", "allgatherv")
 ORDERED_EFFECT = False
 try:  # the ordered effect: AOTAutograd threads a token through these ops in program order
     from torch._higher_order_ops.effects import _EffectType, _register_effectful_op
@@ -371,6 +399,17 @@ class compiled:
         cap = x.shape[0] * comm.Get_size() if recv_capacity is None else recv_capacity
         _dispatch.check_alltoallv_args(comm, x, send_counts, cap)
         return torch.ops.mpi4jax_b200.alltoallv(x, send_counts, cap, None, comm._id)
+
+    @staticmethod
+    def allgatherv(x, count, *, recv_capacity=None, comm=None):
+        """``(out, recv_counts)`` of :func:`mpi4jax_b200.allgatherv`; ``count`` must be an integer device
+        tensor of shape ``()``."""
+        comm = comm or get_default_comm()
+        if x.dim() == 0:
+            raise ValueError("Allgatherv input must have shape (rows, ...)")
+        cap = x.shape[0] * comm.Get_size() if recv_capacity is None else recv_capacity
+        _dispatch.check_allgatherv_args(x, count, cap)
+        return torch.ops.mpi4jax_b200.allgatherv(x, count, cap, comm._id)
 
     @staticmethod
     def bcast(x, root, *, comm=None):

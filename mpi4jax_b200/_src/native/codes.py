@@ -43,5 +43,6 @@ OPC_ALLREDUCE, OPC_REDUCE, OPC_SCAN, OPC_ALLGATHER, OPC_ALLTOALL = 1, 2, 3, 4, 5
 OPC_BCAST, OPC_GATHER, OPC_SCATTER = 6, 7, 8
 OPC_REDUCE_SCATTER = 13
 OPC_ALLTOALLV = 14
+OPC_ALLGATHERV = 15
 
 ANY = -1  # ANY_SOURCE / ANY_TAG on the wire

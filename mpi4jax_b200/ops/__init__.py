@@ -1,9 +1,9 @@
-"""Functional op namespace: the 14 primitives plus the fused ops that go beyond the
+"""Functional op namespace: the 15 primitives plus the fused ops that go beyond the
 reference's one-MPI-call-per-op model (fused multi-field halo exchange)."""
 
 from .._src import (  # noqa: F401
-    allgather, allreduce, alltoall, alltoallv, barrier, bcast, gather, recv, reduce, reduce_scatter, scan, scatter,
-    send, send_with_grad, sendrecv,
+    allgather, allgatherv, allreduce, alltoall, alltoallv, barrier, bcast, gather, recv, reduce, reduce_scatter,
+    scan, scatter, send, send_with_grad, sendrecv,
 )
 from .halo import halo_exchange  # noqa: F401
 from .linear import linear_allreduce  # noqa: F401
