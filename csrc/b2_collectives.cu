@@ -261,14 +261,20 @@ b2_k_move(const __grid_constant__ B2DevComm c, const __grid_constant__ B2MoveArg
 }
 
 // ---------------------------------------------------------------------------
-// alltoallv: row counts that exist only on the device
+// alltoallv / allgatherv: row counts that exist only on the device
 //
-// Staging parity of every rank: [header: this rank's clamped send counts, int64 x B2_MAX_RANKS]
-// [the rows it sends, in destination order].  Every CTA writes the header (identical values) before
-// its first arrive, so after the first wait each CTA reads the P x P count matrix from the peers and
-// derives the whole schedule locally -- the same on every rank.  Chunk k indexes bytes of every rank's
-// staged rows and belongs to CTA k mod grid everywhere, as in b2_k_move; the pull of chunk k from
-// peer q is its intersection with q's segment for this rank.
+// Staging parity of every rank: [header: this rank's clamped counts, int64 x B2_MAX_RANKS]
+// [the rows it stages].  Every CTA writes the header (identical values) before its first arrive, so
+// after the first wait each CTA reads the peers' headers and derives the whole schedule locally -- the
+// same on every rank.  Chunk k indexes bytes of every rank's staged rows and belongs to CTA k mod grid
+// everywhere, as in b2_k_move; the pull of chunk k from peer q is its intersection with q's segment
+// for this rank.
+//
+// alltoallv: the header holds P send counts and the rows follow in destination order, so peer q's
+// segment for rank r starts after q's rows for the ranks below r.
+// allgatherv (`count` set, "gather mode"): the header holds one count in slot 0 and the rows are staged
+// once -- every rank reads the same segment, from source offset 0.  Only the header write and the
+// schedule (thread-0 code) know the mode; chunks, pulls and the zero fill are shared.
 // ---------------------------------------------------------------------------
 #define B2_A2AV_HDR ((size_t)B2_MAX_RANKS * sizeof(long long))
 
@@ -277,6 +283,7 @@ struct B2AlltoallvArgs {
   void* out;
   const long long* send_counts;    // [P] rows to each rank (any value: clamped here)
   const long long* place_counts;   // [P] reverse mode: where the segments land (null: packed, forward)
+  const long long* count;          // gather mode: the rows this rank sends to every rank (null: alltoallv)
   long long* recv_counts;          // [P] rows written from each rank
   size_t row_bytes;
   size_t in_rows;
@@ -303,26 +310,28 @@ __device__ __forceinline__ void a2av_zero(char* out, size_t lo, size_t hi) {
 }
 
 __global__ void __launch_bounds__(B2_THREADS, 1)
-b2_k_alltoallv(const __grid_constant__ B2DevComm c, const __grid_constant__ B2AlltoallvArgs a) {
-  __shared__ unsigned long long s_cnt[B2_MAX_RANKS][B2_MAX_RANKS];   // [q][p]: rows rank q sends to p
+b2_k_rowsv(const __grid_constant__ B2DevComm c, const __grid_constant__ B2AlltoallvArgs a) {
+  __shared__ unsigned long long s_cnt[B2_MAX_RANKS][B2_MAX_RANKS];   // [q][p]: rows q sends to p (gather: [q][0])
   __shared__ size_t s_src[B2_MAX_RANKS], s_dst[B2_MAX_RANKS], s_len[B2_MAX_RANKS];   // bytes
-  __shared__ size_t s_gap[B2_MAX_RANKS + 1][2];                    // output bytes nobody writes
+  __shared__ size_t s_gap[B2_MAX_RANKS + 1][2];                    // output bytes nobody writes (non-empty)
   __shared__ size_t s_mine, s_nch;
+  __shared__ int s_ngap;
   const unsigned ticket = b2_ticket_read(c.ticket);
   const size_t par = (size_t)(ticket & 1u) * c.stage_half;
   unsigned e = b2_ld_volatile(c.epoch + blockIdx.x);
   const int t = threadIdx.x, P = c.size, r = c.rank;
+  const bool gather = a.count != nullptr;
   const char* in = (const char*)a.in;
   char* out = (char*)a.out;
   char* mine = c.stage[r] + par;
   const size_t rb = a.row_bytes;
-  // 1. this rank's send counts, clamped in rank order to the rows that exist -> header
+  // 1. this rank's counts, clamped in rank order to the rows that exist -> header
   if (t == 0) {
     const size_t n = a.in_rows < a.max_rows ? a.in_rows : a.max_rows;
+    const long long* want = gather ? a.count : a.send_counts;
     size_t used = 0;
-    for (int q = 0; q < P; ++q) {
-      const long long want = a.send_counts[q];
-      size_t s = want > 0 ? (size_t)want : 0;
+    for (int q = 0; q < (gather ? 1 : P); ++q) {
+      size_t s = want[q] > 0 ? (size_t)want[q] : 0;
       if (s > n - used) s = n - used;
       used += s;
       ((volatile unsigned long long*)mine)[q] = s;
@@ -340,21 +349,33 @@ b2_k_alltoallv(const __grid_constant__ B2DevComm c, const __grid_constant__ B2Al
   b2_barrier_arrive(c, ++e);
   unsigned e_cur = e;
   b2_barrier_wait(c, e_cur, a.opcode);              // every rank's header and chunk blockIdx.x are staged
-  // 2. the count matrix and this rank's receive schedule
-  if (t < P * P) s_cnt[t / P][t % P] = ((const volatile unsigned long long*)(c.stage[t / P] + par))[t % P];
+  // 2. the peers' headers and this rank's receive schedule
+  if (gather) {
+    if (t < P) s_cnt[t][0] = ((const volatile unsigned long long*)(c.stage[t] + par))[0];
+  } else if (t < P * P) {
+    s_cnt[t / P][t % P] = ((const volatile unsigned long long*)(c.stage[t / P] + par))[t % P];
+  }
   __syncthreads();
   if (t == 0) {
     size_t smax = 0, filled = 0;
+    int ng = 0;
     for (int q = 0; q < P; ++q) {
-      size_t tot = 0, d = 0;
-      for (int p = 0; p < P; ++p) {
-        if (p == r) d = tot;
-        tot += s_cnt[q][p];
+      // q's staged rows, the first of them it sends to this rank (gather: 0), and how many
+      size_t tot, d = 0, k;
+      if (gather) {
+        tot = k = s_cnt[q][0];
+      } else {
+        tot = 0;
+        for (int p = 0; p < P; ++p) {
+          if (p == r) d = tot;
+          tot += s_cnt[q][p];
+        }
+        k = s_cnt[q][r];
       }
       if (tot > smax) smax = tot;
       // forward: packed in source order, clipped to the output rows; reverse: at the sum of the
       // (clamped) place counts of the lower ranks, at most place_counts[q] rows
-      size_t k = s_cnt[q][r], slot = a.out_rows - filled;
+      size_t slot = a.out_rows - filled;
       if (a.place_counts != nullptr) {
         const long long w = a.place_counts[q];
         if (w < 0) slot = 0;
@@ -365,13 +386,20 @@ b2_k_alltoallv(const __grid_constant__ B2DevComm c, const __grid_constant__ B2Al
       s_src[q] = d * rb;
       s_dst[q] = filled * rb;
       s_len[q] = k * rb;
-      s_gap[q][0] = (filled + k) * rb;
-      s_gap[q][1] = (filled + slot) * rb;
+      if (slot > k) {
+        s_gap[ng][0] = (filled + k) * rb;
+        s_gap[ng][1] = (filled + slot) * rb;
+        ++ng;
+      }
       if (blockIdx.x == 0) a.recv_counts[q] = (long long)k;
       filled += slot;
     }
-    s_gap[P][0] = filled * rb;
-    s_gap[P][1] = a.out_rows * rb;
+    if (a.out_rows > filled) {
+      s_gap[ng][0] = filled * rb;
+      s_gap[ng][1] = a.out_rows * rb;
+      ++ng;
+    }
+    s_ngap = ng;
     s_nch = (smax * rb + a.chunk - 1) / a.chunk;     // the same on every rank
   }
   __syncthreads();
@@ -396,104 +424,7 @@ b2_k_alltoallv(const __grid_constant__ B2DevComm c, const __grid_constant__ B2Al
   }
 #undef CH_LEN
   // 4. rows nobody sends are zero: the output is fully written on every call
-  for (int q = 0; q <= P; ++q) a2av_zero(out, s_gap[q][0], s_gap[q][1]);
-  __syncthreads();
-  if (t == 0) b2_st_volatile(c.epoch + blockIdx.x, e);
-  b2_finish_bump(c.ticket, c.ticket + 1, 1u, gridDim.x);
-}
-
-// ---------------------------------------------------------------------------
-// allgatherv: every rank contributes a row count that exists only on the device
-//
-// Staging parity of every rank: [header: this rank's clamped row count, in a B2_A2AV_HDR-sized slot so
-// the rows stay 16-byte aligned] [its first n_r rows].  Unlike alltoallv the rows are staged once and
-// every peer reads the same segment from offset 0, so the header holds one count, not P.  After the
-// first wait each CTA reads the P headers and derives the packed offsets, the clipped counts and the
-// loop bound (the largest n_q) -- the same on every rank.
-// ---------------------------------------------------------------------------
-struct B2AllgathervArgs {
-  const void* in;
-  void* out;
-  const long long* count;          // this rank's rows (any value: clamped here)
-  long long* recv_counts;          // [P] rows written from each rank
-  size_t row_bytes;
-  size_t in_rows;                  // N, the same on every rank (sizes the staging and the chunks)
-  size_t out_rows;
-  size_t chunk;
-  int opcode;
-};
-
-__global__ void __launch_bounds__(B2_THREADS, 1)
-b2_k_allgatherv(const __grid_constant__ B2DevComm c, const __grid_constant__ B2AllgathervArgs a) {
-  __shared__ unsigned long long s_cnt[B2_MAX_RANKS];              // n_q: rows rank q staged
-  __shared__ size_t s_dst[B2_MAX_RANKS], s_len[B2_MAX_RANKS];      // bytes
-  __shared__ size_t s_mine, s_nch, s_fill;
-  const unsigned ticket = b2_ticket_read(c.ticket);
-  const size_t par = (size_t)(ticket & 1u) * c.stage_half;
-  unsigned e = b2_ld_volatile(c.epoch + blockIdx.x);
-  const int t = threadIdx.x, P = c.size, r = c.rank;
-  const char* in = (const char*)a.in;
-  char* out = (char*)a.out;
-  char* mine = c.stage[r] + par;
-  const size_t rb = a.row_bytes;
-  // 1. this rank's count, clamped to the rows that exist -> header
-  if (t == 0) {
-    const long long want = *a.count;
-    size_t n = want > 0 ? (size_t)want : 0;
-    if (n > a.in_rows) n = a.in_rows;
-    ((volatile unsigned long long*)mine)[0] = n;
-    s_mine = n * rb;
-  }
-  __syncthreads();
-  const size_t mine_bytes = s_mine;
-  char* mine_rows = mine + B2_A2AV_HDR;
-#define CH_LEN(ch) ((ch) * a.chunk < mine_bytes                                                         \
-                        ? (mine_bytes - (ch) * a.chunk < a.chunk ? mine_bytes - (ch) * a.chunk : a.chunk) \
-                        : (size_t)0)
-  size_t ch = blockIdx.x;
-  b2_copy_bytes<false>(mine_rows + ch * a.chunk, in + ch * a.chunk, CH_LEN(ch));
-  b2_barrier_arrive(c, ++e);
-  unsigned e_cur = e;
-  b2_barrier_wait(c, e_cur, a.opcode);              // every rank's header and chunk blockIdx.x are staged
-  // 2. the P counts (one remote load per thread) and this rank's packed schedule
-  if (t < P) s_cnt[t] = ((const volatile unsigned long long*)(c.stage[t] + par))[0];
-  __syncthreads();
-  if (t == 0) {
-    size_t nmax = 0, filled = 0;
-    for (int q = 0; q < P; ++q) {
-      const size_t n = s_cnt[q];
-      if (n > nmax) nmax = n;
-      const size_t k = n < a.out_rows - filled ? n : a.out_rows - filled;   // clipped to the output rows
-      s_dst[q] = filled * rb;
-      s_len[q] = k * rb;
-      if (blockIdx.x == 0) a.recv_counts[q] = (long long)k;
-      filled += k;
-    }
-    s_fill = filled * rb;
-    s_nch = (nmax * rb + a.chunk - 1) / a.chunk;     // the same on every rank
-  }
-  __syncthreads();
-  // 3. stage -> arrive -> wait -> pull, software-pipelined over the chunks of this CTA; the pull from
-  // peer q is the part of the chunk below c[q] rows, written at q's packed offset
-  const size_t nch = s_nch;
-  for (; ch < nch; ch += gridDim.x) {
-    if (ch != blockIdx.x) b2_barrier_wait(c, e_cur, a.opcode);
-    const size_t off = ch * a.chunk, end = off + a.chunk;
-    for (int s2 = 0; s2 < P; ++s2) {
-      const int q = (s2 + r) % P;                    // stagger peers across ranks
-      const size_t hi = end < s_len[q] ? end : s_len[q];
-      if (off < hi) b2_copy_bytes<true>(out + s_dst[q] + off, c.stage[q] + par + B2_A2AV_HDR + off, hi - off);
-    }
-    const size_t nxt = ch + gridDim.x;
-    if (nxt < nch) {
-      b2_copy_bytes<false>(mine_rows + nxt * a.chunk, in + nxt * a.chunk, CH_LEN(nxt));
-      b2_barrier_arrive(c, ++e);
-      e_cur = e;
-    }
-  }
-#undef CH_LEN
-  // 4. rows past the last received one are zero: the output is fully written on every call
-  a2av_zero(out, s_fill, a.out_rows * rb);
+  for (int g = 0; g < s_ngap; ++g) a2av_zero(out, s_gap[g][0], s_gap[g][1]);
   __syncthreads();
   if (t == 0) b2_st_volatile(c.epoch + blockIdx.x, e);
   b2_finish_bump(c.ticket, c.ticket + 1, 1u, gridDim.x);
@@ -1177,9 +1108,19 @@ extern "C" int b2_scatter(B2Comm* c, const void* in, void* out, size_t blk_bytes
   return rc;
 }
 
-// The launch geometry depends only on sizes every rank agrees on: the forward's input rows (the same
-// everywhere) or, in reverse mode, nranks x its output rows (the forward's input rows again).  The
-// counts are read on the device, so the host never waits for them.
+// The staging and the launch geometry come from a.max_rows, which every rank agrees on: the input
+// rows (the same everywhere) or, in alltoallv's reverse mode, nranks x its output rows (the forward's
+// input rows again).  The counts are read on the device, so the host never waits for them.
+static int rowsv_launch(B2Comm* c, B2AlltoallvArgs& a, const char* name, cudaStream_t stream) {
+  const size_t stage_bytes = a.max_rows * a.row_bytes;
+  int rc = check_stage(c, a.opcode, stage_bytes, name);
+  if (rc) return rc;
+  int grid;
+  pick_chunks(c, stage_bytes, coresident_blocks(c, (const void*)b2_k_rowsv), &a.chunk, &grid);
+  b2_k_rowsv<<<grid, B2_THREADS, 0, stream>>>(c->dev, a);
+  return b2_launched(c, name);
+}
+
 extern "C" int b2_alltoallv(B2Comm* c, const void* in, void* out, size_t row_bytes, size_t in_rows, size_t out_rows,
                             const long long* send_counts, long long* recv_counts, const long long* place_counts,
                             cudaStream_t stream) {
@@ -1189,42 +1130,31 @@ extern "C" int b2_alltoallv(B2Comm* c, const void* in, void* out, size_t row_byt
   a.in = in; a.out = out; a.send_counts = send_counts; a.place_counts = place_counts; a.recv_counts = recv_counts;
   a.row_bytes = row_bytes; a.in_rows = in_rows; a.out_rows = out_rows; a.opcode = B2_OPC_ALLTOALLV;
   a.max_rows = place_counts == nullptr ? in_rows : (size_t)c->dev.size * out_rows;
-  int rc = 0;
+  int rc;
   if (send_counts == nullptr || recv_counts == nullptr) {
     b2_set_error("alltoallv: send_counts and recv_counts must be device arrays of %d int64", c->dev.size);
     rc = B2_ERR_BAD_ARG;
-  }
-  if (rc == 0) rc = check_stage(c, a.opcode, a.max_rows * row_bytes, "alltoallv");
-  if (rc == 0) {
-    int grid;
-    pick_chunks(c, a.max_rows * row_bytes, coresident_blocks(c, (const void*)b2_k_alltoallv), &a.chunk, &grid);
-    b2_k_alltoallv<<<grid, B2_THREADS, 0, stream>>>(c->dev, a);
-    rc = b2_launched(c, "alltoallv");
+  } else {
+    rc = rowsv_launch(c, a, "alltoallv", stream);
   }
   b2_debug_end(dbg, rc);
   return rc;
 }
 
-// The staging and the chunk geometry come from in_rows, which every rank agrees on; the count is read
-// on the device, so the host never waits for it.
 extern "C" int b2_allgatherv(B2Comm* c, const void* in, void* out, size_t row_bytes, size_t in_rows, size_t out_rows,
                              const long long* count, long long* recv_counts, cudaStream_t stream) {
   B2DebugScope* dbg = b2_debug_begin(c, "Allgatherv", stream, "with %zu rows of %zu bytes", in_rows, row_bytes);
-  B2AllgathervArgs a;
+  B2AlltoallvArgs a;
   memset(&a, 0, sizeof a);
   a.in = in; a.out = out; a.count = count; a.recv_counts = recv_counts;
   a.row_bytes = row_bytes; a.in_rows = in_rows; a.out_rows = out_rows; a.opcode = B2_OPC_ALLGATHERV;
-  int rc = 0;
+  a.max_rows = in_rows;
+  int rc;
   if (count == nullptr || recv_counts == nullptr) {
     b2_set_error("allgatherv: count and recv_counts must be device arrays of 1 and %d int64", c->dev.size);
     rc = B2_ERR_BAD_ARG;
-  }
-  if (rc == 0) rc = check_stage(c, a.opcode, in_rows * row_bytes, "allgatherv");
-  if (rc == 0) {
-    int grid;
-    pick_chunks(c, in_rows * row_bytes, coresident_blocks(c, (const void*)b2_k_allgatherv), &a.chunk, &grid);
-    b2_k_allgatherv<<<grid, B2_THREADS, 0, stream>>>(c->dev, a);
-    rc = b2_launched(c, "allgatherv");
+  } else {
+    rc = rowsv_launch(c, a, "allgatherv", stream);
   }
   b2_debug_end(dbg, rc);
   return rc;

@@ -163,9 +163,24 @@ def _clamp_in_order(counts, n: int) -> list:
     return out
 
 
+def _pack(stack: torch.Tensor, counts: list, displs: list, out_rows: int, place: Optional[list] = None):
+    """Rows ``[displs[q], displs[q] + counts[q])`` of ``stack[q]`` for every rank q, packed in rank order
+    into ``out_rows`` rows and clipped to them (``place``: at most ``place[q]`` rows each, at the sum of
+    the lower ranks' ``place``), zero elsewhere; and the rows written from each rank."""
+    out = torch.zeros((out_rows, *stack.shape[2:]), dtype=stack.dtype)
+    recv, filled = [], 0
+    for q, (n, d) in enumerate(zip(counts, displs)):
+        slot = out_rows - filled if place is None else place[q]
+        k = min(n, slot)
+        out[filled: filled + k] = stack[q, d: d + k]
+        recv.append(k)
+        filled += k if place is None else slot
+    return out, torch.tensor(recv, dtype=torch.int64)
+
+
 def alltoallv(comm: Comm, x: torch.Tensor, send_counts: torch.Tensor, out_rows: int,
               place_counts: Optional[torch.Tensor] = None):
-    """Same rules as the kernel (csrc/b2_collectives.cu: b2_k_alltoallv): everybody gathers every
+    """Same rules as the kernel (csrc/b2_collectives.cu: b2_k_rowsv): everybody gathers every
     rank's clamped counts and sent rows, then assembles its own output (correctness path)."""
     P, r = comm.size, comm.rank
     rows = x.shape[0]
@@ -176,33 +191,17 @@ def alltoallv(comm: Comm, x: torch.Tensor, send_counts: torch.Tensor, out_rows: 
     mine = torch.zeros((width, *x.shape[1:]), dtype=x.dtype)
     mine[: sum(sent)] = x[: sum(sent)]
     stack = _gather_stack(comm, mine)                                                   # (P, width, *S)
-    out = torch.zeros((out_rows, *x.shape[1:]), dtype=x.dtype)
     place = None if place_counts is None else _clamp_in_order(place_counts.tolist(), out_rows)
-    recv, filled = [], 0
-    for q in range(P):
-        d = sum(counts[q][:r])
-        slot = out_rows - filled if place is None else place[q]
-        k = min(counts[q][r], slot)
-        out[filled: filled + k] = stack[q, d: d + k]
-        recv.append(k)
-        filled += k if place is None else slot
-    return out, torch.tensor(recv, dtype=torch.int64)
+    return _pack(stack, [row[r] for row in counts], [sum(row[:r]) for row in counts], out_rows, place)
 
 
 def allgatherv(comm: Comm, x: torch.Tensor, count: torch.Tensor, out_rows: int):
-    """Same rules as the kernel (csrc/b2_collectives.cu: b2_k_allgatherv): everybody gathers every
-    rank's rows and clamped count, then packs the segments in rank order (correctness path)."""
+    """Same rules as the kernel's gather mode (csrc/b2_collectives.cu: b2_k_rowsv): alltoallv where every rank
+    sends its first ``count`` rows to every rank, each segment from row 0 of its source (correctness
+    path)."""
     n = min(max(int(count), 0), x.shape[0])
     counts = _gather_stack(comm, torch.tensor(n, dtype=torch.int64)).tolist()
-    stack = _gather_stack(comm, x)                                                      # (P, N, *S)
-    out = torch.zeros((out_rows, *x.shape[1:]), dtype=x.dtype)
-    recv, filled = [], 0
-    for q in range(comm.size):
-        k = min(counts[q], out_rows - filled)
-        out[filled: filled + k] = stack[q, :k]
-        recv.append(k)
-        filled += k
-    return out, torch.tensor(recv, dtype=torch.int64)
+    return _pack(_gather_stack(comm, x), counts, [0] * comm.size, out_rows)
 
 
 def bcast(comm: Comm, x: torch.Tensor, root: int) -> torch.Tensor:

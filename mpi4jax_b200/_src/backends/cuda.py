@@ -555,33 +555,30 @@ class NativeComm:
         """``(out, recv_counts)``: rows of ``x`` exchanged by the device-resident ``send_counts``
         (``collective_ops/alltoallv.py`` states the rules).  ``place_counts``: the reverse mode, which
         puts the rows from rank q where a forward call with these send counts took them from."""
-        x = _prep(x)
-        row_bytes = math.prod(x.shape[1:]) * x.element_size()
         max_rows = x.shape[0] if place_counts is None else self.comm.size * out_rows
-        out = torch.empty((out_rows, *x.shape[1:]), dtype=x.dtype, device=x.device)
-        recv_counts = torch.empty(self.comm.size, dtype=torch.int64, device=x.device)
-        send_counts = send_counts.to(torch.int64).contiguous()
         if place_counts is not None:
             place_counts = place_counts.to(torch.int64).contiguous()
-        self.ensure_stage(codes.OPC_ALLTOALLV, max_rows * row_bytes)
-        rc = _lib().b2_alltoallv(self.handle, x.data_ptr(), out.data_ptr(), row_bytes, x.shape[0], out_rows,
-                                 send_counts.data_ptr(), recv_counts.data_ptr(),
-                                 None if place_counts is None else place_counts.data_ptr(), self._stream())
-        self._check(rc, "Alltoallv")
-        return out, recv_counts
+        return self._rowsv(_lib().b2_alltoallv, "Alltoallv", codes.OPC_ALLTOALLV, max_rows, x, out_rows,
+                           send_counts, None if place_counts is None else place_counts.data_ptr())
 
     def allgatherv(self, x: torch.Tensor, count: torch.Tensor, out_rows: int):
         """``(out, recv_counts)``: the first ``count`` rows of every rank's ``x``, packed in rank order
         (``collective_ops/allgatherv.py`` states the rules); the count is read on the device."""
+        return self._rowsv(_lib().b2_allgatherv, "Allgatherv", codes.OPC_ALLGATHERV, x.shape[0], x, out_rows, count)
+
+    def _rowsv(self, fn, opname: str, opcode: int, stage_rows: int, x: torch.Tensor, out_rows: int,
+               counts: torch.Tensor, *place_ptr):
+        """Calls ``fn`` (b2_alltoallv / b2_allgatherv) with staging for ``stage_rows`` rows of ``x``;
+        ``place_ptr``: alltoallv's place counts."""
         x = _prep(x)
         row_bytes = math.prod(x.shape[1:]) * x.element_size()
         out = torch.empty((out_rows, *x.shape[1:]), dtype=x.dtype, device=x.device)
         recv_counts = torch.empty(self.comm.size, dtype=torch.int64, device=x.device)
-        count = count.to(torch.int64).contiguous()
-        self.ensure_stage(codes.OPC_ALLGATHERV, x.shape[0] * row_bytes)
-        rc = _lib().b2_allgatherv(self.handle, x.data_ptr(), out.data_ptr(), row_bytes, x.shape[0], out_rows,
-                                  count.data_ptr(), recv_counts.data_ptr(), self._stream())
-        self._check(rc, "Allgatherv")
+        counts = counts.to(torch.int64).contiguous()
+        self.ensure_stage(opcode, stage_rows * row_bytes)
+        rc = fn(self.handle, x.data_ptr(), out.data_ptr(), row_bytes, x.shape[0], out_rows, counts.data_ptr(),
+                recv_counts.data_ptr(), *place_ptr, self._stream())
+        self._check(rc, opname)
         return out, recv_counts
 
     # -- point to point ------------------------------------------------------------

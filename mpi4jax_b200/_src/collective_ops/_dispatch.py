@@ -9,6 +9,7 @@ device back ends, chosen by where the operand lives.
 from __future__ import annotations
 
 import math
+import operator
 from typing import Optional
 
 import torch
@@ -148,70 +149,77 @@ def alltoall(comm: Comm, x: torch.Tensor) -> torch.Tensor:
     return out
 
 
-def check_alltoallv_args(comm: Comm, x: torch.Tensor, counts: torch.Tensor, out_rows: int,
-                         name: str = "send_counts") -> None:
-    """Host-side checks of an alltoallv call.  Every entry point (the op, ``compiled.alltoallv``, the raw
-    ``torch.ops`` op, the backends) passes through them: the kernel dereferences the counts as ``nproc``
-    int64 values in x's device memory, so anything else must be refused before the launch."""
+def check_rows(opname: str, x: torch.Tensor) -> None:
     if x.dim() == 0:
-        raise ValueError("Alltoallv input must have shape (rows, ...)")
+        raise ValueError(f"{opname} input must have shape (rows, ...)")
+
+
+def as_counts(counts, x: torch.Tensor, scalar: bool = False) -> torch.Tensor:
+    """One int (``scalar``) or a sequence of ints becomes an int64 tensor on x's device; tensors are
+    checked, not moved."""
+    if isinstance(counts, torch.Tensor):
+        return counts
+    value = operator.index(counts) if scalar else [operator.index(c) for c in counts]
+    return torch.tensor(value, dtype=torch.int64, device=x.device)
+
+
+def check_rowsv_args(opname: str, comm: Comm, x: torch.Tensor, counts: torch.Tensor, out_rows: int,
+                     name: str) -> None:
+    """Host-side checks of an alltoallv / allgatherv call.  Every entry point (the op, its ``compiled``
+    twin, the raw ``torch.ops`` op and its fake kernel, the backends) passes through them: the kernel
+    dereferences the counts as int64 values in x's device memory -- ``nproc`` of them for alltoallv, one
+    for allgatherv -- so anything else must be refused before the launch."""
+    shape, shape_text = ((), "()") if opname == "Allgatherv" else ((comm.Get_size(),), "(nproc,)")
+    check_rows(opname, x)
     if not isinstance(counts, torch.Tensor):
-        raise TypeError(f"Alltoallv {name} must be an integer tensor (got {type(counts).__name__})")
+        raise TypeError(f"{opname} {name} must be an integer tensor (got {type(counts).__name__})")
     if counts.dtype.is_floating_point or counts.dtype.is_complex or counts.dtype == torch.bool:
-        raise TypeError(f"Alltoallv {name} must be an integer tensor (got {counts.dtype})")
-    if tuple(counts.shape) != (comm.Get_size(),):
-        raise ValueError(f"Alltoallv {name} must have shape (nproc,) (got {tuple(counts.shape)})")
+        raise TypeError(f"{opname} {name} must be an integer tensor (got {counts.dtype})")
+    if tuple(counts.shape) != shape:
+        raise ValueError(f"{opname} {name} must have shape {shape_text} (got {tuple(counts.shape)})")
     if counts.device != x.device:
-        raise ValueError(f"Alltoallv {name} must live on the device of x ({x.device}, got {counts.device})")
+        raise ValueError(f"{opname} {name} must live on the device of x ({x.device}, got {counts.device})")
     if out_rows < 0:
-        raise ValueError(f"Alltoallv recv_capacity must be >= 0 (got {out_rows})")
+        raise ValueError(f"{opname} recv_capacity must be >= 0 (got {out_rows})")
+
+
+def rowsv_capacity(opname: str, comm: Comm, x: torch.Tensor, counts: torch.Tensor, recv_capacity,
+                   name: str):
+    """The output rows of a public alltoallv / allgatherv call or its ``compiled`` twin, after the checks:
+    ``recv_capacity``, or ``N * nproc``, which never drops a row."""
+    check_rows(opname, x)
+    out_rows = x.shape[0] * comm.Get_size() if recv_capacity is None else recv_capacity
+    check_rowsv_args(opname, comm, x, counts, out_rows, name)
+    return out_rows
+
+
+def _cpu_rowsv(opname: str, fn, comm: Comm, x: torch.Tensor, *args):
+    """``fn(comm, x, *args)``, the CPU backend's alltoallv / allgatherv, with its log line."""
+    row_bytes = math.prod(x.shape[1:]) * x.element_size()
+    done = _log(comm, opname, f"with {x.shape[0]} rows of {row_bytes} bytes")
+    out = fn(comm, x, *args)
+    if done:
+        done()
+    return out
 
 
 def alltoallv(comm: Comm, x: torch.Tensor, send_counts: torch.Tensor, out_rows: int,
               place_counts: Optional[torch.Tensor] = None):
     _plain(x)
-    check_alltoallv_args(comm, x, send_counts, out_rows)
+    check_rowsv_args("Alltoallv", comm, x, send_counts, out_rows, "send_counts")
     if place_counts is not None:
-        check_alltoallv_args(comm, x, place_counts, out_rows, "place_counts")
+        check_rowsv_args("Alltoallv", comm, x, place_counts, out_rows, "place_counts")
     if x.is_cuda:
         return comm._native_comm().alltoallv(x, send_counts, out_rows, place_counts)
-    row_bytes = math.prod(x.shape[1:]) * x.element_size()
-    done = _log(comm, "Alltoallv", f"with {x.shape[0]} rows of {row_bytes} bytes")
-    out = _cpu.alltoallv(comm, x, send_counts, out_rows, place_counts)
-    if done:
-        done()
-    return out
-
-
-def check_allgatherv_args(x: torch.Tensor, count: torch.Tensor, out_rows: int) -> None:
-    """Host-side checks of an allgatherv call.  Every entry point (the op, ``compiled.allgatherv``, the raw
-    ``torch.ops`` op and its fake kernel, the backends) passes through them: the kernel dereferences the
-    count as one int64 value in x's device memory, so anything else must be refused before the launch."""
-    if x.dim() == 0:
-        raise ValueError("Allgatherv input must have shape (rows, ...)")
-    if not isinstance(count, torch.Tensor):
-        raise TypeError(f"Allgatherv count must be an integer tensor (got {type(count).__name__})")
-    if count.dtype.is_floating_point or count.dtype.is_complex or count.dtype == torch.bool:
-        raise TypeError(f"Allgatherv count must be an integer tensor (got {count.dtype})")
-    if count.dim() != 0:
-        raise ValueError(f"Allgatherv count must have shape () (got {tuple(count.shape)})")
-    if count.device != x.device:
-        raise ValueError(f"Allgatherv count must live on the device of x ({x.device}, got {count.device})")
-    if out_rows < 0:
-        raise ValueError(f"Allgatherv recv_capacity must be >= 0 (got {out_rows})")
+    return _cpu_rowsv("Alltoallv", _cpu.alltoallv, comm, x, send_counts, out_rows, place_counts)
 
 
 def allgatherv(comm: Comm, x: torch.Tensor, count: torch.Tensor, out_rows: int):
     _plain(x)
-    check_allgatherv_args(x, count, out_rows)
+    check_rowsv_args("Allgatherv", comm, x, count, out_rows, "count")
     if x.is_cuda:
         return comm._native_comm().allgatherv(x, count, out_rows)
-    row_bytes = math.prod(x.shape[1:]) * x.element_size()
-    done = _log(comm, "Allgatherv", f"with {x.shape[0]} rows of {row_bytes} bytes")
-    out = _cpu.allgatherv(comm, x, count, out_rows)
-    if done:
-        done()
-    return out
+    return _cpu_rowsv("Allgatherv", _cpu.allgatherv, comm, x, count, out_rows)
 
 
 def bcast(comm: Comm, x: torch.Tensor, root: int) -> torch.Tensor:

@@ -16,16 +16,15 @@ rank; capacity ``C_r``, which may differ between ranks):
 
 An invalid count is never an error and never makes the kernel read or write out of bounds.
 
-GPU: every rank stages its ``n_r`` rows once, behind a header holding ``n_r``; after one barrier each
-CTA reads the P headers, derives the packed offsets itself and pulls its chunks of every peer's segment
-straight into the output (csrc/b2_collectives.cu: b2_k_allgatherv).  Differentiable: the adjoint (SUM)
+GPU: alltoallv's kernel in gather mode (csrc/b2_collectives.cu: b2_k_rowsv).  Every rank stages its
+``n_r`` rows once, behind a header holding ``n_r``; after one barrier each CTA reads the P headers,
+derives the packed offsets itself and pulls its chunks of every peer's segment, each read from offset
+0, straight into the output.  Differentiable: the adjoint (SUM)
 cuts every received segment out of the cotangent into a ``(P, N, *S)`` tensor, zero-padded, and
 reduce-scatters it, so rank r gets the rank-order sum of what the receivers kept of its rows.
 """
 
 from __future__ import annotations
-
-import operator
 
 import numpy as np
 import torch
@@ -87,13 +86,6 @@ class _Allgatherv(torch.autograd.Function):
         return (out, counts), (1, None)
 
 
-def _as_count(count, x: torch.Tensor) -> torch.Tensor:
-    """A Python int becomes an int64 scalar tensor on x's device; tensors are checked, not moved."""
-    if isinstance(count, torch.Tensor):
-        return count
-    return torch.tensor(operator.index(count), dtype=torch.int64, device=x.device)
-
-
 @enforce_types(recv_capacity=(type(None), np.integer), comm=(type(None), Comm))
 def allgatherv(x, count, *, recv_capacity=None, comm=None, token=NOTSET):
     """Perform a variable-count allgather operation (``MPI_Allgatherv``) with a device-resident count.
@@ -117,11 +109,9 @@ def allgatherv(x, count, *, recv_capacity=None, comm=None, token=NOTSET):
         comm = get_default_comm()
     x = as_tensor(x, comm)
     check_dtype(x)
-    if x.dim() == 0:
-        raise ValueError("Allgatherv input must have shape (rows, ...)")
-    count = _as_count(count, x)
-    cap = x.shape[0] * comm.Get_size() if recv_capacity is None else int(recv_capacity)
-    _dispatch.check_allgatherv_args(x, count, cap)
+    _dispatch.check_rows("Allgatherv", x)
+    count = _dispatch.as_counts(count, x, scalar=True)
+    cap = int(_dispatch.rowsv_capacity("Allgatherv", comm, x, count, recv_capacity, "count"))
     if not needs_autograd(x):
         return _dispatch.allgatherv(comm, x, count, cap)
     return _Allgatherv.apply(x, count, cap, comm)

@@ -15,13 +15,11 @@ Rules, on rank r of P (``x_r`` has ``N`` rows, the same on every rank; capacity 
 
 GPU: every rank stages its send rows behind a header of its clamped counts; after one barrier each
 CTA reads all headers and pulls its chunks of the peers' segments straight into the output
-(csrc/b2_collectives.cu: b2_k_alltoallv).  Differentiable: the adjoint is the *reverse mode* of the
+(csrc/b2_collectives.cu: b2_k_rowsv).  Differentiable: the adjoint is the *reverse mode* of the
 same kernel, which puts the rows received from rank q back where rank q sent them from.
 """
 
 from __future__ import annotations
-
-import operator
 
 import numpy as np
 import torch
@@ -76,13 +74,6 @@ class _Alltoallv(torch.autograd.Function):
         return (out, counts), (1, None)
 
 
-def _as_counts(counts, x: torch.Tensor) -> torch.Tensor:
-    """A sequence of ints becomes an int64 tensor on x's device; tensors are checked, not moved."""
-    if isinstance(counts, torch.Tensor):
-        return counts
-    return torch.tensor([operator.index(c) for c in counts], dtype=torch.int64, device=x.device)
-
-
 @enforce_types(recv_capacity=(type(None), np.integer), comm=(type(None), Comm))
 def alltoallv(x, send_counts, *, recv_capacity=None, comm=None, token=NOTSET):
     """Perform a variable-count alltoall operation (``MPI_Alltoallv``) with device-resident counts.
@@ -108,11 +99,9 @@ def alltoallv(x, send_counts, *, recv_capacity=None, comm=None, token=NOTSET):
         comm = get_default_comm()
     x = as_tensor(x, comm)
     check_dtype(x)
-    if x.dim() == 0:
-        raise ValueError("Alltoallv input must have shape (rows, ...)")
-    send_counts = _as_counts(send_counts, x)
-    cap = x.shape[0] * comm.Get_size() if recv_capacity is None else int(recv_capacity)
-    _dispatch.check_alltoallv_args(comm, x, send_counts, cap)
+    _dispatch.check_rows("Alltoallv", x)
+    send_counts = _dispatch.as_counts(send_counts, x)
+    cap = int(_dispatch.rowsv_capacity("Alltoallv", comm, x, send_counts, recv_capacity, "send_counts"))
     if not needs_autograd(x):
         return _dispatch.alltoallv(comm, x, send_counts, cap)
     return _Alltoallv.apply(x, send_counts, cap, None, comm)
@@ -124,9 +113,9 @@ def alltoallv_reverse(y: torch.Tensor, recv_counts: torch.Tensor, send_counts: t
     like that call's output) travel back to the rank they came from and land where it sent them from,
     in an output of ``rows`` rows (that call's ``N``).  Rows that were dropped or never sent are zero.
     Differentiable (the adjoint is the forward exchange)."""
-    recv_counts, send_counts = _as_counts(recv_counts, y), _as_counts(send_counts, y)
-    _dispatch.check_alltoallv_args(comm, y, recv_counts, rows, "recv_counts")
-    _dispatch.check_alltoallv_args(comm, y, send_counts, rows)
+    recv_counts, send_counts = _dispatch.as_counts(recv_counts, y), _dispatch.as_counts(send_counts, y)
+    _dispatch.check_rowsv_args("Alltoallv", comm, y, recv_counts, rows, "recv_counts")
+    _dispatch.check_rowsv_args("Alltoallv", comm, y, send_counts, rows, "send_counts")
     if not needs_autograd(y):
         return _dispatch.alltoallv(comm, y, recv_counts, rows, send_counts)[0]
     return _Alltoallv.apply(y, recv_counts, rows, send_counts, comm)[0]

@@ -161,7 +161,7 @@ def _alltoallv(x: torch.Tensor, send_counts: torch.Tensor, out_rows: int, place_
 @_alltoallv.register_fake
 def _(x, send_counts, out_rows, place_counts, comm_id):
     comm = _c(comm_id)
-    _dispatch.check_alltoallv_args(comm, x, send_counts, out_rows)
+    _dispatch.check_rowsv_args("Alltoallv", comm, x, send_counts, out_rows, "send_counts")
     return x.new_empty((out_rows, *x.shape[1:])), x.new_empty((comm.Get_size(),), dtype=torch.int64)
 
 
@@ -192,8 +192,9 @@ def _allgatherv(x: torch.Tensor, count: torch.Tensor, out_rows: int, comm_id: in
 
 @_allgatherv.register_fake
 def _(x, count, out_rows, comm_id):
-    _dispatch.check_allgatherv_args(x, count, out_rows)
-    return x.new_empty((out_rows, *x.shape[1:])), x.new_empty((_c(comm_id).Get_size(),), dtype=torch.int64)
+    comm = _c(comm_id)
+    _dispatch.check_rowsv_args("Allgatherv", comm, x, count, out_rows, "count")
+    return x.new_empty((out_rows, *x.shape[1:])), x.new_empty((comm.Get_size(),), dtype=torch.int64)
 
 
 def _allgatherv_setup(ctx, inputs, output):
@@ -394,10 +395,7 @@ class compiled:
         """``(out, recv_counts)`` of :func:`mpi4jax_b200.alltoallv`; ``send_counts`` must be a device
         tensor of shape ``(nproc,)``."""
         comm = comm or get_default_comm()
-        if x.dim() == 0:
-            raise ValueError("Alltoallv input must have shape (rows, ...)")
-        cap = x.shape[0] * comm.Get_size() if recv_capacity is None else recv_capacity
-        _dispatch.check_alltoallv_args(comm, x, send_counts, cap)
+        cap = _dispatch.rowsv_capacity("Alltoallv", comm, x, send_counts, recv_capacity, "send_counts")
         return torch.ops.mpi4jax_b200.alltoallv(x, send_counts, cap, None, comm._id)
 
     @staticmethod
@@ -405,10 +403,7 @@ class compiled:
         """``(out, recv_counts)`` of :func:`mpi4jax_b200.allgatherv`; ``count`` must be an integer device
         tensor of shape ``()``."""
         comm = comm or get_default_comm()
-        if x.dim() == 0:
-            raise ValueError("Allgatherv input must have shape (rows, ...)")
-        cap = x.shape[0] * comm.Get_size() if recv_capacity is None else recv_capacity
-        _dispatch.check_allgatherv_args(x, count, cap)
+        cap = _dispatch.rowsv_capacity("Allgatherv", comm, x, count, recv_capacity, "count")
         return torch.ops.mpi4jax_b200.allgatherv(x, count, cap, comm._id)
 
     @staticmethod
