@@ -1,2 +1,12 @@
 """The 13 communication primitives (one module per op, like the reference's
 mpi4jax/_src/collective_ops/)."""
+
+from types import SimpleNamespace
+
+from . import allgather, allreduce, alltoall, alltoallv, reduce, reduce_scatter, sendrecv
+
+# the eager frontend as ``F`` of the shared adjoint rules (_adjoints.py)
+eager = SimpleNamespace(allgather=allgather.allgather, allreduce=allreduce.allreduce, alltoall=alltoall.alltoall,
+                        alltoallv=alltoallv.alltoallv, _alltoallv_reverse=alltoallv.alltoallv_reverse,
+                        reduce=reduce.reduce, reduce_scatter=reduce_scatter.reduce_scatter,
+                        sendrecv=sendrecv.sendrecv)

@@ -10,11 +10,12 @@ from __future__ import annotations
 
 import torch
 
-from ..comm import SUM, Comm
+from .. import collective_ops
+from ..comm import Comm
 from ..utils import (NOTSET, as_tensor, check_dtype, get_default_comm, needs_autograd,
                      raise_if_token_is_set)
 from ..validation import enforce_types
-from . import _dispatch
+from . import _adjoints, _dispatch
 
 
 class _Allgather(torch.autograd.Function):
@@ -28,10 +29,7 @@ class _Allgather(torch.autograd.Function):
 
     @staticmethod
     def backward(ctx, g):
-        from .allreduce import allreduce      # the differentiable op: works under torch.func too
-
-        total = allreduce(g.contiguous(), SUM, comm=ctx.comm)
-        return total[ctx.comm.rank], None
+        return _adjoints.allgather(collective_ops.eager, g, ctx.comm), None
 
     @staticmethod
     def vmap(info, in_dims, x, comm):

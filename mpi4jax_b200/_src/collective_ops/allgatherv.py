@@ -29,25 +29,12 @@ from __future__ import annotations
 import numpy as np
 import torch
 
-from ..comm import SUM, Comm
+from .. import collective_ops
+from ..comm import Comm
 from ..utils import (NOTSET, as_tensor, check_dtype, get_default_comm, needs_autograd,
                      raise_if_token_is_set)
 from ..validation import enforce_types
-from . import _dispatch
-
-
-def segments(g: torch.Tensor, recv_counts: torch.Tensor, rows: int) -> torch.Tensor:
-    """``G`` of shape ``(P, rows, *S)`` with ``G[q, i] = g[o[q] + i]`` for ``i < recv_counts[q]`` and 0
-    otherwise, where ``o`` is the exclusive prefix sum of ``recv_counts``: the segments of an allgatherv
-    output, each back at the start of its source's rows.  Device ops only (no host read of the counts);
-    differentiable in ``g``."""
-    P = recv_counts.shape[0]
-    offsets = torch.cumsum(recv_counts, 0) - recv_counts
-    i = torch.arange(rows, device=g.device)
-    # entries past a segment read a zero row appended to g (index g.shape[0])
-    idx = torch.where(i < recv_counts.view(P, 1), offsets.view(P, 1) + i, g.shape[0])
-    padded = torch.cat([g, g.new_zeros((1, *g.shape[1:]))])
-    return padded[idx]
+from . import _adjoints, _dispatch
 
 
 class _Allgatherv(torch.autograd.Function):
@@ -64,10 +51,8 @@ class _Allgatherv(torch.autograd.Function):
 
     @staticmethod
     def backward(ctx, g, _g_counts):
-        from .reduce_scatter import reduce_scatter      # the differentiable op: double backward works
-
         (recv_counts,) = ctx.saved_tensors
-        return reduce_scatter(segments(g, recv_counts, ctx.in_rows), SUM, comm=ctx.comm), None, None, None
+        return _adjoints.allgatherv(collective_ops.eager, g, ctx.comm, ctx.in_rows, recv_counts), None, None, None
 
     @staticmethod
     def jvp(ctx, x_t, *_):

@@ -9,11 +9,12 @@ from __future__ import annotations
 
 import torch
 
+from .. import collective_ops
 from ..comm import Comm
 from ..utils import (NOTSET, as_tensor, check_dtype, get_default_comm, needs_autograd,
                      raise_if_token_is_set)
 from ..validation import enforce_types
-from . import _dispatch
+from . import _adjoints, _dispatch
 
 
 class _Alltoall(torch.autograd.Function):
@@ -27,7 +28,7 @@ class _Alltoall(torch.autograd.Function):
 
     @staticmethod
     def backward(ctx, g):
-        return _Alltoall.apply(g.contiguous(), ctx.comm), None
+        return _adjoints.alltoall(collective_ops.eager, g, ctx.comm), None
 
     @staticmethod
     def vmap(info, in_dims, x, comm):

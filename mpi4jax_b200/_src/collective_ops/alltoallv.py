@@ -24,11 +24,12 @@ from __future__ import annotations
 import numpy as np
 import torch
 
+from .. import collective_ops
 from ..comm import Comm
 from ..utils import (NOTSET, as_tensor, check_dtype, get_default_comm, needs_autograd,
                      raise_if_token_is_set)
 from ..validation import enforce_types
-from . import _dispatch
+from . import _adjoints, _dispatch
 
 
 class _Alltoallv(torch.autograd.Function):
@@ -50,11 +51,9 @@ class _Alltoallv(torch.autograd.Function):
     @staticmethod
     def backward(ctx, g, _g_counts):
         (recv_counts,) = ctx.saved_tensors
-        if ctx.place_counts is None:       # forward -> reverse mode: rows go back where they came from
-            back = _Alltoallv.apply(g.contiguous(), recv_counts, ctx.in_rows, ctx.send_counts, ctx.comm)
-        else:                              # reverse -> forward mode with the forward's counts and capacity
-            back = _Alltoallv.apply(g.contiguous(), ctx.place_counts, ctx.in_rows, None, ctx.comm)
-        return back[0], None, None, None, None
+        back = _adjoints.alltoallv(collective_ops.eager, g, ctx.comm, ctx.in_rows, ctx.send_counts, recv_counts,
+                                   ctx.place_counts)
+        return back, None, None, None, None
 
     @staticmethod
     def jvp(ctx, x_t, *_):

@@ -12,11 +12,12 @@ from __future__ import annotations
 import numpy as np
 import torch
 
-from ..comm import SUM, Comm
+from .. import collective_ops
+from ..comm import Comm
 from ..utils import (NOTSET, as_tensor, check_dtype, get_default_comm, needs_autograd,
                      raise_if_token_is_set)
 from ..validation import enforce_types
-from . import _dispatch
+from . import _adjoints, _dispatch
 
 
 class _Bcast(torch.autograd.Function):
@@ -31,11 +32,7 @@ class _Bcast(torch.autograd.Function):
 
     @staticmethod
     def backward(ctx, g):
-        comm, root = ctx.comm, ctx.root
-        total = _dispatch.run_opaque(lambda t: _dispatch.reduce(comm, t, SUM.code, root), g.contiguous())
-        if comm.rank == root:
-            return total, None, None
-        return torch.zeros_like(g), None, None
+        return _adjoints.bcast(collective_ops.eager, g, ctx.root, ctx.comm), None, None
 
     @staticmethod
     def vmap(info, in_dims, x, root, comm):

@@ -11,11 +11,12 @@ from __future__ import annotations
 
 import torch
 
+from .. import collective_ops
 from ..comm import OP_TYPES, SUM, Comm, Op, as_op
 from ..utils import (NOTSET, as_tensor, check_dtype, fold, get_default_comm, needs_autograd,
                      raise_if_token_is_set)
 from ..validation import enforce_types
-from . import _dispatch
+from . import _adjoints, _dispatch
 
 
 def _require_sum(op: Op, what: str) -> None:
@@ -34,10 +35,8 @@ class _ReduceScatter(torch.autograd.Function):
 
     @staticmethod
     def backward(ctx, g):
-        from .allgather import allgather      # the differentiable op: works under torch.func too
-
         _require_sum(ctx.op, "adjoint")
-        return allgather(g.contiguous(), comm=ctx.comm), None, None
+        return _adjoints.reduce_scatter(collective_ops.eager, g, ctx.comm), None, None
 
     @staticmethod
     def jvp(ctx, x_t, *_):

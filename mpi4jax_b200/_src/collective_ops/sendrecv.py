@@ -13,11 +13,12 @@ from __future__ import annotations
 import numpy as np
 import torch
 
+from .. import collective_ops
 from ..comm import ANY_TAG, PROC_NULL, Comm, Status
 from ..utils import (NOTSET, as_tensor, carries_grad, check_dtype, check_rank, get_default_comm,
                      needs_autograd, raise_if_token_is_set)
 from ..validation import enforce_types
-from . import _dispatch
+from . import _adjoints, _dispatch
 
 
 class _Sendrecv(torch.autograd.Function):
@@ -32,9 +33,8 @@ class _Sendrecv(torch.autograd.Function):
 
     @staticmethod
     def backward(ctx, g):
-        # transpose: the cotangent travels the opposite way (source <-> dest swapped)
-        gs = _Sendrecv.apply(g.contiguous(), ctx.send_template, ctx.dest, ctx.source,
-                             ctx.sendtag, ctx.recvtag, ctx.comm, None)
+        gs = _adjoints.sendrecv(collective_ops.eager, g, ctx.send_template, ctx.source, ctx.dest, ctx.sendtag,
+                                ctx.recvtag, ctx.comm)
         return gs, None, None, None, None, None, None, None
 
     @staticmethod

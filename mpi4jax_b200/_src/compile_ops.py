@@ -27,8 +27,7 @@ import torch
 from torch.library import custom_op
 
 from . import comm as _comm_mod
-from .collective_ops import _dispatch
-from .collective_ops.allgatherv import segments
+from .collective_ops import _adjoints, _dispatch
 from .comm import ANY_SOURCE, ANY_TAG, SUM, Comm, as_op
 from .native import codes
 from .utils import get_default_comm
@@ -101,8 +100,7 @@ def _reduce_scatter_setup(ctx, inputs, output):
 def _reduce_scatter_backward(ctx, g):
     if ctx.op != SUM.code:
         raise NotImplementedError("The adjoint of reduce_scatter is only defined for SUM")
-    size = _c(ctx.comm_id).Get_size()
-    return torch.ops.mpi4jax_b200.allgather(g.contiguous(), ctx.comm_id, size), None, None
+    return _adjoints.reduce_scatter(compiled, g, _c(ctx.comm_id)), None, None
 
 
 _reduce_scatter.register_autograd(_reduce_scatter_backward, setup_context=_reduce_scatter_setup)
@@ -123,9 +121,7 @@ def _allgather_setup(ctx, inputs, output):
 
 
 def _allgather_backward(ctx, g):
-    # adjoint of allgather = reduce-scatter of the cotangent (here: allreduce + own slice)
-    total = torch.ops.mpi4jax_b200.allreduce(g.contiguous(), SUM.code, ctx.comm_id)
-    return total[_c(ctx.comm_id).Get_rank()], None, None
+    return _adjoints.allgather(compiled, g, _c(ctx.comm_id)), None, None
 
 
 _allgather.register_autograd(_allgather_backward, setup_context=_allgather_setup)
@@ -146,7 +142,7 @@ def _alltoall_setup(ctx, inputs, output):
 
 
 def _alltoall_backward(ctx, g):
-    return torch.ops.mpi4jax_b200.alltoall(g.contiguous(), ctx.comm_id), None      # self-adjoint up to the swap
+    return _adjoints.alltoall(compiled, g, _c(ctx.comm_id)), None
 
 
 _alltoall.register_autograd(_alltoall_backward, setup_context=_alltoall_setup)
@@ -168,18 +164,13 @@ def _(x, send_counts, out_rows, place_counts, comm_id):
 def _alltoallv_setup(ctx, inputs, output):
     x, send_counts, _, place_counts, ctx.comm_id = inputs
     ctx.in_rows = x.shape[0]
-    ctx.reverse = place_counts is not None
     ctx.save_for_backward(send_counts, place_counts, output[1])
 
 
 def _alltoallv_backward(ctx, g, _g_counts):
-    # forward <-> reverse mode (collective_ops/alltoallv.py): the rows travel back the way they came
     send_counts, place_counts, recv_counts = ctx.saved_tensors
-    if ctx.reverse:
-        back = torch.ops.mpi4jax_b200.alltoallv(g.contiguous(), place_counts, ctx.in_rows, None, ctx.comm_id)
-    else:
-        back = torch.ops.mpi4jax_b200.alltoallv(g.contiguous(), recv_counts, ctx.in_rows, send_counts, ctx.comm_id)
-    return back[0], None, None, None, None
+    back = _adjoints.alltoallv(compiled, g, _c(ctx.comm_id), ctx.in_rows, send_counts, recv_counts, place_counts)
+    return back, None, None, None, None
 
 
 _alltoallv.register_autograd(_alltoallv_backward, setup_context=_alltoallv_setup)
@@ -204,10 +195,8 @@ def _allgatherv_setup(ctx, inputs, output):
 
 
 def _allgatherv_backward(ctx, g, _g_counts):
-    # SUM adjoint (collective_ops/allgatherv.py): the received segments, zero-padded to (P, N, ...), reduce-scattered
     (recv_counts,) = ctx.saved_tensors
-    G = segments(g.contiguous(), recv_counts, ctx.in_rows)
-    return torch.ops.mpi4jax_b200.reduce_scatter(G, SUM.code, ctx.comm_id), None, None, None
+    return _adjoints.allgatherv(compiled, g, _c(ctx.comm_id), ctx.in_rows, recv_counts), None, None, None
 
 
 _allgatherv.register_autograd(_allgatherv_backward, setup_context=_allgatherv_setup)
@@ -229,11 +218,7 @@ def _bcast_setup(ctx, inputs, output):
 
 
 def _bcast_backward(ctx, g):
-    # adjoint of bcast = sum of the cotangents on the root, nothing elsewhere
-    total = torch.ops.mpi4jax_b200.reduce(g.contiguous(), SUM.code, ctx.root, ctx.comm_id)
-    if _c(ctx.comm_id).Get_rank() == ctx.root:
-        return total, None, None
-    return torch.zeros_like(g), None, None
+    return _adjoints.bcast(compiled, g, ctx.root, _c(ctx.comm_id)), None, None
 
 
 _bcast.register_autograd(_bcast_backward, setup_context=_bcast_setup)
@@ -341,12 +326,10 @@ def _sendrecv_setup(ctx, inputs, output):
 
 
 def _sendrecv_backward(ctx, g):
-    # transpose: the cotangent of what was received travels back to where it came from
-    # (the reference swaps source and dest the same way, sendrecv.py:277-292)
     shape, dtype, device = ctx.send_meta
     template = torch.empty(shape, dtype=dtype, device=device)
-    back = torch.ops.mpi4jax_b200.sendrecv(g.contiguous(), template, ctx.dest, ctx.source,
-                                           max(ctx.recvtag, 0), ctx.sendtag, ctx.comm_id, 0)
+    back = _adjoints.sendrecv(compiled, g, template, ctx.source, ctx.dest, ctx.sendtag, ctx.recvtag,
+                              _c(ctx.comm_id))
     return back, None, None, None, None, None, None, None
 
 
@@ -397,6 +380,11 @@ class compiled:
         comm = comm or get_default_comm()
         cap = _dispatch.rowsv_capacity("Alltoallv", comm, x, send_counts, recv_capacity, "send_counts")
         return torch.ops.mpi4jax_b200.alltoallv(x, send_counts, cap, None, comm._id)
+
+    @staticmethod
+    def _alltoallv_reverse(y, recv_counts, send_counts, rows, comm):
+        # the counterpart of the eager alltoallv_reverse, for alltoallv's adjoint (collective_ops/_adjoints.py)
+        return torch.ops.mpi4jax_b200.alltoallv(y, recv_counts, rows, send_counts, comm._id)[0]
 
     @staticmethod
     def allgatherv(x, count, *, recv_capacity=None, comm=None):

@@ -16,7 +16,8 @@ REPO = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 SUITE = ["tests/collective_ops", "tests/test_transforms.py", "tests/test_models.py",
          "tests/test_examples.py", "tests/test_jit.py", "tests/test_common.py", "tests/test_gemm.py",
          "tests/test_compile.py", "tests/test_transport.py", "tests/test_object_api.py",
-         "tests/test_more_examples.py", "tests/test_extensions.py", "tests/test_coresidency.py"]
+         "tests/test_more_examples.py", "tests/test_extensions.py", "tests/test_coresidency.py",
+         "tests/test_shared_adjoints.py"]
 
 inside_job = MPI.COMM_WORLD.Get_size() > 1 or "MPI4JAX_B200_NESTED" in os.environ
 
