@@ -817,6 +817,35 @@ extern "C" int b2_barrier(B2Comm* c, cudaStream_t stream) {
   return rc;
 }
 
+// The transport of a reduction of `nbytes` bytes per rank (per block for reduce-scatter): `algo` itself
+// unless it is B2_ALGO_AUTO, else the size-based choice -- the same on every rank.
+static int reduce_algo(const B2Comm* c, size_t nbytes, int dtype, int op, int algo, int opcode) {
+  if (algo != B2_ALGO_AUTO) return algo;
+  const int P = c->dev.size;
+  // reduce-scatter: a block travels to each peer like a whole allreduce payload (LL) or is pulled
+  // from every peer's staging (the one-shot branch of the kernel)
+  const bool ll_fits = P > 1 && nbytes <= c->ll_max && nbytes * 2 <= c->dev.lay.ll_cap;
+  if (opcode == B2_OPC_REDUCE_SCATTER) return ll_fits ? B2_ALGO_LL : B2_ALGO_ONESHOT;
+  if (opcode != B2_OPC_ALLREDUCE) return B2_ALGO_ONESHOT;
+  if (ll_fits) return B2_ALGO_LL;
+  if (P <= 2) return B2_ALGO_ONESHOT;
+  if (nvls_capable(c, dtype, op) && nbytes >= c->nvls_min) return B2_ALGO_NVLS;
+  if (nbytes <= c->oneshot_max) return B2_ALGO_ONESHOT;
+  return B2_ALGO_TWOSHOT;
+}
+
+// the transport's name at the end of the debug log line ("MPI_Allreduce (GPU) with 4096 items via twoshot")
+static const char* algo_name(int algo) {
+  switch (algo) {
+    case B2_ALGO_LL: return "ll";
+    case B2_ALGO_ONESHOT: return "oneshot";
+    case B2_ALGO_TWOSHOT: return "twoshot";
+    case B2_ALGO_NVLS: return "nvls";
+    default: return "auto";
+  }
+}
+
+// `algo`: a transport resolved by reduce_algo
 static int reduce_common(B2Comm* c, const void* in, void* out, size_t count, int dtype, int op,
                          int algo, int src_lo, int src_hi, int has_out, int opcode,
                          const char* name, cudaStream_t stream) {
@@ -828,20 +857,7 @@ static int reduce_common(B2Comm* c, const void* in, void* out, size_t count, int
   }
   const size_t nbytes = count * b2_dtype_size(dtype);
   if (nbytes == 0) return 0;
-  const int P = c->dev.size;
-  // reduce-scatter: `count` and `nbytes` are per block; a block travels to each peer like a whole
-  // allreduce payload (LL) or is pulled from every peer's staging (the one-shot branch of the kernel)
   const bool rs = opcode == B2_OPC_REDUCE_SCATTER;
-  const bool ll_fits = P > 1 && nbytes <= c->ll_max && nbytes * 2 <= c->dev.lay.ll_cap;
-  if (algo == B2_ALGO_AUTO) {
-    if (rs) algo = ll_fits ? B2_ALGO_LL : B2_ALGO_ONESHOT;
-    else if (opcode != B2_OPC_ALLREDUCE) algo = B2_ALGO_ONESHOT;
-    else if (ll_fits) algo = B2_ALGO_LL;
-    else if (P <= 2) algo = B2_ALGO_ONESHOT;
-    else if (nvls_capable(c, dtype, op) && nbytes >= c->nvls_min) algo = B2_ALGO_NVLS;
-    else if (nbytes <= c->oneshot_max) algo = B2_ALGO_ONESHOT;
-    else algo = B2_ALGO_TWOSHOT;
-  }
   if (algo == B2_ALGO_LL) {
     if ((opcode != B2_OPC_ALLREDUCE && !rs) || nbytes * 2 > c->dev.lay.ll_cap) {
       b2_set_error("%s: LL algorithm needs an allreduce of <= %zu bytes", name,
@@ -886,7 +902,8 @@ static int reduce_common(B2Comm* c, const void* in, void* out, size_t count, int
 
 extern "C" int b2_allreduce(B2Comm* c, const void* in, void* out, size_t count, int dtype, int op,
                             int algo, cudaStream_t stream) {
-  B2DebugScope* dbg = b2_debug_begin(c, "Allreduce", stream, "with %zu items", count);
+  algo = reduce_algo(c, count * b2_dtype_size(dtype), dtype, op, algo, B2_OPC_ALLREDUCE);
+  B2DebugScope* dbg = b2_debug_begin(c, "Allreduce", stream, "with %zu items via %s", count, algo_name(algo));
   int rc = reduce_common(c, in, out, count, dtype, op, algo, 0, c->dev.size, 1, B2_OPC_ALLREDUCE,
                          "allreduce", stream);
   b2_debug_end(dbg, rc);
@@ -923,16 +940,18 @@ extern "C" int b2_allreduce_sym(B2Comm* c, void* mc, size_t count, int dtype, cu
 
 extern "C" int b2_reduce(B2Comm* c, const void* in, void* out, size_t count, int dtype, int op,
                          int root, cudaStream_t stream) {
-  B2DebugScope* dbg = b2_debug_begin(c, "Reduce", stream, "with %zu items to root %d", count, root);
+  const size_t nbytes = count * b2_dtype_size(dtype);
+  const bool nvls = c->dev.size > 2 && nvls_capable(c, dtype, op) && nbytes >= c->nvls_min;
+  const int algo = nvls ? B2_ALGO_NVLS : B2_ALGO_ONESHOT;
+  B2DebugScope* dbg = b2_debug_begin(c, "Reduce", stream, "with %zu items to root %d via %s", count, root,
+                                     algo_name(algo));
   int rc;
   if (root < 0 || root >= c->dev.size) {
     b2_set_error("reduce: invalid root %d", root);
     rc = B2_ERR_BAD_ARG;
   } else {
-    const size_t nbytes = count * b2_dtype_size(dtype);
-    const bool nvls = c->dev.size > 2 && nvls_capable(c, dtype, op) && nbytes >= c->nvls_min;
-    rc = reduce_common(c, in, out, count, dtype, op, nvls ? B2_ALGO_NVLS : B2_ALGO_ONESHOT, 0, c->dev.size,
-                       c->dev.rank == root, B2_OPC_REDUCE, "reduce", stream);
+    rc = reduce_common(c, in, out, count, dtype, op, algo, 0, c->dev.size, c->dev.rank == root, B2_OPC_REDUCE,
+                       "reduce", stream);
   }
   b2_debug_end(dbg, rc);
   return rc;
@@ -940,12 +959,12 @@ extern "C" int b2_reduce(B2Comm* c, const void* in, void* out, size_t count, int
 
 extern "C" int b2_scan(B2Comm* c, const void* in, void* out, size_t count, int dtype, int op,
                        cudaStream_t stream) {
-  B2DebugScope* dbg = b2_debug_begin(c, "Scan", stream, "with %zu items", count);
   // small: rank r pulls the copies of ranks 0..r (one phase); large: rank s computes ALL prefixes of
   // sub-slice s and pushes prefix q to rank q (two phases, S bytes in and out per rank instead of
   // up to P * S into the last rank)
   const size_t nbytes = count * b2_dtype_size(dtype);
   const int algo = (c->dev.size > 2 && nbytes > c->oneshot_max) ? B2_ALGO_TWOSHOT : B2_ALGO_ONESHOT;
+  B2DebugScope* dbg = b2_debug_begin(c, "Scan", stream, "with %zu items via %s", count, algo_name(algo));
   int rc = reduce_common(c, in, out, count, dtype, op, algo, 0, c->dev.rank + 1, 1, B2_OPC_SCAN, "scan", stream);
   b2_debug_end(dbg, rc);
   return rc;
@@ -955,8 +974,10 @@ extern "C" int b2_scan(B2Comm* c, const void* in, void* out, size_t count, int d
 // block r over all ranks, folded in rank order.  P == 1 copies the one block.
 extern "C" int b2_reduce_scatter(B2Comm* c, const void* in, void* out, size_t count, int dtype, int op,
                                  cudaStream_t stream) {
-  B2DebugScope* dbg = b2_debug_begin(c, "Reduce_scatter_block", stream, "with %zu items per block", count);
-  int rc = reduce_common(c, in, out, count, dtype, op, B2_ALGO_AUTO, 0, c->dev.size, 1, B2_OPC_REDUCE_SCATTER,
+  const int algo = reduce_algo(c, count * b2_dtype_size(dtype), dtype, op, B2_ALGO_AUTO, B2_OPC_REDUCE_SCATTER);
+  B2DebugScope* dbg = b2_debug_begin(c, "Reduce_scatter_block", stream, "with %zu items per block via %s", count,
+                                     algo_name(algo));
+  int rc = reduce_common(c, in, out, count, dtype, op, algo, 0, c->dev.size, 1, B2_OPC_REDUCE_SCATTER,
                          "reduce_scatter", stream);
   b2_debug_end(dbg, rc);
   return rc;

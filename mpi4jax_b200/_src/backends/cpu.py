@@ -45,6 +45,16 @@ def reduce_stack(stack: torch.Tensor, op_code: int) -> torch.Tensor:
             return stack.all(dim=0)
         if op_code in (codes.LXOR, codes.BXOR):
             return (stack.to(torch.int32).sum(dim=0) % 2).to(torch.bool)
+    if dt in (torch.uint16, torch.uint32, torch.uint64) and op_code in (codes.SUM, codes.PROD, codes.MIN, codes.MAX):
+        # CPU torch has no arithmetic on these: int64 holds the same bits modulo 2^64 (sums and products
+        # wrap alike), and a flipped sign bit makes its order the unsigned order of uint64
+        wide = stack.view(torch.int64) if dt == torch.uint64 else stack.to(torch.int64)
+        if op_code in (codes.MIN, codes.MAX):
+            bias = -(1 << 63) if dt == torch.uint64 else 0
+            res = reduce_stack(wide ^ bias, op_code) ^ bias
+        else:
+            res = reduce_stack(wide, op_code)
+        return res.view(dt) if dt == torch.uint64 else res.to(dt)
     is_float = dt.is_floating_point
     is_cplx = dt.is_complex
     if op_code == codes.SUM:

@@ -63,7 +63,7 @@ def needs_peers(reason: str, max_rank: int = None):
             return fn
 
         @functools.wraps(fn)
-        def at_world_size_1(device):
+        def at_world_size_1(device, **fixtures):     # (other fixtures the test takes, e.g. capsys)
             if device.type != "cuda":
                 pytest.skip(reason)
             _expect_passed_in_pair_job(fn)
