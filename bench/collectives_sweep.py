@@ -9,6 +9,8 @@
   plus balanced rows of 8190 bytes (the byte-wise path for rows that are not a multiple of 16 bytes)
 * allgatherv bf16 rows, full / half / skewed counts, 64 KiB - 256 MiB per rank, vs the allgather of the
   padded rows (alone and followed by a device-side compaction) and vs NCCL all_gather_into_tensor
+* reduce_scatterv bf16 rows, equal / skewed / small counts, 64 KiB - 256 MiB output per rank, vs the
+  reduce_scatter of the zero-padded segments (with the padding gather) and vs NCCL reduce_scatter_tensor
 * bcast, reduce, gather, scatter (root = last rank) vs NCCL, scan (no NCCL counterpart)
 * sendrecv ring, halo exchange latency
 
@@ -43,6 +45,7 @@ ap.add_argument("--skip-allreduce-algos", action="store_true", help="time only t
 ap.add_argument("--only-allreduce", action="store_true", help="stop after the allreduce tables")
 ap.add_argument("--only-p2p", action="store_true", help="only the p2p ring, barrier and halo lines")
 ap.add_argument("--only-allgatherv", action="store_true", help="only the allgatherv rows")
+ap.add_argument("--only-reduce-scatterv", action="store_true", help="only the reduce_scatterv rows")
 ap.add_argument("--max-blocks", type=int, default=0, help="override the collective grid cap")
 ap.add_argument("--nvls-pipeline", type=int, default=-1, help="0 / 1: software pipelining of the NVLS allreduce")
 ap.add_argument("--min-bytes", type=int, default=1 << 10)
@@ -178,6 +181,60 @@ def allgatherv_rows():
                 print("allgatherv", kind, nbytes, {k: (v["us"], v["busbw"]) for k, v in row.items()}, flush=True)
             del x
 
+
+# ------------------------------------------------------------ reduce_scatterv (N rows out = nbytes, 64 KiB - 256 MiB)
+# bf16 rows of hidden size 4096 (8 KiB); every rank holds P segments of up to N rows (x has P * N rows) and sends
+# s[p] rows to rank p: "equal" (N: the reduce_scatter of x.view(P, N, hidden)), "skewed" (N * (p + 1) / P) and
+# "small" (N / 8, the case of a capacity far above the counts).  Next to what a user writes without
+# reduce_scatterv -- the segments zero-padded into (P, N, hidden) with a device-side gather (capturable, no
+# host read), then reduce_scatter -- and to NCCL's reduce_scatter_tensor of that padded tensor (alone).
+# Bandwidth: the rows a rank receives from its peers, sum_{q != r} s_q[r] * row_bytes (the most over ranks),
+# divided by the time.
+def reduce_scatterv_rows():
+    result["reduce_scatterv"] = {"equal": {}, "skewed": {}, "small": {}}
+    hidden = 4096
+    for nbytes in [b for b in sizes if (64 << 10) <= b <= (256 << 20) and b * size <= (1 << 30)]:
+        n = nbytes // (hidden * 2)
+        for kind in ("equal", "skewed", "small"):
+            counts = [n if kind == "equal" else n * (p + 1) // size if kind == "skewed" else n // 8
+                      for p in range(size)]
+            useful = max(counts) * (size - 1) * hidden * 2
+            bw = lambda us: round(useful / us / 1e3, 1) if useful else 0.0
+            x = torch.ones(size * n, hidden, dtype=torch.bfloat16, device=dev)
+            send = torch.tensor(counts, dtype=torch.int64, device=dev)
+            reps = reps_for(nbytes * size // 2)
+            row = {}
+            us = time_graph(lambda: m.reduce_scatterv(x, send, MPI.SUM, recv_capacity=n, comm=comm), reps)
+            row["ours"] = {"us": round(us, 2), "busbw": bw(us)}
+            i = torch.arange(n, device=dev)
+            idx = torch.where(i < send.view(size, 1), (torch.cumsum(send, 0) - send).view(size, 1) + i, size * n)
+            padded = torch.zeros(size, n, hidden, dtype=x.dtype, device=dev)
+
+            def pad_reduce_scatter():
+                xp = torch.cat([x, x.new_zeros(1, hidden)])
+                return m.reduce_scatter(xp[idx], MPI.SUM, comm=comm)
+
+            us = time_graph(pad_reduce_scatter, reps)
+            row["pad_reduce_scatter"] = {"us": round(us, 2), "busbw": bw(us)}
+            if nccl is not None:
+                out = torch.empty(n, hidden, dtype=x.dtype, device=dev)
+                us = time_nccl(lambda: dist.reduce_scatter_tensor(out, padded.view(size * n, hidden), group=nccl), reps)
+                row["nccl_padded"] = {"us": round(us, 2), "busbw": bw(us)}
+                del out
+            result["reduce_scatterv"][kind][str(nbytes)] = row
+            if rank == 0:
+                print("reduce_scatterv", kind, nbytes, {k: (v["us"], v["busbw"]) for k, v in row.items()}, flush=True)
+            del x, padded
+
+
+if ns.only_reduce_scatterv:
+    reduce_scatterv_rows()
+    if rank == 0:
+        os.makedirs(os.path.dirname(ns.out) or ".", exist_ok=True)
+        with open(ns.out, "w") as f:
+            json.dump(result, f, indent=1)
+    m.flush()
+    sys.exit(0)
 
 if ns.only_allgatherv:
     allgatherv_rows()
@@ -345,6 +402,7 @@ for nbytes in [b for b in sizes if (64 << 10) <= b <= (256 << 20)]:
         del x, y
 
 allgatherv_rows()
+reduce_scatterv_rows()
 
 # ---------------------------------------------------------------- rooted ops + scan (per-rank payload = nbytes)
 result.update({"bcast": {}, "reduce": {}, "gather": {}, "scatter": {}, "scan": {}})

@@ -22,6 +22,8 @@
 
 b2_reduce_launch_fn b2_reduce_table[B2_DTYPE_COUNT][B2_OP_COUNT];
 b2_ll_launch_fn b2_ll_table[B2_DTYPE_COUNT][B2_OP_COUNT];
+b2_rsv_launch_fn b2_rsv_table[B2_DTYPE_COUNT][B2_OP_COUNT];
+const void* b2_rsv_kernel[B2_DTYPE_COUNT][B2_OP_COUNT];
 
 static void b2_ensure_tables() {
   static bool done = false;
@@ -276,8 +278,6 @@ b2_k_move(const __grid_constant__ B2DevComm c, const __grid_constant__ B2MoveArg
 // once -- every rank reads the same segment, from source offset 0.  Only the header write and the
 // schedule (thread-0 code) know the mode; chunks, pulls and the zero fill are shared.
 // ---------------------------------------------------------------------------
-#define B2_A2AV_HDR ((size_t)B2_MAX_RANKS * sizeof(long long))
-
 struct B2AlltoallvArgs {
   const void* in;
   void* out;
@@ -292,22 +292,6 @@ struct B2AlltoallvArgs {
   size_t chunk;
   int opcode;
 };
-
-// zero bytes [lo, hi) of `out`, spread over every thread of the grid
-__device__ __forceinline__ void a2av_zero(char* out, size_t lo, size_t hi) {
-  const size_t gt = (size_t)blockIdx.x * blockDim.x + threadIdx.x, gs = (size_t)gridDim.x * blockDim.x;
-  if (lo >= hi) return;
-  const size_t v0 = lo + ((16 - ((uintptr_t)(out + lo) & 15)) & 15);     // first 16-byte aligned byte
-  const size_t tail = (uintptr_t)(out + hi) & 15;
-  const size_t v1 = hi - tail;                                           // end of the aligned vectors
-  if (hi - lo < 32 || v0 >= v1) {
-    for (size_t i = lo + gt; i < hi; i += gs) out[i] = 0;
-    return;
-  }
-  for (size_t i = lo + gt; i < v0; i += gs) out[i] = 0;
-  for (size_t i = v0 + (gt << 4); i < v1; i += gs << 4) b2_st16(out + i, make_uint4(0, 0, 0, 0));
-  for (size_t i = v1 + gt; i < hi; i += gs) out[i] = 0;
-}
 
 __global__ void __launch_bounds__(B2_THREADS, 1)
 b2_k_rowsv(const __grid_constant__ B2DevComm c, const __grid_constant__ B2AlltoallvArgs a) {
@@ -774,6 +758,8 @@ extern "C" size_t b2_stage_need(int opcode, int nranks, size_t blk_bytes) {
     case B2_OPC_ALLTOALLV:                       // blk_bytes: the most bytes of rows a rank stages
     case B2_OPC_ALLGATHERV:
       return B2_A2AV_HDR + stride + 4096;
+    case B2_OPC_REDUCE_SCATTERV:                 // blk_bytes: the output rows N x row bytes, one block per rank
+      return B2_A2AV_HDR + stride * (size_t)nranks + 4096;
     default:
       return stride + 4096;
   }
@@ -1163,11 +1149,12 @@ extern "C" int b2_alltoallv(B2Comm* c, const void* in, void* out, size_t row_byt
 }
 
 extern "C" int b2_allgatherv(B2Comm* c, const void* in, void* out, size_t row_bytes, size_t in_rows, size_t out_rows,
-                             const long long* count, long long* recv_counts, cudaStream_t stream) {
+                             const long long* count, long long* recv_counts, const long long* place_counts,
+                             cudaStream_t stream) {
   B2DebugScope* dbg = b2_debug_begin(c, "Allgatherv", stream, "with %zu rows of %zu bytes", in_rows, row_bytes);
   B2AlltoallvArgs a;
   memset(&a, 0, sizeof a);
-  a.in = in; a.out = out; a.count = count; a.recv_counts = recv_counts;
+  a.in = in; a.out = out; a.count = count; a.place_counts = place_counts; a.recv_counts = recv_counts;
   a.row_bytes = row_bytes; a.in_rows = in_rows; a.out_rows = out_rows; a.opcode = B2_OPC_ALLGATHERV;
   a.max_rows = in_rows;
   int rc;
@@ -1176,6 +1163,42 @@ extern "C" int b2_allgatherv(B2Comm* c, const void* in, void* out, size_t row_by
     rc = B2_ERR_BAD_ARG;
   } else {
     rc = rowsv_launch(c, a, "allgatherv", stream);
+  }
+  b2_debug_end(dbg, rc);
+  return rc;
+}
+
+// The staging (a header and P blocks of out_rows rows) and the chunk geometry come from out_rows, which
+// every rank agrees on; the input rows may differ between ranks.  Always launched, even for an empty
+// output: recv_counts is written on the device.
+extern "C" int b2_reduce_scatterv(B2Comm* c, const void* in, void* out, size_t row_bytes, size_t in_rows,
+                                  size_t out_rows, const long long* send_counts, long long* recv_counts, int dtype,
+                                  int op, cudaStream_t stream) {
+  B2DebugScope* dbg = b2_debug_begin(c, "Reduce_scatterv", stream, "with %zu rows of %zu bytes via pull", in_rows,
+                                     row_bytes);
+  b2_ensure_tables();
+  int rc;
+  if (dtype < 0 || dtype >= B2_DTYPE_COUNT || op < 0 || op >= B2_OP_COUNT || b2_rsv_table[dtype][op] == nullptr) {
+    b2_set_error("reduce_scatterv: unsupported dtype/op combination (dtype=%d, op=%d)", dtype, op);
+    rc = B2_ERR_BAD_ARG;
+  } else if (send_counts == nullptr || recv_counts == nullptr) {
+    b2_set_error("reduce_scatterv: send_counts and recv_counts must be device arrays of %d int64", c->dev.size);
+    rc = B2_ERR_BAD_ARG;
+  } else if (row_bytes % b2_dtype_size(dtype) != 0) {
+    b2_set_error("reduce_scatterv: %zu-byte rows are not whole elements of dtype %d", row_bytes, dtype);
+    rc = B2_ERR_BAD_ARG;
+  } else {
+    B2RsvArgs a;
+    a.in = in; a.out = out; a.send_counts = send_counts; a.recv_counts = recv_counts;
+    a.row_bytes = row_bytes; a.in_rows = in_rows; a.out_rows = out_rows; a.opcode = B2_OPC_REDUCE_SCATTERV;
+    const size_t blk_bytes = out_rows * row_bytes;
+    rc = check_stage(c, B2_OPC_REDUCE_SCATTERV, blk_bytes, "reduce_scatterv");
+    if (rc == 0) {
+      int grid;
+      pick_chunks(c, blk_bytes, coresident_blocks(c, b2_rsv_kernel[dtype][op]), &a.chunk, &grid);
+      b2_rsv_table[dtype][op](c->dev, a, grid, stream);
+      rc = b2_launched(c, "reduce_scatterv");
+    }
   }
   b2_debug_end(dbg, rc);
   return rc;

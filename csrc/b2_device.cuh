@@ -341,3 +341,19 @@ __device__ __forceinline__ void b2_store_partial(void* dst, uint4 v, int nbytes)
   unsigned char* d = (unsigned char*)dst;
   for (int i = 0; i < nbytes; ++i) d[i] = tmp[i];
 }
+
+// zero bytes [lo, hi) of `out`, spread over every thread of the grid
+__device__ __forceinline__ void a2av_zero(char* out, size_t lo, size_t hi) {
+  const size_t gt = (size_t)blockIdx.x * blockDim.x + threadIdx.x, gs = (size_t)gridDim.x * blockDim.x;
+  if (lo >= hi) return;
+  const size_t v0 = lo + ((16 - ((uintptr_t)(out + lo) & 15)) & 15);     // first 16-byte aligned byte
+  const size_t tail = (uintptr_t)(out + hi) & 15;
+  const size_t v1 = hi - tail;                                           // end of the aligned vectors
+  if (hi - lo < 32 || v0 >= v1) {
+    for (size_t i = lo + gt; i < hi; i += gs) out[i] = 0;
+    return;
+  }
+  for (size_t i = lo + gt; i < v0; i += gs) out[i] = 0;
+  for (size_t i = v0 + (gt << 4); i < v1; i += gs << 4) b2_st16(out + i, make_uint4(0, 0, 0, 0));
+  for (size_t i = v1 + gt; i < hi; i += gs) out[i] = 0;
+}

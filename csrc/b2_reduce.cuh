@@ -227,11 +227,173 @@ b2_k_allreduce_ll(const B2DevComm c, const B2LLArgs a) {
 }
 
 // ---------------------------------------------------------------------------
+// reduce_scatterv: variable row counts that exist only on the device.
+//
+// Staging parity of every rank: [header: this rank's send counts clamped in rank order to its input
+// rows, int64 x B2_MAX_RANKS (B2_A2AV_HDR)] [P blocks of round16(N * row_bytes)].  Block p holds the
+// first min(s_r[p], N) rows of this rank's segment for rank p -- only real rows are staged.
+//
+// The schedule is b2_k_rowsv's: every CTA writes the header and stages its first chunk before its first
+// arrive; after the first wait it reads the P x P counts, and the chunks of a block (bytes, up to the
+// largest min(s_q[p], N) rows of any pair -- the same on every rank) belong to CTA k mod grid everywhere.
+// Chunk k of block r is then folded from every peer's staging, in rank order over the ranks whose
+// segment reaches that element; rows [max_q c[q], N) are zero.
+// ---------------------------------------------------------------------------
+struct B2RsvArgs {
+  const void* in;
+  void* out;
+  const long long* send_counts;    // [P] rows to each rank (any value: clamped here)
+  long long* recv_counts;          // [P] rows folded from each rank
+  size_t row_bytes;
+  size_t in_rows;                  // may differ between ranks
+  size_t out_rows;                 // N: the same on every rank (sizes the staging and the chunks)
+  size_t chunk;
+  int opcode;
+};
+
+// Fold the vector at byte v of block `rank` over the ranks q with v < len[q], in rank order.  Segments
+// are prefixes of the block, so the ranks that reach element j of the vector are exactly those with
+// len[q] > v + j * sizeof(T); `covered` is how far into the vector an earlier rank reached.  The peers'
+// loads are issued RSV_BATCH at a time before any of them is folded, so their NVLink round trips overlap.
+#define RSV_BATCH 4
+template <typename T, int OP>
+__device__ __forceinline__ uint4 rsv_fold(const B2DevComm& c, size_t src, size_t v, const size_t* len) {
+  using Tr = B2Traits<T>;
+  constexpr int N = B2Vec<T>::N;
+  B2Vec<T> acc;
+  size_t covered = 0;
+  for (int q0 = 0; q0 < c.size; q0 += RSV_BATCH) {
+    uint4 x[RSV_BATCH];
+#pragma unroll
+    for (int k = 0; k < RSV_BATCH; ++k) {
+      x[k] = make_uint4(0, 0, 0, 0);
+      if (q0 + k < c.size && v < len[q0 + k]) x[k] = b2_ld_peer16(c.stage[q0 + k] + src + v);
+    }
+#pragma unroll
+    for (int k = 0; k < RSV_BATCH; ++k) {
+      const int q = q0 + k;
+      if (q >= c.size || v >= len[q]) continue;
+      const size_t nb = len[q] - v < 16 ? len[q] - v : 16;
+      if (covered == 0) {
+        acc.load(x[k]);
+      } else if (nb == 16 && covered == 16) {
+        acc.template accumulate<OP>(x[k]);
+      } else {             // a segment ends inside this vector (row_bytes % 16 != 0)
+        alignas(16) T tmp[N];
+        *reinterpret_cast<uint4*>(tmp) = x[k];
+#pragma unroll
+        for (int j = 0; j < N; ++j) {
+          const size_t eb = (size_t)j * sizeof(T);
+          if (eb < nb) {
+            const typename Tr::Acc u = Tr::up(tmp[j]);
+            acc.a[j] = eb < covered ? b2_apply<OP, typename Tr::Acc>(acc.a[j], u) : u;
+          }
+        }
+      }
+      if (nb > covered) covered = nb;
+    }
+  }
+  return acc.store();
+}
+#undef RSV_BATCH
+
+template <typename T, int OP>
+__global__ void __launch_bounds__(B2_THREADS, 1)
+b2_k_reduce_scatterv(const B2DevComm c, const B2RsvArgs a) {
+  __shared__ size_t s_src[B2_MAX_RANKS], s_mine[B2_MAX_RANKS];   // this rank's segments: input byte, staged bytes
+  __shared__ size_t s_len[B2_MAX_RANKS];                         // bytes of block `rank` staged by peer q
+  __shared__ size_t s_cnt[B2_MAX_RANKS][B2_MAX_RANKS];           // [q][p]: min(s_q[p], N)
+  __shared__ size_t s_fold, s_nch;
+  const unsigned ticket = b2_ticket_read(c.ticket);
+  const size_t par = (size_t)(ticket & 1u) * c.stage_half;
+  unsigned e = b2_ld_volatile(c.epoch + blockIdx.x);
+  const int t = threadIdx.x, nt = blockDim.x, P = c.size, r = c.rank;
+  const char* in = (const char*)a.in;
+  char* out = (char*)a.out;
+  char* mine = c.stage[r] + par;
+  const size_t rb = a.row_bytes;
+  const size_t bs = (a.out_rows * rb + 15) & ~(size_t)15;
+  char* blocks = mine + B2_A2AV_HDR;
+  // 1. this rank's counts, clamped in rank order to the rows that exist -> header
+  if (t == 0) {
+    size_t used = 0;
+    for (int p = 0; p < P; ++p) {
+      size_t s = a.send_counts[p] > 0 ? (size_t)a.send_counts[p] : 0;
+      if (s > a.in_rows - used) s = a.in_rows - used;
+      ((volatile unsigned long long*)mine)[p] = s;
+      s_src[p] = used * rb;
+      s_mine[p] = (s < a.out_rows ? s : a.out_rows) * rb;
+      used += s;
+    }
+  }
+  __syncthreads();
+  // chunk ch of every block this rank sends
+  auto stage = [&](size_t ch) {
+    const size_t off = ch * a.chunk;
+    for (int p = 0; p < P; ++p)
+      if (off < s_mine[p]) {
+        const size_t n = s_mine[p] - off < a.chunk ? s_mine[p] - off : a.chunk;
+        b2_copy_bytes<false>(blocks + (size_t)p * bs + off, in + s_src[p] + off, n);
+      }
+  };
+  size_t ch = blockIdx.x;
+  stage(ch);
+  b2_barrier_arrive(c, ++e);
+  unsigned e_cur = e;
+  b2_barrier_wait(c, e_cur, a.opcode);   // every rank's header and chunk blockIdx.x are staged
+  // 2. the peers' headers: what each sends here, and the longest segment of any pair (the loop bound)
+  if (t < P * P) {
+    const unsigned long long h = ((const volatile unsigned long long*)(c.stage[t / P] + par))[t % P];
+    s_cnt[t / P][t % P] = h < a.out_rows ? (size_t)h : a.out_rows;
+  }
+  __syncthreads();
+  if (t == 0) {
+    size_t lmax = 0, cmax = 0;
+    for (int q = 0; q < P; ++q) {
+      for (int p = 0; p < P; ++p)
+        if (s_cnt[q][p] > lmax) lmax = s_cnt[q][p];
+      const size_t k = s_cnt[q][r];
+      s_len[q] = k * rb;
+      if (k > cmax) cmax = k;
+      if (blockIdx.x == 0) a.recv_counts[q] = (long long)k;
+    }
+    s_fold = cmax * rb;
+    s_nch = (lmax * rb + a.chunk - 1) / a.chunk;        // the same on every rank
+  }
+  __syncthreads();
+  // 3. stage -> arrive -> wait -> fold, software-pipelined over the chunks of this CTA
+  const size_t nch = s_nch, fold = s_fold;
+  const size_t src = par + B2_A2AV_HDR + (size_t)r * bs;
+  for (; ch < nch; ch += gridDim.x) {
+    if (ch != blockIdx.x) b2_barrier_wait(c, e_cur, a.opcode);
+    const size_t off = ch * a.chunk;
+    const size_t end = off + a.chunk < fold ? off + a.chunk : fold;
+    for (size_t v = off + ((size_t)t << 4); v < end; v += (size_t)nt << 4) {
+      const uint4 res = rsv_fold<T, OP>(c, src, v, s_len);
+      if (v + 16 <= end) b2_st16(out + v, res);
+      else b2_store_partial(out + v, res, (int)(end - v));
+    }
+    const size_t nxt = ch + gridDim.x;
+    if (nxt < nch) {
+      stage(nxt);
+      b2_barrier_arrive(c, ++e);
+      e_cur = e;
+    }
+  }
+  // 4. rows nobody sends are zero: the output is fully written on every call
+  a2av_zero(out, fold, a.out_rows * rb);
+  __syncthreads();
+  if (t == 0) b2_st_volatile(c.epoch + blockIdx.x, e);
+  b2_finish_bump(c.ticket, c.ticket + 1, 1u, gridDim.x);
+}
+
+// ---------------------------------------------------------------------------
 // host-side typed dispatch.  Each b2_reduce_inst_N.cu registers the launchers of
 // one dtype group (keeps nvcc parallel and fast); the caller checks the launch.
 // ---------------------------------------------------------------------------
 typedef void (*b2_reduce_launch_fn)(const B2DevComm&, const B2ReduceArgs&, int grid, cudaStream_t);
 typedef void (*b2_ll_launch_fn)(const B2DevComm&, const B2LLArgs&, int grid, cudaStream_t);
+typedef void (*b2_rsv_launch_fn)(const B2DevComm&, const B2RsvArgs&, int grid, cudaStream_t);
 
 template <typename T, int OP>
 void b2_launch_reduce(const B2DevComm& c, const B2ReduceArgs& a, int grid, cudaStream_t s) {
@@ -241,18 +403,27 @@ template <typename T, int OP>
 void b2_launch_ll(const B2DevComm& c, const B2LLArgs& a, int grid, cudaStream_t s) {
   b2_k_allreduce_ll<T, OP><<<grid, B2_THREADS, 0, s>>>(c, a);
 }
+template <typename T, int OP>
+void b2_launch_rsv(const B2DevComm& c, const B2RsvArgs& a, int grid, cudaStream_t s) {
+  b2_k_reduce_scatterv<T, OP><<<grid, B2_THREADS, 0, s>>>(c, a);
+}
 
-// tables filled by the instance files: [dtype][op] -> launcher (nullptr = invalid combo)
+// tables filled by the instance files: [dtype][op] -> launcher (nullptr = invalid combo); b2_rsv_kernel
+// holds the kernel itself, for the co-residency query
 extern b2_reduce_launch_fn b2_reduce_table[B2_DTYPE_COUNT][B2_OP_COUNT];
 extern b2_ll_launch_fn b2_ll_table[B2_DTYPE_COUNT][B2_OP_COUNT];
+extern b2_rsv_launch_fn b2_rsv_table[B2_DTYPE_COUNT][B2_OP_COUNT];
+extern const void* b2_rsv_kernel[B2_DTYPE_COUNT][B2_OP_COUNT];
 void b2_register_reduce_group_0();
 void b2_register_reduce_group_1();
 void b2_register_reduce_group_2();
 void b2_register_reduce_group_3();
 
-#define B2_REG(DT, T, OP)                               \
-  b2_reduce_table[DT][OP] = &b2_launch_reduce<T, OP>;   \
-  b2_ll_table[DT][OP] = &b2_launch_ll<T, OP>;
+#define B2_REG(DT, T, OP)                                                \
+  b2_reduce_table[DT][OP] = &b2_launch_reduce<T, OP>;                    \
+  b2_ll_table[DT][OP] = &b2_launch_ll<T, OP>;                            \
+  b2_rsv_table[DT][OP] = &b2_launch_rsv<T, OP>;                          \
+  b2_rsv_kernel[DT][OP] = (const void*)&b2_k_reduce_scatterv<T, OP>;
 
 #define B2_REG_ARITH(DT, T) \
   B2_REG(DT, T, B2_SUM) B2_REG(DT, T, B2_PROD) B2_REG(DT, T, B2_MIN) B2_REG(DT, T, B2_MAX)

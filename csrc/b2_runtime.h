@@ -161,11 +161,22 @@ int b2_alltoallv(B2Comm* c, const void* in, void* out, size_t row_bytes, size_t 
                  cudaStream_t stream);
 // Variable-count allgather whose counts stay on the device.  `in`: in_rows rows of row_bytes bytes
 // (contiguous, in_rows the same on every rank); `count`: one int64 on the device, clamped to
-// [0, in_rows]; `recv_counts`: [nranks] int64.  The segments of all ranks are packed in rank order and
-// clipped to out_rows; output rows past the last one received are zeroed; recv_counts holds the rows
-// written from each rank.
+// [0, in_rows]; `recv_counts`: [nranks] int64.  Forward (place_counts null): the segments of all ranks
+// are packed in rank order and clipped to out_rows.  Reverse (place_counts: [nranks] int64, the send
+// counts of a reduce_scatterv): the segment from rank q lands at the sum of place_counts[p] over p < q,
+// at most place_counts[q] rows of it, all clamped in rank order to out_rows.  Output rows that receive
+// nothing are zeroed; recv_counts holds the rows written from each rank.
 int b2_allgatherv(B2Comm* c, const void* in, void* out, size_t row_bytes, size_t in_rows, size_t out_rows,
-                  const long long* count, long long* recv_counts, cudaStream_t stream);
+                  const long long* count, long long* recv_counts, const long long* place_counts,
+                  cudaStream_t stream);
+// Variable-count reduce-scatter whose counts stay on the device.  `in`: in_rows rows of row_bytes bytes
+// (contiguous; in_rows may differ between ranks); `send_counts`: [nranks] int64, clamped in rank order
+// to in_rows; out_rows (N) must be the same on every rank.  Row i of `out` is `op` folded in rank order
+// over the ranks q whose segment for this rank has more than i rows (at most N), rows past the longest
+// segment are zeroed; `recv_counts`: [nranks] int64, min(send_counts_q[rank], N).
+int b2_reduce_scatterv(B2Comm* c, const void* in, void* out, size_t row_bytes, size_t in_rows, size_t out_rows,
+                       const long long* send_counts, long long* recv_counts, int dtype, int op,
+                       cudaStream_t stream);
 
 // --- point to point ----------------------------------------------------------
 // source/tag may be -1 (ANY).  `status` is a host-mapped B2StatusRecord or null.

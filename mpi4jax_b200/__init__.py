@@ -27,6 +27,7 @@ from ._src import (  # noqa: F401
     recv,
     reduce,
     reduce_scatter,
+    reduce_scatterv,
     scan,
     scatter,
     send,
@@ -42,7 +43,7 @@ effects_barrier = flush
 
 __all__ = [
     "allgather", "allgatherv", "allreduce", "alltoall", "alltoallv", "barrier", "bcast", "gather", "recv", "reduce",
-    "reduce_scatter", "scan", "scatter", "send", "sendrecv", "has_cuda_support", "has_sycl_support",
+    "reduce_scatter", "reduce_scatterv", "scan", "scatter", "send", "sendrecv", "has_cuda_support", "has_sycl_support",
     "MPI", "jit", "compiled", "flush", "effects_barrier", "linear_transpose", "send_with_grad", "comm_reserve",
     "symmetric_empty", "allreduce_",
 ]

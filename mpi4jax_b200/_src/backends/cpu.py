@@ -95,6 +95,14 @@ def reduce_stack(stack: torch.Tensor, op_code: int) -> torch.Tensor:
     return acc.to(dt)
 
 
+def check_op(dtype: torch.dtype, op_code: int) -> None:
+    """Refuse a dtype / op pair that ``reduce_stack`` (and the CUDA kernels) do not define, with its error."""
+    if dtype.is_complex and op_code not in (codes.SUM, codes.PROD):
+        raise NotImplementedError("only SUM and PROD are defined for complex dtypes")
+    if dtype.is_floating_point and op_code not in (codes.SUM, codes.PROD, codes.MIN, codes.MAX):
+        raise NotImplementedError("logical/bitwise reductions need an integer or bool dtype")
+
+
 class CpuState:
     """Per-communicator host-side p2p state (unexpected queues, pending sends)."""
 
@@ -205,13 +213,38 @@ def alltoallv(comm: Comm, x: torch.Tensor, send_counts: torch.Tensor, out_rows: 
     return _pack(stack, [row[r] for row in counts], [sum(row[:r]) for row in counts], out_rows, place)
 
 
-def allgatherv(comm: Comm, x: torch.Tensor, count: torch.Tensor, out_rows: int):
+def allgatherv(comm: Comm, x: torch.Tensor, count: torch.Tensor, out_rows: int,
+               place_counts: Optional[torch.Tensor] = None):
     """Same rules as the kernel's gather mode (csrc/b2_collectives.cu: b2_k_rowsv): alltoallv where every rank
     sends its first ``count`` rows to every rank, each segment from row 0 of its source (correctness
     path)."""
     n = min(max(int(count), 0), x.shape[0])
     counts = _gather_stack(comm, torch.tensor(n, dtype=torch.int64)).tolist()
-    return _pack(_gather_stack(comm, x), counts, [0] * comm.size, out_rows)
+    place = None if place_counts is None else _clamp_in_order(place_counts.tolist(), out_rows)
+    return _pack(_gather_stack(comm, x), counts, [0] * comm.size, out_rows, place)
+
+
+def reduce_scatterv(comm: Comm, x: torch.Tensor, send_counts: torch.Tensor, out_rows: int, op_code: int):
+    """Same rules as the kernel (csrc/b2_reduce.cuh: b2_k_reduce_scatterv): everybody gathers every rank's
+    clamped counts and rows, padded to a common width, then folds the segments for its own rank -- each
+    run of rows over the ranks whose segment reaches it, in rank order (correctness path)."""
+    P, r = comm.size, comm.rank
+    check_op(x.dtype, op_code)         # on every call, also when no row has two contributors
+    sent = _clamp_in_order(send_counts.tolist(), x.shape[0])
+    counts = _gather_stack(comm, torch.tensor(sent, dtype=torch.int64)).tolist()       # [q][p]
+    width = max(sum(row) for row in counts)
+    mine = torch.zeros((width, *x.shape[1:]), dtype=x.dtype)
+    mine[: sum(sent)] = x[: sum(sent)]
+    stack = _gather_stack(comm, mine)                                                   # (P, width, *S)
+    recv = [min(row[r], out_rows) for row in counts]
+    displ = [sum(row[:r]) for row in counts]
+    out = torch.zeros((out_rows, *x.shape[1:]), dtype=x.dtype)
+    lo = 0
+    for hi in sorted(set(recv) - {0}):          # rows [lo, hi) have the same contributors
+        qs = [q for q in range(P) if recv[q] >= hi]
+        out[lo:hi] = reduce_stack(torch.stack([stack[q, displ[q] + lo: displ[q] + hi] for q in qs]), op_code)
+        lo = hi
+    return out, torch.tensor(recv, dtype=torch.int64)
 
 
 def bcast(comm: Comm, x: torch.Tensor, root: int) -> torch.Tensor:

@@ -63,6 +63,8 @@ def stage_need(opcode: int, nranks: int, blk_bytes: int) -> int:
     stride = (blk_bytes + 15) & ~15
     if opcode in (codes.OPC_ALLTOALLV, codes.OPC_ALLGATHERV):    # a header of the counts in front of the rows
         return ALLTOALLV_HEADER + stride + 4096
+    if opcode == codes.OPC_REDUCE_SCATTERV:                        # the header, then one block per rank
+        return ALLTOALLV_HEADER + stride * nranks + 4096
     mult = nranks if opcode in (codes.OPC_ALLTOALL, codes.OPC_SCATTER, codes.OPC_REDUCE_SCATTER) else 1
     return stride * mult + 4096
 
@@ -561,15 +563,28 @@ class NativeComm:
         return self._rowsv(_lib().b2_alltoallv, "Alltoallv", codes.OPC_ALLTOALLV, max_rows, x, out_rows,
                            send_counts, None if place_counts is None else place_counts.data_ptr())
 
-    def allgatherv(self, x: torch.Tensor, count: torch.Tensor, out_rows: int):
+    def allgatherv(self, x: torch.Tensor, count: torch.Tensor, out_rows: int,
+                   place_counts: Optional[torch.Tensor] = None):
         """``(out, recv_counts)``: the first ``count`` rows of every rank's ``x``, packed in rank order
-        (``collective_ops/allgatherv.py`` states the rules); the count is read on the device."""
-        return self._rowsv(_lib().b2_allgatherv, "Allgatherv", codes.OPC_ALLGATHERV, x.shape[0], x, out_rows, count)
+        (``collective_ops/allgatherv.py`` states the rules); the count is read on the device.
+        ``place_counts``: the reverse mode, the adjoint of a reduce_scatterv with these send counts."""
+        if place_counts is not None:
+            place_counts = place_counts.to(torch.int64).contiguous()
+        return self._rowsv(_lib().b2_allgatherv, "Allgatherv", codes.OPC_ALLGATHERV, x.shape[0], x, out_rows, count,
+                           None if place_counts is None else place_counts.data_ptr())
+
+    def reduce_scatterv(self, x: torch.Tensor, send_counts: torch.Tensor, out_rows: int, op_code: int):
+        """``(out, recv_counts)``: ``op`` over the ranks' segments for this rank, folded in rank order
+        (``collective_ops/reduce_scatterv.py`` states the rules); the counts are read on the device."""
+        x, dt, op_code = _prep_reduce(x, op_code)
+        return self._rowsv(_lib().b2_reduce_scatterv, "Reduce_scatterv", codes.OPC_REDUCE_SCATTERV, out_rows, x,
+                           out_rows, send_counts, dt, op_code)
 
     def _rowsv(self, fn, opname: str, opcode: int, stage_rows: int, x: torch.Tensor, out_rows: int,
-               counts: torch.Tensor, *place_ptr):
-        """Calls ``fn`` (b2_alltoallv / b2_allgatherv) with staging for ``stage_rows`` rows of ``x``;
-        ``place_ptr``: alltoallv's place counts."""
+               counts: torch.Tensor, *extra):
+        """Calls ``fn`` (b2_alltoallv / b2_allgatherv / b2_reduce_scatterv) with staging for ``stage_rows``
+        rows of ``x`` (per block: see ``stage_need``); ``extra``: the place counts of alltoallv and
+        allgatherv, or reduce_scatterv's dtype and op codes."""
         x = _prep(x)
         row_bytes = math.prod(x.shape[1:]) * x.element_size()
         out = torch.empty((out_rows, *x.shape[1:]), dtype=x.dtype, device=x.device)
@@ -577,7 +592,7 @@ class NativeComm:
         counts = counts.to(torch.int64).contiguous()
         self.ensure_stage(opcode, stage_rows * row_bytes)
         rc = fn(self.handle, x.data_ptr(), out.data_ptr(), row_bytes, x.shape[0], out_rows, counts.data_ptr(),
-                recv_counts.data_ptr(), *place_ptr, self._stream())
+                recv_counts.data_ptr(), *extra, self._stream())
         self._check(rc, opname)
         return out, recv_counts
 
@@ -691,7 +706,8 @@ def _nvtx_wrap(name: str, fn):
 #: ``MPI4JAX_B200_NVTX=1``: one NVTX range per op (visible in Nsight Systems timelines); the
 #: methods are left untouched otherwise, so the fast path pays nothing (SURVEY 5.1)
 NVTX_OPS = ("barrier", "allreduce", "reduce", "scan", "allgather", "alltoall", "bcast", "gather", "scatter",
-            "send", "recv", "sendrecv", "reduce_scatter", "alltoallv", "allgatherv", "gemm_allreduce",
+            "send", "recv", "sendrecv", "reduce_scatter", "alltoallv", "allgatherv", "reduce_scatterv",
+            "gemm_allreduce",
             "halo_exchange")
 if env_flag("MPI4JAX_B200_NVTX", False):
     for _name in NVTX_OPS:

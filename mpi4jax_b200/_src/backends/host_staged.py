@@ -94,8 +94,13 @@ class HostStagedComm:
                                           None if place_counts is None else self._down(place_counts))
         return self._up(out, x), self._up(recv_counts, x)
 
-    def allgatherv(self, x, count, out_rows: int):
-        out, recv_counts = _cpu.allgatherv(self.comm, self._down(x), self._down(count), out_rows)
+    def allgatherv(self, x, count, out_rows: int, place_counts=None):
+        out, recv_counts = _cpu.allgatherv(self.comm, self._down(x), self._down(count), out_rows,
+                                           None if place_counts is None else self._down(place_counts))
+        return self._up(out, x), self._up(recv_counts, x)
+
+    def reduce_scatterv(self, x, send_counts, out_rows: int, op_code: int):
+        out, recv_counts = _cpu.reduce_scatterv(self.comm, self._down(x), self._down(send_counts), out_rows, op_code)
         return self._up(out, x), self._up(recv_counts, x)
 
     def bcast(self, x, root: int):

@@ -40,24 +40,17 @@ def alltoallv(F, g, comm, rows, send_counts, recv_counts, place_counts):
     return F.alltoallv(g, place_counts, recv_capacity=rows, comm=comm)[0]
 
 
-def segments(g: torch.Tensor, recv_counts: torch.Tensor, rows: int) -> torch.Tensor:
-    """``G`` of shape ``(P, rows, *S)`` with ``G[q, i] = g[o[q] + i]`` for ``i < recv_counts[q]`` and 0
-    otherwise, where ``o`` is the exclusive prefix sum of ``recv_counts``: the segments of an allgatherv
-    output, each back at the start of its source's rows.  Device ops only (no host read of the counts);
-    differentiable in ``g``."""
-    P = recv_counts.shape[0]
-    offsets = torch.cumsum(recv_counts, 0) - recv_counts
-    i = torch.arange(rows, device=g.device)
-    # entries past a segment read a zero row appended to g (index g.shape[0])
-    idx = torch.where(i < recv_counts.view(P, 1), offsets.view(P, 1) + i, g.shape[0])
-    padded = torch.cat([g, g.new_zeros((1, *g.shape[1:]))])
-    return padded[idx]
-
-
 def allgatherv(F, g, comm, rows, recv_counts):
-    """SUM: the received segments, zero-padded to ``(P, rows, *S)``, reduce-scattered, so rank r gets the
-    rank-order sum of what the receivers kept of its rows."""
-    return F.reduce_scatter(segments(g, recv_counts, rows), SUM, comm=comm)
+    """SUM: each received segment travels back to its source, which folds them in rank order into its
+    ``rows`` input rows.  ``recv_counts``: the forward call's (the segments are packed), or in the reverse
+    mode its place counts (the segments lie where a reduce_scatterv took them from)."""
+    return F.reduce_scatterv(g.contiguous(), recv_counts, SUM, recv_capacity=rows, comm=comm)[0]
+
+
+def reduce_scatterv(F, g, comm, rows, send_counts):
+    """SUM: the reverse-mode allgatherv of the cotangent -- every rank's result rows land on each rank where
+    its segment for that rank came from, in an output of the differentiated call's ``rows`` input rows."""
+    return F._allgatherv_reverse(g.contiguous(), send_counts, rows, comm)
 
 
 def bcast(F, g, root, comm):

@@ -165,11 +165,11 @@ def as_counts(counts, x: torch.Tensor, scalar: bool = False) -> torch.Tensor:
 
 def check_rowsv_args(opname: str, comm: Comm, x: torch.Tensor, counts: torch.Tensor, out_rows: int,
                      name: str) -> None:
-    """Host-side checks of an alltoallv / allgatherv call.  Every entry point (the op, its ``compiled``
-    twin, the raw ``torch.ops`` op and its fake kernel, the backends) passes through them: the kernel
-    dereferences the counts as int64 values in x's device memory -- ``nproc`` of them for alltoallv, one
-    for allgatherv -- so anything else must be refused before the launch."""
-    shape, shape_text = ((), "()") if opname == "Allgatherv" else ((comm.Get_size(),), "(nproc,)")
+    """Host-side checks of an alltoallv / allgatherv / reduce_scatterv call.  Every entry point (the op, its
+    ``compiled`` twin, the raw ``torch.ops`` op and its fake kernel, the backends) passes through them: the
+    kernel dereferences the counts as int64 values in x's device memory -- one for allgatherv's ``count``,
+    ``nproc`` for every other counts argument -- so anything else must be refused before the launch."""
+    shape, shape_text = ((), "()") if name == "count" else ((comm.Get_size(),), "(nproc,)")
     check_rows(opname, x)
     if not isinstance(counts, torch.Tensor):
         raise TypeError(f"{opname} {name} must be an integer tensor (got {type(counts).__name__})")
@@ -185,16 +185,20 @@ def check_rowsv_args(opname: str, comm: Comm, x: torch.Tensor, counts: torch.Ten
 
 def rowsv_capacity(opname: str, comm: Comm, x: torch.Tensor, counts: torch.Tensor, recv_capacity,
                    name: str):
-    """The output rows of a public alltoallv / allgatherv call or its ``compiled`` twin, after the checks:
-    ``recv_capacity``, or ``N * nproc``, which never drops a row."""
+    """The output rows of a public alltoallv / allgatherv / reduce_scatterv call or its ``compiled`` twin,
+    after the checks: ``recv_capacity``, or by default the rows that never drop one -- ``N * nproc`` for the
+    gathering ops, ``N`` for reduce_scatterv (when every rank passes ``N`` rows)."""
     check_rows(opname, x)
-    out_rows = x.shape[0] * comm.Get_size() if recv_capacity is None else recv_capacity
+    if recv_capacity is not None:
+        out_rows = recv_capacity
+    else:
+        out_rows = x.shape[0] * (1 if opname == "Reduce_scatterv" else comm.Get_size())
     check_rowsv_args(opname, comm, x, counts, out_rows, name)
     return out_rows
 
 
 def _cpu_rowsv(opname: str, fn, comm: Comm, x: torch.Tensor, *args):
-    """``fn(comm, x, *args)``, the CPU backend's alltoallv / allgatherv, with its log line."""
+    """``fn(comm, x, *args)``, the CPU backend's alltoallv / allgatherv / reduce_scatterv, with its log line."""
     row_bytes = math.prod(x.shape[1:]) * x.element_size()
     done = _log(comm, opname, f"with {x.shape[0]} rows of {row_bytes} bytes")
     out = fn(comm, x, *args)
@@ -214,12 +218,23 @@ def alltoallv(comm: Comm, x: torch.Tensor, send_counts: torch.Tensor, out_rows: 
     return _cpu_rowsv("Alltoallv", _cpu.alltoallv, comm, x, send_counts, out_rows, place_counts)
 
 
-def allgatherv(comm: Comm, x: torch.Tensor, count: torch.Tensor, out_rows: int):
+def allgatherv(comm: Comm, x: torch.Tensor, count: torch.Tensor, out_rows: int,
+               place_counts: Optional[torch.Tensor] = None):
     _plain(x)
     check_rowsv_args("Allgatherv", comm, x, count, out_rows, "count")
+    if place_counts is not None:
+        check_rowsv_args("Allgatherv", comm, x, place_counts, out_rows, "place_counts")
     if x.is_cuda:
-        return comm._native_comm().allgatherv(x, count, out_rows)
-    return _cpu_rowsv("Allgatherv", _cpu.allgatherv, comm, x, count, out_rows)
+        return comm._native_comm().allgatherv(x, count, out_rows, place_counts)
+    return _cpu_rowsv("Allgatherv", _cpu.allgatherv, comm, x, count, out_rows, place_counts)
+
+
+def reduce_scatterv(comm: Comm, x: torch.Tensor, send_counts: torch.Tensor, out_rows: int, op_code: int):
+    _plain(x)
+    check_rowsv_args("Reduce_scatterv", comm, x, send_counts, out_rows, "send_counts")
+    if x.is_cuda:
+        return comm._native_comm().reduce_scatterv(x, send_counts, out_rows, op_code)
+    return _cpu_rowsv("Reduce_scatterv", _cpu.reduce_scatterv, comm, x, send_counts, out_rows, op_code)
 
 
 def bcast(comm: Comm, x: torch.Tensor, root: int) -> torch.Tensor:

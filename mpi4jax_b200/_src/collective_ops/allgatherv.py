@@ -19,9 +19,10 @@ An invalid count is never an error and never makes the kernel read or write out 
 GPU: alltoallv's kernel in gather mode (csrc/b2_collectives.cu: b2_k_rowsv).  Every rank stages its
 ``n_r`` rows once, behind a header holding ``n_r``; after one barrier each CTA reads the P headers,
 derives the packed offsets itself and pulls its chunks of every peer's segment, each read from offset
-0, straight into the output.  Differentiable: the adjoint (SUM)
-cuts every received segment out of the cotangent into a ``(P, N, *S)`` tensor, zero-padded, and
-reduce-scatters it, so rank r gets the rank-order sum of what the receivers kept of its rows.
+0, straight into the output.  Differentiable: the adjoint is ``reduce_scatterv`` of the cotangent with
+the received counts as send counts, so rank r gets the rank-order sum of what the receivers kept of its
+rows, and only those rows travel.  The kernel's *reverse mode* (place counts) is in turn the adjoint of
+``reduce_scatterv``.
 """
 
 from __future__ import annotations
@@ -38,13 +39,17 @@ from . import _adjoints, _dispatch
 
 
 class _Allgatherv(torch.autograd.Function):
+    """``place_counts`` None: the forward gather into ``out_rows`` packed rows.  Otherwise the reverse mode:
+    ``place_counts`` are a reduce_scatterv's send counts and ``out_rows`` its input rows; the segment from
+    rank q lands where that call took rank q's rows from."""
+
     @staticmethod
-    def forward(x, count, out_rows, comm):
-        return _dispatch.allgatherv(comm, x, count, out_rows)
+    def forward(x, count, out_rows, place_counts, comm):
+        return _dispatch.allgatherv(comm, x, count, out_rows, place_counts)
 
     @staticmethod
     def setup_context(ctx, inputs, output):
-        x, ctx.count, ctx.out_rows, ctx.comm = inputs
+        x, ctx.count, ctx.out_rows, ctx.place_counts, ctx.comm = inputs
         ctx.in_rows = x.shape[0]
         ctx.mark_non_differentiable(output[1])
         ctx.save_for_backward(output[1])
@@ -52,22 +57,23 @@ class _Allgatherv(torch.autograd.Function):
     @staticmethod
     def backward(ctx, g, _g_counts):
         (recv_counts,) = ctx.saved_tensors
-        return _adjoints.allgatherv(collective_ops.eager, g, ctx.comm, ctx.in_rows, recv_counts), None, None, None
+        counts = recv_counts if ctx.place_counts is None else ctx.place_counts
+        return _adjoints.allgatherv(collective_ops.eager, g, ctx.comm, ctx.in_rows, counts), None, None, None, None
 
     @staticmethod
     def jvp(ctx, x_t, *_):
-        out_t, _counts = _Allgatherv.apply(x_t, ctx.count, ctx.out_rows, ctx.comm)
+        out_t, _counts = _Allgatherv.apply(x_t, ctx.count, ctx.out_rows, ctx.place_counts, ctx.comm)
         return out_t, None
 
     @staticmethod
-    def vmap(info, in_dims, x, count, out_rows, comm):
-        if in_dims[1] is not None:
+    def vmap(info, in_dims, x, count, out_rows, place_counts, comm):
+        if in_dims[1] is not None or in_dims[3] is not None:
             raise ValueError("allgatherv under vmap: the count must not be batched (one exchange moves every "
                              "batch entry)")
         if in_dims[0] is None:
-            return _Allgatherv.apply(x, count, out_rows, comm), (None, None)
+            return _Allgatherv.apply(x, count, out_rows, place_counts, comm), (None, None)
         # keep the row axis in front: (B, N, *S) -> (N, B, *S), gathered as one message of B-times larger rows
-        out, counts = _Allgatherv.apply(x.movedim(in_dims[0], 1).contiguous(), count, out_rows, comm)
+        out, counts = _Allgatherv.apply(x.movedim(in_dims[0], 1).contiguous(), count, out_rows, place_counts, comm)
         return (out, counts), (1, None)
 
 
@@ -99,4 +105,17 @@ def allgatherv(x, count, *, recv_capacity=None, comm=None, token=NOTSET):
     cap = int(_dispatch.rowsv_capacity("Allgatherv", comm, x, count, recv_capacity, "count"))
     if not needs_autograd(x):
         return _dispatch.allgatherv(comm, x, count, cap)
-    return _Allgatherv.apply(x, count, cap, comm)
+    return _Allgatherv.apply(x, count, cap, None, comm)
+
+
+def allgatherv_reverse(y: torch.Tensor, place_counts: torch.Tensor, rows: int, comm: Comm) -> torch.Tensor:
+    """The adjoint of ``reduce_scatterv(x, place_counts, SUM)`` (``y`` laid out like its output, ``rows``
+    its input rows): every rank's ``y`` travels to every rank q and lands where q took its segment for
+    that rank from -- at most ``min(place_counts_q[p], len(y))`` rows from rank p, the counts clamped in
+    rank order to ``rows``.  Other rows are zero.  Differentiable (the adjoint is reduce_scatterv)."""
+    place_counts = _dispatch.as_counts(place_counts, y)
+    count = torch.full((), y.shape[0], dtype=torch.int64, device=y.device)
+    _dispatch.check_rowsv_args("Allgatherv", comm, y, place_counts, rows, "place_counts")
+    if not needs_autograd(y):
+        return _dispatch.allgatherv(comm, y, count, rows, place_counts)[0]
+    return _Allgatherv.apply(y, count, rows, place_counts, comm)[0]

@@ -1,4 +1,4 @@
-"""``torch.library`` registration of the 15 ops -- the traceable frontend.
+"""``torch.library`` registration of the ops -- the traceable frontend.
 
 The reference's ops are JAX *primitives*: abstract-eval rules give shapes, an ordered effect
 threads a token through every custom call so XLA keeps them in program order
@@ -177,29 +177,62 @@ _alltoallv.register_autograd(_alltoallv_backward, setup_context=_alltoallv_setup
 
 
 @custom_op("mpi4jax_b200::allgatherv", mutates_args=())
-def _allgatherv(x: torch.Tensor, count: torch.Tensor, out_rows: int, comm_id: int) -> tuple[torch.Tensor, torch.Tensor]:
-    return _dispatch.allgatherv(_c(comm_id), x.contiguous(), count, out_rows)
+def _allgatherv(x: torch.Tensor, count: torch.Tensor, out_rows: int, comm_id: int,
+                place_counts: Optional[torch.Tensor] = None) -> tuple[torch.Tensor, torch.Tensor]:
+    return _dispatch.allgatherv(_c(comm_id), x.contiguous(), count, out_rows, place_counts)
 
 
 @_allgatherv.register_fake
-def _(x, count, out_rows, comm_id):
+def _(x, count, out_rows, comm_id, place_counts=None):
     comm = _c(comm_id)
     _dispatch.check_rowsv_args("Allgatherv", comm, x, count, out_rows, "count")
+    if place_counts is not None:
+        _dispatch.check_rowsv_args("Allgatherv", comm, x, place_counts, out_rows, "place_counts")
     return x.new_empty((out_rows, *x.shape[1:])), x.new_empty((comm.Get_size(),), dtype=torch.int64)
 
 
 def _allgatherv_setup(ctx, inputs, output):
-    x, _, _, ctx.comm_id = inputs
+    x, _, _, ctx.comm_id, place_counts = inputs
     ctx.in_rows = x.shape[0]
-    ctx.save_for_backward(output[1])
+    ctx.save_for_backward(output[1], place_counts)
 
 
 def _allgatherv_backward(ctx, g, _g_counts):
-    (recv_counts,) = ctx.saved_tensors
-    return _adjoints.allgatherv(compiled, g, _c(ctx.comm_id), ctx.in_rows, recv_counts), None, None, None
+    recv_counts, place_counts = ctx.saved_tensors
+    counts = recv_counts if place_counts is None else place_counts
+    return _adjoints.allgatherv(compiled, g, _c(ctx.comm_id), ctx.in_rows, counts), None, None, None, None
 
 
 _allgatherv.register_autograd(_allgatherv_backward, setup_context=_allgatherv_setup)
+
+
+@custom_op("mpi4jax_b200::reduce_scatterv", mutates_args=())
+def _reduce_scatterv(x: torch.Tensor, send_counts: torch.Tensor, out_rows: int, op: int,
+                     comm_id: int) -> tuple[torch.Tensor, torch.Tensor]:
+    return _dispatch.reduce_scatterv(_c(comm_id), x.contiguous(), send_counts, out_rows, op)
+
+
+@_reduce_scatterv.register_fake
+def _(x, send_counts, out_rows, op, comm_id):
+    comm = _c(comm_id)
+    _dispatch.check_rowsv_args("Reduce_scatterv", comm, x, send_counts, out_rows, "send_counts")
+    return x.new_empty((out_rows, *x.shape[1:])), x.new_empty((comm.Get_size(),), dtype=torch.int64)
+
+
+def _reduce_scatterv_setup(ctx, inputs, output):
+    x, send_counts, _, ctx.op, ctx.comm_id = inputs
+    ctx.in_rows = x.shape[0]
+    ctx.save_for_backward(send_counts)
+
+
+def _reduce_scatterv_backward(ctx, g, _g_counts):
+    if ctx.op != SUM.code:
+        raise NotImplementedError("The adjoint of reduce_scatterv is only defined for SUM")
+    (send_counts,) = ctx.saved_tensors
+    return _adjoints.reduce_scatterv(compiled, g, _c(ctx.comm_id), ctx.in_rows, send_counts), None, None, None, None
+
+
+_reduce_scatterv.register_autograd(_reduce_scatterv_backward, setup_context=_reduce_scatterv_setup)
 
 
 @custom_op("mpi4jax_b200::bcast", mutates_args=())
@@ -337,7 +370,8 @@ _sendrecv.register_autograd(_sendrecv_backward, setup_context=_sendrecv_setup)
 
 
 ALL_OPS = ("allreduce", "allgather", "alltoall", "bcast", "scan", "reduce", "gather_root", "gather_leaf",
-           "scatter", "barrier", "send", "recv", "sendrecv", "reduce_scatter", "alltoallv", "allgatherv")
+           "scatter", "barrier", "send", "recv", "sendrecv", "reduce_scatter", "alltoallv", "allgatherv",
+           "reduce_scatterv")
 ORDERED_EFFECT = False
 try:  # the ordered effect: AOTAutograd threads a token through these ops in program order
     from torch._higher_order_ops.effects import _EffectType, _register_effectful_op
@@ -393,6 +427,20 @@ class compiled:
         comm = comm or get_default_comm()
         cap = _dispatch.rowsv_capacity("Allgatherv", comm, x, count, recv_capacity, "count")
         return torch.ops.mpi4jax_b200.allgatherv(x, count, cap, comm._id)
+
+    @staticmethod
+    def _allgatherv_reverse(y, place_counts, rows, comm):
+        # the counterpart of the eager allgatherv_reverse, for reduce_scatterv's adjoint (collective_ops/_adjoints.py)
+        count = torch.full((), y.shape[0], dtype=torch.int64, device=y.device)
+        return torch.ops.mpi4jax_b200.allgatherv(y, count, rows, comm._id, place_counts)[0]
+
+    @staticmethod
+    def reduce_scatterv(x, send_counts, op, *, recv_capacity=None, comm=None):
+        """``(out, recv_counts)`` of :func:`mpi4jax_b200.reduce_scatterv` for the built-in operators;
+        ``send_counts`` must be a device tensor of shape ``(nproc,)``."""
+        comm = comm or get_default_comm()
+        cap = _dispatch.rowsv_capacity("Reduce_scatterv", comm, x, send_counts, recv_capacity, "send_counts")
+        return torch.ops.mpi4jax_b200.reduce_scatterv(x, send_counts, cap, as_op(op).code, comm._id)
 
     @staticmethod
     def bcast(x, root, *, comm=None):

@@ -44,5 +44,6 @@ OPC_BCAST, OPC_GATHER, OPC_SCATTER = 6, 7, 8
 OPC_REDUCE_SCATTER = 13
 OPC_ALLTOALLV = 14
 OPC_ALLGATHERV = 15
+OPC_REDUCE_SCATTERV = 16
 
 ANY = -1  # ANY_SOURCE / ANY_TAG on the wire
