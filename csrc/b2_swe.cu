@@ -57,9 +57,11 @@ swe_k34_friction_u(B2SweParams p, const float* __restrict__ u, float* __restrict
                    const float* __restrict__ v, float* __restrict__ fe2, float* __restrict__ fn2,
                    int has_south) {
   b2_pdl_enter();
-  int j, i0;
+  int j, i0 = -1;
   bool m[4];
-  if (!swe_map(p, j, i0, m)) return;
+  // also the group that holds only the east halo column (nx % 4 == 1): u_new's halo cells are copies
+  // of u's, there as everywhere else
+  if (!swe_map(p, j, i0, m) && i0 != p.nx - 1) return;
   swe_k34_body(p, u, u_new, v, fe2, fn2, j, i0, m, has_south != 0);
 }
 

@@ -24,7 +24,9 @@ def halo_exchange(fields: Sequence[torch.Tensor], kinds: Sequence[str], *, west:
     updated in place) with the neighbouring ranks; ``None`` means a physical wall.  The corner
     halo cells come straight from the diagonal neighbours ``sw/se/nw/ne`` (``None`` where the
     row of processes below/above does not exist).
-    ``kinds`` ("h" | "u" | "v") select the wall condition applied after the exchange."""
+    ``kinds`` ("h" | "u" | "v") select the wall condition applied after the exchange.
+    The receive channels of a communicator count messages per side, so every call on one
+    communicator must name the same neighbours; use a ``Clone()`` per neighbour layout."""
     comm = comm or get_default_comm()
     if not fields or not all(f.is_cuda for f in fields):
         raise ValueError("halo_exchange needs CUDA tensors")

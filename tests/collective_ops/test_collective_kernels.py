@@ -5,7 +5,7 @@ result locally: integers in 64-bit arithmetic and then wrapped to the dtype (two
 wrap-around), floats folded in rank order in the accumulate type and rounded once -- the order the
 kernels document ("bitwise identical result on every rank", csrc/b2_reduce.cuh) -- and, as a second
 contract, checked against an extended-precision fold within ``(P-1) u_acc sum|x_q| + ulp/2``.
-That every rank holds the same bits is checked over the control plane (a hash per result).
+That every rank holds the same bits is checked over the control plane (a hash per result, tests/_peer_job.py).
 
 Each transport is forced explicitly (``algorithm=``, communicator options) and the debug log line,
 which names the transport a reduction launched, shows that it was taken.  In a single-process run the
@@ -14,22 +14,19 @@ three ranks (a non-power-of-two world, chunk unit 48 B, the two-phase scan) and 
 with five (the widest pull-and-stage instantiations of b2_k_move)."""
 
 import contextlib
-import hashlib
 import os
 import re
-import tempfile
 import zlib
 
 import numpy as np
 import pytest
 import torch
-import torch.distributed as dist
 
 import mpi4jax_b200 as m
 from mpi4jax_b200 import MPI
 from mpi4jax_b200._src.native import codes, set_logging
 
-from .._peer_job import needs_peers
+from .._peer_job import Checks, expect_passed, job, needs_peers
 
 comm = MPI.COMM_WORLD
 rank = comm.Get_rank()
@@ -203,41 +200,6 @@ def _assert_same(got, want, label):
                                f"got {got[diff][0].item()!r}, want {want[diff][0].item()!r}"
 
 
-def _digest(t):
-    t = t.detach().cpu().contiguous()
-    return hashlib.sha1(t.view(torch.uint8).numpy().tobytes() if t.numel() else b"").hexdigest()
-
-
-class _Checks:
-    """The assertions of a multi-rank test, raised at its end.  A check that fails on one rank only must
-    not leave the ranks running different sequences of collectives, so ``chk(fn, *args)`` records an
-    AssertionError of ``fn(*args)`` and goes on; ``chk.add`` records a hash of a result that every rank
-    must hold bit for bit, and ``chk.finish()`` compares those over the control plane (gloo)."""
-
-    def __init__(self):
-        self.rows = []
-        self.failures = []
-
-    def __call__(self, fn, *args):
-        try:
-            fn(*args)
-        except AssertionError as exc:
-            self.failures.append(str(exc))
-
-    def add(self, label, t):
-        self.rows.append((label, _digest(t)))
-
-    def finish(self):
-        if size > 1:
-            out = [None] * size
-            dist.all_gather_object(out, self.rows, group=comm._group)
-            for q, rows in enumerate(out):
-                for (label, h), (_, h0) in zip(rows, out[0]):
-                    self(_expect, h == h0, f"{label}: rank {q}'s result differs from rank 0's")
-                self(_expect, len(rows) == len(out[0]), f"rank {q} checked {len(rows)} results, rank 0 {len(out[0])}")
-        assert not self.failures, f"{len(self.failures)} checks failed on rank {rank}, the first:\n{self.failures[0]}"
-
-
 def _expect(ok, message):
     assert ok, message
 
@@ -319,7 +281,7 @@ ALL_DTYPES = tuple(codes.DTYPE_CODE)
 @peers
 def test_allreduce_every_dtype_op_and_transport(device, capsys):
     """Every dtype x op x forced transport at 1 element, 17 B and 4095 B (odd vector counts, tails)."""
-    chk = _Checks()
+    chk = Checks()
     for algo in ALGOS:
         for dtype in ALL_DTYPES:
             for opname in _ops_for(dtype) if dtype != torch.bool else OPS:
@@ -333,7 +295,7 @@ def test_allreduce_every_dtype_op_and_transport(device, capsys):
 @peers
 def test_allreduce_sizes_around_vector_and_ll_limits(device, capsys):
     """15 / 16 / 17 B, 4095 B, just below and at the LL capacity, and past it (auto: one-shot or two-shot)."""
-    chk = _Checks()
+    chk = Checks()
     cases = ((torch.float32, "SUM"), (torch.bfloat16, "SUM"), (torch.float16, "PROD"), (torch.int8, "SUM"),
              (torch.uint64, "MAX"), (torch.complex128, "SUM"), (torch.int32, "BXOR"))
     for algo in ALGOS:
@@ -350,7 +312,7 @@ def test_allreduce_sizes_around_vector_and_ll_limits(device, capsys):
 def test_allreduce_multichunk_with_one_or_two_ctas(device, capsys):
     """max_blocks 1 and 2 with 2-4 MiB: chunks are capped at 512 KiB, so every CTA walks several chunks
     (the ``ch += gridDim.x`` loops and a barrier epoch per chunk), in the one-shot and two-shot kernels."""
-    chk = _Checks()
+    chk = Checks()
     for blocks, nbytes in ((1, (2 << 20) + 16), (2, (3 << 20) + 4), (2, 4 << 20)):
         with _options(device, max_blocks=blocks):
             for algo in ("oneshot", "twoshot"):
@@ -405,7 +367,7 @@ def test_allreduce_edge_values(device, capsys):
     """NaN in one rank (MIN / MAX propagate it like numpy), +-inf and +-0.0, fp32 subnormals (no flush
     to zero), INT_MIN / INT_MAX, uint64 values >= 2^63 (an unsigned comparison), wrapping int8 / uint8 /
     uint16 sums and products -- through every transport."""
-    chk = _Checks()
+    chk = Checks()
     for algo in ALGOS:
         for name, dtype, opname, xs in _edge_cases():
             _run_allreduce(device, capsys, chk, None, dtype, opname, xs[0].numel(), algo, xs=xs)
@@ -419,7 +381,7 @@ def test_allreduce_nvls(device):
     nc = comm._native_comm() if device.type == "cuda" else None
     if nc is None or size < 3 or not nc.has_nvls:
         pytest.skip("NVLS needs >= 3 ranks on distinct GPUs with multicast support")
-    chk = _Checks()
+    chk = Checks()
     for dtype in (torch.float32, torch.bfloat16, torch.float16):
         n = (1 << 20) // dtype.itemsize + 8
         xs = [_input(("nvls", str(dtype)), q, n, dtype) for q in range(size)]
@@ -436,7 +398,7 @@ def test_allreduce_nvls(device):
 def test_reduce_roots_dtypes_and_sizes(device, capsys):
     """Roots 0 and P-1; the root gets the rank-order fold, every other rank its input back (its kernel
     runs with has_out = 0)."""
-    chk = _Checks()
+    chk = Checks()
     for root in sorted({0, size - 1}):
         for dtype in ALL_DTYPES:
             for opname in _ops_for(dtype):
@@ -482,7 +444,7 @@ SCAN_CASES = ((torch.float32, "SUM"), (torch.bfloat16, "SUM"), (torch.float64, "
 @peers
 def test_scan_one_phase(device, capsys):
     """Rank r pulls the copies of ranks 0..r; random data, each prefix against its own rank-order fold."""
-    chk = _Checks()
+    chk = Checks()
     for dtype, opname in SCAN_CASES:
         for nbytes in (1, 17, 4095, LL_BYTES + 48):
             n = _n_for(nbytes, dtype)
@@ -494,7 +456,7 @@ def test_scan_one_phase(device, capsys):
 def test_scan_two_phase(device, capsys):
     """P >= 3 with oneshot_max below the message: rank s computes every prefix of sub-slice s and
     writes prefix q into rank q's staging (B2_OPC_SCAN); with one CTA, over several chunks."""
-    chk = _Checks()
+    chk = Checks()
     for blocks, sizes in ((None, (17, 4095, 20000)), (1, ((1 << 20) + 16,))):
         opts = dict(oneshot_max=8) if blocks is None else dict(oneshot_max=8, max_blocks=blocks)
         with _options(device, **opts):
@@ -537,7 +499,7 @@ def _mixed_oracle(ins):
 def test_mixed_call_sequences_eager_and_jit(device):
     """allreduce LL -> two-shot -> reduce -> scan -> allgather -> LL ... with different sizes, eagerly
     and as a captured CUDA graph replayed with new inputs (m.jit: warm-up, capture, replays)."""
-    chk = _Checks()
+    chk = Checks()
     names = ("allreduce ll", "allreduce twoshot", "reduce", "scan", "allgather", "allreduce ll PROD",
              "allreduce oneshot MAX", "allreduce ll BXOR")
     f = m.jit(_mixed_sequence)
@@ -557,7 +519,7 @@ def test_mixed_call_sequences_eager_and_jit(device):
 def test_reduce_scatter_names_its_transport(device, capsys):
     """reduce_scatter sends a block within ll_max by LL and pulls it through the staging otherwise
     (ll_max = 0); the debug line names the transport either way."""
-    chk = _Checks()
+    chk = Checks()
     for ll_max, want_via in ((1 << 30, "ll"), (0, "oneshot")):
         with _options(device, ll_max=ll_max):
             xs = [_input(("rs", ll_max), q, size * 33, torch.float32).reshape(size, 33) for q in range(size)]
@@ -640,7 +602,7 @@ def _move_lead(device, chk, case, shape, dtype, make=None, roots=None):
 def test_move_element_sizes_and_tails(device):
     """Element sizes 1 / 2 / 4 / 8 / 16, blocks of 1, 15, 17 elements (tails), 256 elements (whole
     vectors: the fused pull-and-stage loop), roots != 0."""
-    chk = _Checks()
+    chk = Checks()
     for dtype in MOVE_DTYPES:
         for n in (1, 15, 17, 256):
             _move_all(device, chk, ("tails", n), (n,), dtype)
@@ -652,7 +614,7 @@ def test_move_element_sizes_and_tails(device):
 def test_move_multichunk_one_cta(device):
     """max_blocks = 1 and blocks above 512 KiB: one CTA walks several chunks and stages the next one
     while it pulls the current one (b2_k_move's software pipeline), with and without a tail."""
-    chk = _Checks()
+    chk = Checks()
     with _options(device, max_blocks=1):
         for dtype, n in ((torch.uint8, (1 << 20) + 17), (torch.float32, (600 << 10) // 4 * 3),
                          (torch.complex128, (1 << 20) // 16 + 1)):
@@ -666,7 +628,7 @@ def test_move_strided_inputs(device):
     """Non-contiguous inputs that the movers gather element by element while they stage (the fused
     pack): a transpose, a stepped slice whose base is not 16-byte aligned, a lead stride other than the
     block size, a 4-d layout that does not merge, and a 5-d one (packed by a copy instead)."""
-    chk = _Checks()
+    chk = Checks()
     for dtype in MOVE_DTYPES:
         _move_all(device, chk, "transpose", (7, 12), dtype, make=lambda t: t.t())
         _move_all(device, chk, "stepped slice", (2 * 45 + 1,), dtype, make=lambda t: t[1::2])
@@ -687,7 +649,7 @@ def test_move_bcast_multicast(device):
     nc = comm._native_comm() if device.type == "cuda" else None
     if nc is None or size < 3 or not nc.has_nvls:
         pytest.skip("the multicast bcast needs >= 3 ranks on distinct GPUs with multicast support")
-    chk = _Checks()
+    chk = Checks()
     with _options(device, bcast_mc_min=16):
         for n in (16, 4096 + 3, (1 << 20) + 5):
             want = _bits((n,), torch.uint8, "mc", size - 1)
@@ -702,40 +664,13 @@ def test_move_bcast_multicast(device):
 _inside_job = size > 1 or "MPI4JAX_B200_NESTED" in os.environ
 
 
-def _job(nranks, select, env):
-    from mpi4jax_b200.run import launch
-
-    if not torch.cuda.is_available():
-        pytest.skip("no CUDA device")
-    repo = os.path.dirname(os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
-    test_file = os.path.relpath(os.path.abspath(__file__), repo)
-    args = ["-m", "pytest", test_file, "-q", "-rp", "-m", "gpu", "-k", select, "-p", "no:cacheprovider"]
-    cwd = os.getcwd()
-    os.chdir(repo)
-    try:
-        with tempfile.TemporaryDirectory(prefix=f"mpi4jax-b200-kernels-{nranks}-") as logs:
-            code, _ = launch(nranks, args, timeout=900, output_dir=logs,
-                             env_extra={"MPI4JAX_B200_NESTED": "1", **env})
-            outs = [open(os.path.join(logs, f"rank{r}.log")).read() for r in range(nranks)]
-    finally:
-        os.chdir(cwd)
-    return code, outs
-
-
-def _expect_passed(code, outs, nranks, tests):
-    for r, out in enumerate(outs):
-        missing = [t for t in tests if not re.search(rf"^PASSED .*::{t}\[cuda\]", out, re.M)]
-        assert code == 0 and not missing, \
-            f"rank {r} of the {nranks}-rank job (exit code {code}), not passed: {missing}:\n{out[-4000:]}"
-
-
 @pytest.mark.gpu
 @pytest.mark.skipif(_inside_job, reason="already inside a multi-rank job")
 def test_collective_kernels_three_ranks_gpu():
     """P = 3: a non-power-of-two world (chunk unit 48 B, uneven two-shot splits), the two-phase scan,
     and the <3,1,2> (allgather) and <4,4,1> (alltoall) pull-and-stage loops."""
-    code, outs = _job(3, "not nvls and not multicast", {})
-    _expect_passed(code, outs, 3, [
+    code, outs = job(__file__, 3, "not nvls and not multicast")
+    expect_passed(code, outs, 3, [
         "test_allreduce_every_dtype_op_and_transport", "test_allreduce_sizes_around_vector_and_ll_limits",
         "test_allreduce_multichunk_with_one_or_two_ctas", "test_allreduce_edge_values",
         "test_reduce_roots_dtypes_and_sizes", "test_scan_one_phase", "test_scan_two_phase",
@@ -749,6 +684,6 @@ def test_collective_kernels_three_ranks_gpu():
 def test_collective_kernels_five_ranks_gpu():
     """P = 5, data movement only: the <8,1,1> (allgather) and <8,8,1,SPLIT> (alltoall) instantiations,
     which otherwise need >= 5 GPUs.  Smaller p2p ring slots keep five contexts' rings small."""
-    code, outs = _job(5, "test_move_element_sizes_and_tails or test_move_multichunk_one_cta",
-                      {"MPI4JAX_B200_P2P_SLOT_BYTES": "1048576"})
-    _expect_passed(code, outs, 5, ["test_move_element_sizes_and_tails", "test_move_multichunk_one_cta"])
+    code, outs = job(__file__, 5, "test_move_element_sizes_and_tails or test_move_multichunk_one_cta",
+                     {"MPI4JAX_B200_P2P_SLOT_BYTES": "1048576"})
+    expect_passed(code, outs, 5, ["test_move_element_sizes_and_tails", "test_move_multichunk_one_cta"])

@@ -80,7 +80,7 @@ void emu_k34(const B2SweParams* p, const float* u, float* u_new, const float* v,
     for (int i0 = 0; i0 < p->pitch; i0 += 4) {
       bool m[4];
       masks(*p, i0, m);
-      if (!(m[0] || m[1] || m[2] || m[3])) continue;
+      if (!(m[0] || m[1] || m[2] || m[3]) && i0 != p->nx - 1) continue;     // (swe_k34_friction_u's groups)
       swe_k34_body(*p, u, u_new, v, fe2, fn2, j, i0, m, has_south != 0);
     }
 }

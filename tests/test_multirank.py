@@ -17,7 +17,7 @@ SUITE = ["tests/collective_ops", "tests/test_transforms.py", "tests/test_models.
          "tests/test_examples.py", "tests/test_jit.py", "tests/test_common.py", "tests/test_gemm.py",
          "tests/test_compile.py", "tests/test_transport.py", "tests/test_object_api.py",
          "tests/test_more_examples.py", "tests/test_extensions.py", "tests/test_coresidency.py",
-         "tests/test_shared_adjoints.py"]
+         "tests/test_shared_adjoints.py", "tests/test_swe_peers.py"]
 
 inside_job = MPI.COMM_WORLD.Get_size() > 1 or "MPI4JAX_B200_NESTED" in os.environ
 

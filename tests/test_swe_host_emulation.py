@@ -6,121 +6,20 @@ bulk kernel with its lanes in lockstep, frame kernels with owner views and ping-
 deep-halo exchange geometry, bulk / frame partition) against the stand-alone kernels, bit for bit."""
 
 import ctypes
-import os
-import shutil
-import subprocess
 
 import numpy as np
 import pytest
 
 from mpi4jax_b200._src import native
-from mpi4jax_b200.models.shallow_water import fold_constants
 
-REPO = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-CUDA_INC = next((d for d in (os.path.join(os.environ.get("CUDA_HOME", "/usr/local/cuda"), "include"),
-                             "/usr/local/cuda/include") if os.path.exists(os.path.join(d, "cuda_runtime.h"))), None)
+from ._swe_emu import HAVE_TOOLCHAIN, blocks, build, emulate, params, ptr
 
-pytestmark = pytest.mark.skipif(shutil.which("g++") is None or CUDA_INC is None,
-                                reason="needs g++ and the CUDA headers")
-
-
-def _build(tmp_path_factory, name):
-    out = tmp_path_factory.mktemp(name) / f"lib{name}.so"
-    cmd = ["g++", "-O1", "-ffp-contract=off", "-std=c++17", "-shared", "-fPIC", "-I",
-           os.path.join(REPO, "csrc"), "-I", CUDA_INC, os.path.join(REPO, "tests", "native", "swe_host_emu.cpp"),
-           "-o", str(out)]
-    res = subprocess.run(cmd, capture_output=True, text=True)
-    assert res.returncode == 0, res.stderr
-    return ctypes.CDLL(str(out))
+pytestmark = pytest.mark.skipif(not HAVE_TOOLCHAIN, reason="needs g++ and the CUDA headers")
 
 
 @pytest.fixture(scope="module")
 def emu(tmp_path_factory):
-    lib = _build(tmp_path_factory, "swe_emu")
-    # the package's ctypes mirrors of the ABI structs, against the C structs the harness is built with
-    assert lib.emu_sizeof_swe_params() == ctypes.sizeof(native.B2SweParams)
-    assert lib.emu_sizeof_swe_ca() == ctypes.sizeof(native.B2SweCA)
-    return lib
-
-
-def _ptr(a):
-    return a.ctypes.data_as(ctypes.c_void_p)
-
-
-# ---- whole steps: the launch sequence of b2_swe_multistep, emulated on a process grid ------------
-def _blocks(model, PY, PX):
-    """Cut the model's global initial condition into (PY x PX) blocks with one halo cell, as
-    ShallowWaterModel does per rank; returns per-rank dicts of pitch-padded float32 arrays."""
-    h0, u0, v0 = model.initial_conditions_global()
-    NY, NX = h0.shape
-    nyi, nxi = (NY - 2) // PY, (NX - 2) // PX
-    pitch = (nxi + 2 + 3) // 4 * 4
-    ranks = []
-    for py in range(PY):
-        for px in range(PX):
-            blk = {}
-            for name, g in (("h", h0), ("u", u0), ("v", v0)):
-                a = np.zeros((nyi + 2, pitch), np.float32)
-                a[:, :nxi + 2] = g[py * nyi: py * nyi + nyi + 2, px * nxi: px * nxi + nxi + 2]
-                blk[name] = a
-            for name in ("h1", "u1", "v1", "dh", "du", "dv", "fe", "fn", "q", "ke", "fe2", "fn2"):
-                blk[name] = np.zeros((nyi + 2, pitch), np.float32)
-            y_global = np.arange(-1, NY - 1) * model.cfg.dy
-            cor = (model.cfg.coriolis_f + y_global[py * nyi: py * nyi + nyi + 2] * model.cfg.coriolis_beta)
-            blk["cor"] = cor.astype(np.float32)
-            ranks.append(blk)
-    return ranks, nyi + 2, nxi + 2, pitch
-
-
-def _params(model, blk, ny, nx, pitch, py, PY, first):
-    cfg = model.cfg
-    return fold_constants(native.B2SweParams(
-        ny=ny, nx=nx, pitch=pitch, dx=cfg.dx, dy=cfg.dy, dt=cfg.dt, gravity=cfg.gravity,
-        viscosity=cfg.lateral_viscosity, rdx=np.float32(1) / np.float32(cfg.dx),
-        rdy=np.float32(1) / np.float32(cfg.dy), ab_a=cfg.ab_a, ab_b=cfg.ab_b, first_step=int(first),
-        south_wall=int(py == 0), north_wall=int(py == PY - 1), coriolis=blk["cor"].ctypes.data))
-
-
-def _exchange(ranks, names, kinds, nx, PY, PX):
-    from ._halo_sim import new_exchange
-
-    for name, kind in zip(names, kinds):
-        new_exchange([r[name][:, :nx] for r in ranks], PY, PX, kind)
-
-
-def _emulate(emu, model, PY, PX, nsteps):
-    """The launch sequence of b2_swe_multistep: K1 -> exchange -> K2 -> exchange -> K34 -> exchange -> K5."""
-    from ._halo_sim import new_exchange
-
-    ranks, ny, nx, pitch = _blocks(model, PY, PX)
-    # reset(): halos of the initial state, ping-pong partners start as copies
-    for name, kind in (("h", "h"), ("u", "u"), ("v", "v")):
-        new_exchange([r[name][:, :nx] for r in ranks], PY, PX, kind)
-    for r in ranks:
-        r["h1"][:], r["u1"][:], r["v1"][:] = r["h"], r["u"], r["v"]
-    hk, hnk = "h", "h1"
-    for it in range(nsteps):
-        ps = [_params(model, r, ny, nx, pitch, i // PX, PY, it == 0) for i, r in enumerate(ranks)]
-        B = ctypes.byref
-        for r, p in zip(ranks, ps):
-            emu.emu_k1_all(B(p), _ptr(r[hk]), _ptr(r["u"]), _ptr(r["v"]), _ptr(r["fe"]), _ptr(r["fn"]),
-                           _ptr(r["q"]), _ptr(r["ke"]))
-        _exchange(ranks, ("fe", "fn", "q", "ke"), ("u", "v", "h", "h"), nx, PY, PX)
-        for r, p in zip(ranks, ps):
-            emu.emu_k2_all(B(p), _ptr(r[hk]), _ptr(r[hnk]), _ptr(r["u"]), _ptr(r["v"]), _ptr(r["dh"]),
-                           _ptr(r["du"]), _ptr(r["dv"]), _ptr(r["fe"]), _ptr(r["fn"]), _ptr(r["q"]),
-                           _ptr(r["ke"]))
-        _exchange(ranks, (hnk, "u", "v"), ("h", "u", "v"), nx, PY, PX)
-        for i, (r, p) in enumerate(zip(ranks, ps)):
-            emu.emu_k34(B(p), _ptr(r["u"]), _ptr(r["u1"]), _ptr(r["v"]), _ptr(r["fe2"]), _ptr(r["fn2"]),
-                        int(i // PX > 0))
-            r["u"], r["u1"] = r["u1"], r["u"]
-        _exchange(ranks, ("fe2", "fn2"), ("u", "v"), nx, PY, PX)
-        for r, p in zip(ranks, ps):
-            emu.emu_k5(B(p), _ptr(r["v"]), _ptr(r["fe2"]), _ptr(r["fn2"]))
-        hk, hnk = hnk, hk
-    return [dict(h=r[hk][:, :nx], u=r["u"][:, :nx], v=r["v"][:, :nx], dh=r["dh"][:, :nx], du=r["du"][:, :nx],
-                 dv=r["dv"][:, :nx]) for r in ranks]
+    return build(tmp_path_factory, "swe_emu")
 
 
 def _close(a, b, tol):
@@ -138,7 +37,7 @@ def test_emulated_native_step_matches_the_ops_backend(emu):
     cfg = ShallowWaterConfig(nx=48, ny=24)
     model = ShallowWaterModel(cfg, device="cpu", backend="ops")
     nsteps = 6
-    emu_state = _emulate(emu, model, 1, 1, nsteps)[0]
+    emu_state = emulate(emu, model, 1, 1, nsteps)[0]
     model.multistep(nsteps)
     for name, t in model.state._asdict().items():
         got, want = emu_state[name], t.numpy()
@@ -201,7 +100,7 @@ def _emulate_ca(emu, model, PY, PX, nsteps, rows, reverse=0):
     any rank scatters: all sends of a step come from h', u', v' frame cells, which no message writes.)"""
     from ._halo_sim import new_exchange
 
-    ranks, ny, nx, pitch = _blocks(model, PY, PX)
+    ranks, ny, nx, pitch = blocks(model, PY, PX)
     epitch = nx + 4
     for name, kind in (("h", "h"), ("u", "u"), ("v", "v")):
         new_exchange([r[name][:, :nx] for r in ranks], PY, PX, kind)
@@ -215,12 +114,12 @@ def _emulate_ca(emu, model, PY, PX, nsteps, rows, reverse=0):
     B = ctypes.byref
     _ca_exchange(emu, ranks, ("h", "u", "v"), ny, nx, pitch, epitch, PY, PX)       # b2_swe_ca_init
     for i, r in enumerate(ranks):
-        p = _params(model, r, ny, nx, pitch, i // PX, PY, True)
-        emu.emu_ca_init_ext(B(p), B(_ca_ext(r, epitch)), _ptr(r["u"]), _ptr(r["v"]))
+        p = params(model, r, ny, nx, pitch, i // PX, PY, True)
+        emu.emu_ca_init_ext(B(p), B(_ca_ext(r, epitch)), ptr(r["u"]), ptr(r["v"]))
     cur = ""
     for it in range(nsteps):
         nxt = "1" if cur == "" else ""
-        ps = [_params(model, r, ny, nx, pitch, i // PX, PY, it == 0) for i, r in enumerate(ranks)]
+        ps = [params(model, r, ny, nx, pitch, i // PX, PY, it == 0) for i, r in enumerate(ranks)]
         xs = [_ca_ext(r, epitch) for r in ranks]
         es = [EmuStep(**{n: r[n + cur].ctypes.data for n in _PAIRS},
                       **{n + "_o": r[n + nxt].ctypes.data for n in _PAIRS},
@@ -273,6 +172,7 @@ def test_ca_bulk_and_frame_partition_the_interior(emu, shape, rows):
     ((1, 1), (24, 48), 64),                 # one segment covers the bulk
     ((2, 1), (40, 280), 7),                 # several warp strips per row, a partial last strip
     ((1, 2), (33, 140), 16),                # odd bulk height: a short last segment
+    ((2, 2), (18, 39), 5),                  # nx % 4 == 1: the east halo column is a float4 group of its own
 ])
 def test_emulated_one_pass_ca_pipeline_is_bit_identical_to_the_standalone_pipeline(emu, grid, block, rows, nsteps):
     """One deep exchange per step + local recomputation (frame kernels with owner views, one-pass bulk
@@ -282,7 +182,7 @@ def test_emulated_one_pass_ca_pipeline_is_bit_identical_to_the_standalone_pipeli
 
     PY, PX = grid
     model = ShallowWaterModel(ShallowWaterConfig(nx=block[1] * PX, ny=block[0] * PY), device="cpu", backend="ops")
-    a = _emulate(emu, model, PY, PX, nsteps)
+    a = emulate(emu, model, PY, PX, nsteps)
     b = _emulate_ca(emu, model, PY, PX, nsteps, rows)
     c = _emulate_ca(emu, model, PY, PX, nsteps, rows, reverse=1)
     for ra, rb, rc in zip(a, b, c):
