@@ -210,29 +210,27 @@ __device__ __noinline__ void move_pull_and_stage(const B2DevComm& c, const B2Mov
 
 __global__ void __launch_bounds__(B2_THREADS, 1)
 b2_k_move(const __grid_constant__ B2DevComm c, const __grid_constant__ B2MoveArgs a) {
-  const unsigned ticket = b2_ticket_read(c.ticket);
-  const size_t par = (size_t)(ticket & 1u) * c.stage_half;
-  unsigned e = b2_ld_volatile(c.epoch + blockIdx.x);
+  auto [par, e] = b2_staged_begin(c);
   const char* in = (const char*)a.in;
   char* out = (char*)a.out;
   char* mine = c.stage[c.rank] + par;
   const size_t nchunks = (a.blk_bytes + a.chunk - 1) / a.chunk;
   // the fused loop moves whole 16-byte vectors on both sides
   const bool fuse = a.vec_ok && a.lay.nd == 0 && ((((uintptr_t)in) & 15) == 0) && (a.nin <= 1 || (a.blk_bytes & 15) == 0);
-#define CH_OFF(ch) ((ch) * a.chunk)
-#define CH_LEN(ch) ((a.blk_bytes - CH_OFF(ch) < a.chunk) ? (a.blk_bytes - CH_OFF(ch)) : a.chunk)
+  // b2_chunk_len(a.blk_bytes, a.chunk, ch) in a macro: the function changes this kernel's SASS
+#define CH_LEN(ch) ((a.blk_bytes - (ch) * a.chunk < a.chunk) ? (a.blk_bytes - (ch) * a.chunk) : a.chunk)
   size_t ch = blockIdx.x;
   unsigned e_cur = e;
   if (ch < nchunks) {
-    move_stage(a, mine, in, CH_OFF(ch), CH_LEN(ch));
+    move_stage(a, mine, in, ch * a.chunk, CH_LEN(ch));
     b2_barrier_arrive(c, ++e);
     e_cur = e;
   }
   for (; ch < nchunks; ch += gridDim.x) {
     const size_t nxt = ch + gridDim.x;
     const bool more = nxt < nchunks;
-    const size_t off = CH_OFF(ch), len = CH_LEN(ch);
-    const size_t noff = more ? CH_OFF(nxt) : 0, nlen = more ? CH_LEN(nxt) : 0;
+    const size_t off = ch * a.chunk, len = CH_LEN(ch);
+    const size_t noff = more ? nxt * a.chunk : 0, nlen = more ? CH_LEN(nxt) : 0;
     b2_barrier_wait(c, e_cur, a.opcode);            // every rank staged this chunk
     if (fuse && a.nin <= 1 && a.nsrc <= 8) {
       if (a.nsrc <= 1) move_pull_and_stage<1, 1, 4, false>(c, a, par, mine, in, out, off, len, noff, nlen);
@@ -255,11 +253,8 @@ b2_k_move(const __grid_constant__ B2DevComm c, const __grid_constant__ B2MoveArg
       e_cur = e;
     }
   }
-#undef CH_OFF
 #undef CH_LEN
-  __syncthreads();
-  if (threadIdx.x == 0) b2_st_volatile(c.epoch + blockIdx.x, e);
-  b2_finish_bump(c.ticket, c.ticket + 1, 1u, gridDim.x);
+  b2_staged_end(c, e);
 }
 
 // ---------------------------------------------------------------------------
@@ -300,9 +295,7 @@ b2_k_rowsv(const __grid_constant__ B2DevComm c, const __grid_constant__ B2Alltoa
   __shared__ size_t s_gap[B2_MAX_RANKS + 1][2];                    // output bytes nobody writes (non-empty)
   __shared__ size_t s_mine, s_nch;
   __shared__ int s_ngap;
-  const unsigned ticket = b2_ticket_read(c.ticket);
-  const size_t par = (size_t)(ticket & 1u) * c.stage_half;
-  unsigned e = b2_ld_volatile(c.epoch + blockIdx.x);
+  auto [par, e] = b2_staged_begin(c);
   const int t = threadIdx.x, P = c.size, r = c.rank;
   const bool gather = a.count != nullptr;
   const char* in = (const char*)a.in;
@@ -325,11 +318,13 @@ b2_k_rowsv(const __grid_constant__ B2DevComm c, const __grid_constant__ B2Alltoa
   __syncthreads();
   const size_t mine_bytes = s_mine;
   char* mine_rows = mine + B2_A2AV_HDR;
-#define CH_LEN(ch) ((ch) * a.chunk < mine_bytes                                                         \
-                        ? (mine_bytes - (ch) * a.chunk < a.chunk ? mine_bytes - (ch) * a.chunk : a.chunk) \
-                        : (size_t)0)
+  // chunk ch of this rank's rows (none past their end)
+  auto stage = [&](size_t ch) {
+    const size_t off = ch * a.chunk;
+    b2_copy_bytes<false>(mine_rows + off, in + off, off < mine_bytes ? b2_chunk_len(mine_bytes, a.chunk, ch) : 0);
+  };
   size_t ch = blockIdx.x;
-  b2_copy_bytes<false>(mine_rows + ch * a.chunk, in + ch * a.chunk, CH_LEN(ch));
+  stage(ch);
   b2_barrier_arrive(c, ++e);
   unsigned e_cur = e;
   b2_barrier_wait(c, e_cur, a.opcode);              // every rank's header and chunk blockIdx.x are staged
@@ -401,17 +396,14 @@ b2_k_rowsv(const __grid_constant__ B2DevComm c, const __grid_constant__ B2Alltoa
     }
     const size_t nxt = ch + gridDim.x;
     if (nxt < nch) {
-      b2_copy_bytes<false>(mine_rows + nxt * a.chunk, in + nxt * a.chunk, CH_LEN(nxt));
+      stage(nxt);
       b2_barrier_arrive(c, ++e);
       e_cur = e;
     }
   }
-#undef CH_LEN
   // 4. rows nobody sends are zero: the output is fully written on every call
   for (int g = 0; g < s_ngap; ++g) a2av_zero(out, s_gap[g][0], s_gap[g][1]);
-  __syncthreads();
-  if (t == 0) b2_st_volatile(c.epoch + blockIdx.x, e);
-  b2_finish_bump(c.ticket, c.ticket + 1, 1u, gridDim.x);
+  b2_staged_end(c, e);
 }
 
 // ---------------------------------------------------------------------------
@@ -472,17 +464,13 @@ __device__ __forceinline__ void b2_nvls_slice(const B2DevComm& c, char* mc, size
 template <int DT>
 __global__ void __launch_bounds__(B2_THREADS)
 b2_k_allreduce_nvls(const B2DevComm c, const B2ReduceArgs a) {
-  const unsigned ticket = b2_ticket_read(c.ticket);
-  const size_t par = (size_t)(ticket & 1u) * c.stage_half;
-  unsigned e = b2_ld_volatile(c.epoch + blockIdx.x);
+  auto [par, e] = b2_staged_begin(c);
   const char* in = (const char*)a.in;
   char* out = (char*)a.out;
   char* mine = c.stage[c.rank] + par;
   char* mc = c.stage_mc + par;
   const size_t nchunks = (a.nbytes + a.chunk - 1) / a.chunk;
   const int t = threadIdx.x;
-#define CH_OFF(ch) ((ch) * a.chunk)
-#define CH_LEN(ch) ((a.nbytes - CH_OFF(ch) < a.chunk) ? (a.nbytes - CH_OFF(ch)) : a.chunk)
   const bool pipe = a.pipeline != 0;
   unsigned e_a1 = e;
   bool staged = false;
@@ -495,16 +483,16 @@ b2_k_allreduce_nvls(const B2DevComm c, const B2ReduceArgs a) {
     const size_t nxt = ch + gridDim.x;
     const bool more = pipe && nxt < nchunks;
     if (!staged) {
-      b2_copy_bytes<false>(mine + CH_OFF(ch), in + CH_OFF(ch), CH_LEN(ch));
+      b2_copy_bytes<false>(mine + ch * a.chunk, in + ch * a.chunk, b2_chunk_len(a.nbytes, a.chunk, ch));
       b2_barrier_arrive(c, ++e);                                 // A1
       e_a1 = e;
     }
     TRACE();                                                     // 1: staged (or nothing)
-    if (more) b2_copy_bytes<false>(mine + CH_OFF(nxt), in + CH_OFF(nxt), CH_LEN(nxt));
+    if (more) b2_copy_bytes<false>(mine + nxt * a.chunk, in + nxt * a.chunk, b2_chunk_len(a.nbytes, a.chunk, nxt));
     TRACE();                                                     // 2: next chunk staged
     b2_barrier_wait(c, e_a1, a.opcode);                          // W1: every rank staged this chunk
     TRACE();                                                     // 3: W1
-    b2_nvls_slice<DT>(c, mc, CH_OFF(ch), CH_LEN(ch));
+    b2_nvls_slice<DT>(c, mc, ch * a.chunk, b2_chunk_len(a.nbytes, a.chunk, ch));
     TRACE();                                                     // 4: in-switch reduction + broadcast issued
     b2_barrier_arrive(c, ++e);                                   // A2
     const unsigned e_a2 = e;
@@ -515,15 +503,11 @@ b2_k_allreduce_nvls(const B2DevComm c, const B2ReduceArgs a) {
     }
     b2_barrier_wait(c, e_a2, a.opcode);                          // W2: every sub-slice has landed here
     TRACE();                                                     // 5: W2
-    b2_copy_bytes<true>(out + CH_OFF(ch), mine + CH_OFF(ch), CH_LEN(ch));
+    b2_copy_bytes<true>(out + ch * a.chunk, mine + ch * a.chunk, b2_chunk_len(a.nbytes, a.chunk, ch));
     TRACE();                                                     // 6: copied out
   }
 #undef TRACE
-#undef CH_OFF
-#undef CH_LEN
-  __syncthreads();
-  if (t == 0) b2_st_volatile(c.epoch + blockIdx.x, e);
-  b2_finish_bump(c.ticket, c.ticket + 1, 1u, gridDim.x);
+  b2_staged_end(c, e);
 }
 
 // ---------------------------------------------------------------------------
@@ -574,9 +558,7 @@ b2_k_allreduce_sym(const B2DevComm c, const B2SymArgs a) {
 // ---------------------------------------------------------------------------
 __global__ void __launch_bounds__(B2_THREADS)
 b2_k_bcast_mc(const B2DevComm c, const B2MoveArgs a, const int root) {
-  const unsigned ticket = b2_ticket_read(c.ticket);
-  const size_t par = (size_t)(ticket & 1u) * c.stage_half;
-  unsigned e = b2_ld_volatile(c.epoch + blockIdx.x);
+  auto [par, e] = b2_staged_begin(c);
   const char* in = (const char*)a.in;
   char* out = (char*)a.out;
   char* mine = c.stage[c.rank] + par;
@@ -585,7 +567,7 @@ b2_k_bcast_mc(const B2DevComm c, const B2MoveArgs a, const int root) {
   const int t = threadIdx.x, nt = blockDim.x;
   for (size_t ch = blockIdx.x; ch < nchunks; ch += gridDim.x) {
     const size_t off = ch * a.chunk;
-    const size_t len = (a.blk_bytes - off < a.chunk) ? (a.blk_bytes - off) : a.chunk;
+    const size_t len = b2_chunk_len(a.blk_bytes, a.chunk, ch);
     if (c.rank == root) {
       const size_t nv = len >> 4, tail = len & 15;
       size_t i = t;
@@ -609,9 +591,7 @@ b2_k_bcast_mc(const B2DevComm c, const B2MoveArgs a, const int root) {
     b2_barrier_all(c, ++e, a.opcode);
     if (c.rank != root) b2_copy_bytes<true>(out + off, mine + off, len);
   }
-  __syncthreads();
-  if (t == 0) b2_st_volatile(c.epoch + blockIdx.x, e);
-  b2_finish_bump(c.ticket, c.ticket + 1, 1u, gridDim.x);
+  b2_staged_end(c, e);
 }
 
 // reduce (SUM, f32 / bf16 / f16): the root reads the in-switch sum of all ranks' staging with
@@ -619,23 +599,19 @@ b2_k_bcast_mc(const B2DevComm c, const B2MoveArgs a, const int root) {
 template <int DT>
 __global__ void __launch_bounds__(B2_THREADS)
 b2_k_reduce_root_nvls(const B2DevComm c, const B2ReduceArgs a) {
-  const unsigned ticket = b2_ticket_read(c.ticket);
-  const size_t par = (size_t)(ticket & 1u) * c.stage_half;
-  unsigned e = b2_ld_volatile(c.epoch + blockIdx.x);
+  auto [par, e] = b2_staged_begin(c);
   const char* in = (const char*)a.in;
   char* out = (char*)a.out;
   char* mine = c.stage[c.rank] + par;
   const char* mc = c.stage_mc + par;
   const size_t nchunks = (a.nbytes + a.chunk - 1) / a.chunk;
   const int t = threadIdx.x, nt = blockDim.x;
-#define CH_OFF(ch) ((ch) * a.chunk)
-#define CH_LEN(ch) ((a.nbytes - CH_OFF(ch) < a.chunk) ? (a.nbytes - CH_OFF(ch)) : a.chunk)
   // software pipeline: the next chunk is staged while this one is reduced -- on the root in the SAME
   // loop as the multimem.ld_reduce, so the switch round trips and the HBM loads overlap
   size_t ch = blockIdx.x;
   unsigned e_cur = e;
   if (ch < nchunks) {
-    b2_copy_bytes<false>(mine + CH_OFF(ch), in + CH_OFF(ch), CH_LEN(ch));
+    b2_copy_bytes<false>(mine + ch * a.chunk, in + ch * a.chunk, b2_chunk_len(a.nbytes, a.chunk, ch));
     b2_barrier_arrive(c, ++e);
     e_cur = e;
   }
@@ -643,8 +619,8 @@ b2_k_reduce_root_nvls(const B2DevComm c, const B2ReduceArgs a) {
   for (; ch < nchunks; ch += gridDim.x) {
     const size_t nxt = ch + gridDim.x;
     const bool more = nxt < nchunks;
-    const size_t off = CH_OFF(ch), len = CH_LEN(ch);
-    const size_t noff = more ? CH_OFF(nxt) : 0, nlen = more ? CH_LEN(nxt) : 0;
+    const size_t off = ch * a.chunk, len = b2_chunk_len(a.nbytes, a.chunk, ch);
+    const size_t noff = more ? nxt * a.chunk : 0, nlen = more ? b2_chunk_len(a.nbytes, a.chunk, nxt) : 0;
     b2_barrier_wait(c, e_cur, a.opcode);              // every rank staged this chunk
     size_t staged = 0;                                // vectors of the next chunk staged by the fused loop
     if (a.has_out) {
@@ -689,11 +665,7 @@ b2_k_reduce_root_nvls(const B2DevComm c, const B2ReduceArgs a) {
       e_cur = e;
     }
   }
-#undef CH_OFF
-#undef CH_LEN
-  __syncthreads();
-  if (t == 0) b2_st_volatile(c.epoch + blockIdx.x, e);
-  b2_finish_bump(c.ticket, c.ticket + 1, 1u, gridDim.x);
+  b2_staged_end(c, e);
 }
 
 // ---------------------------------------------------------------------------
@@ -765,14 +737,33 @@ extern "C" size_t b2_stage_need(int opcode, int nranks, size_t blk_bytes) {
   }
 }
 
-static int check_stage(B2Comm* c, int opcode, size_t blk_bytes, const char* name) {
+// The launch geometry of a staged kernel: checks that the staging holds what `opcode` stages for
+// `blk_bytes`, then picks the chunk size and the grid of `kernel` (nullptr: one CTA per SM).
+static int plan_staged(B2Comm* c, int opcode, size_t blk_bytes, const void* kernel, const char* name,
+                       size_t* chunk, int* grid) {
   const size_t need = b2_stage_need(opcode, c->dev.size, blk_bytes);
   if (c->stage == nullptr || need > c->dev.stage_half) {
     b2_set_error("%s: staging too small (need %zu bytes, have %zu); the Python layer must grow it",
                  name, need, c->stage ? c->dev.stage_half : (size_t)0);
     return B2_ERR_BAD_ARG;
   }
+  pick_chunks(c, blk_bytes, coresident_blocks(c, kernel), chunk, grid);
   return 0;
+}
+
+static int check_root(const B2Comm* c, int root, const char* name) {
+  if (root >= 0 && root < c->dev.size) return 0;
+  b2_set_error("%s: invalid root %d", name, root);
+  return B2_ERR_BAD_ARG;
+}
+
+// `table`: a typed launcher table of b2_reduce.cuh, nullptr where the dtype/op combination is invalid
+template <typename Fn>
+static int check_dtype_op(Fn (&table)[B2_DTYPE_COUNT][B2_OP_COUNT], int dtype, int op, const char* name) {
+  b2_ensure_tables();
+  if (dtype >= 0 && dtype < B2_DTYPE_COUNT && op >= 0 && op < B2_OP_COUNT && table[dtype][op] != nullptr) return 0;
+  b2_set_error("%s: unsupported dtype/op combination (dtype=%d, op=%d)", name, dtype, op);
+  return B2_ERR_BAD_ARG;
 }
 
 // The in-switch reductions: multicast-bound staging, SUM, f32 / bf16 / f16.
@@ -835,12 +826,8 @@ static const char* algo_name(int algo) {
 static int reduce_common(B2Comm* c, const void* in, void* out, size_t count, int dtype, int op,
                          int algo, int src_lo, int src_hi, int has_out, int opcode,
                          const char* name, cudaStream_t stream) {
-  b2_ensure_tables();
-  if (dtype < 0 || dtype >= B2_DTYPE_COUNT || op < 0 || op >= B2_OP_COUNT ||
-      b2_reduce_table[dtype][op] == nullptr) {
-    b2_set_error("%s: unsupported dtype/op combination (dtype=%d, op=%d)", name, dtype, op);
-    return B2_ERR_BAD_ARG;
-  }
+  int rc = check_dtype_op(b2_reduce_table, dtype, op, name);
+  if (rc) return rc;
   const size_t nbytes = count * b2_dtype_size(dtype);
   if (nbytes == 0) return 0;
   const bool rs = opcode == B2_OPC_REDUCE_SCATTER;
@@ -860,27 +847,26 @@ static int reduce_common(B2Comm* c, const void* in, void* out, size_t count, int
     b2_ll_table[dtype][op](c->dev, a, grid, stream);
     return b2_launched(c, name);
   }
-  int rc = check_stage(c, opcode, nbytes, name);
-  if (rc) return rc;
   B2ReduceArgs a;
   a.in = in; a.out = out; a.nbytes = nbytes;
   a.src_lo = src_lo; a.src_hi = src_hi; a.has_out = has_out; a.opcode = opcode;
   a.pipeline = c->nvls_pipeline;
   a.trace = c->trace; a.trace_cap = c->trace_cap;
+  // the grid of the in-switch kernel, or one CTA per SM for the typed kernels (nullptr)
+  const b2_nvls_kernel kern = algo == B2_ALGO_NVLS ? nvls_kernel(opcode, dtype) : nullptr;
   int grid;
+  rc = plan_staged(c, opcode, nbytes, (const void*)kern, name, &a.chunk, &grid);
+  if (rc) return rc;
   if (algo == B2_ALGO_NVLS) {
     if (!nvls_capable(c, dtype, op)) {
       b2_set_error("%s: NVLS path needs a multicast-bound staging segment and SUM on f32/bf16/f16",
                    name);
       return B2_ERR_BAD_ARG;
     }
-    const b2_nvls_kernel kern = nvls_kernel(opcode, dtype);
-    pick_chunks(c, nbytes, coresident_blocks(c, (const void*)kern), &a.chunk, &grid);
     a.algo = B2_ALGO_NVLS;
     kern<<<grid, B2_THREADS, 0, stream>>>(c->dev, a);
     return b2_launched(c, name);
   }
-  pick_chunks(c, nbytes, coresident_blocks(c, nullptr), &a.chunk, &grid);     // (typed kernels: one CTA per SM)
   a.algo = (algo == B2_ALGO_TWOSHOT) ? B2_ALGO_TWOSHOT : B2_ALGO_ONESHOT;
   b2_reduce_table[dtype][op](c->dev, a, grid, stream);
   return b2_launched(c, name);
@@ -931,14 +917,10 @@ extern "C" int b2_reduce(B2Comm* c, const void* in, void* out, size_t count, int
   const int algo = nvls ? B2_ALGO_NVLS : B2_ALGO_ONESHOT;
   B2DebugScope* dbg = b2_debug_begin(c, "Reduce", stream, "with %zu items to root %d via %s", count, root,
                                      algo_name(algo));
-  int rc;
-  if (root < 0 || root >= c->dev.size) {
-    b2_set_error("reduce: invalid root %d", root);
-    rc = B2_ERR_BAD_ARG;
-  } else {
+  int rc = check_root(c, root, "reduce");
+  if (rc == 0)
     rc = reduce_common(c, in, out, count, dtype, op, algo, 0, c->dev.size, c->dev.rank == root, B2_OPC_REDUCE,
                        "reduce", stream);
-  }
   b2_debug_end(dbg, rc);
   return rc;
 }
@@ -969,6 +951,14 @@ extern "C" int b2_reduce_scatter(B2Comm* c, const void* in, void* out, size_t co
   return rc;
 }
 
+// the fields every data-movement collective sets; the rest start at zero
+static B2MoveArgs move_args(const void* in, void* out, size_t blk_bytes, int opcode) {
+  B2MoveArgs a;
+  memset(&a, 0, sizeof a);
+  a.in = in; a.out = out; a.blk_bytes = blk_bytes; a.opcode = opcode;
+  return a;
+}
+
 static int set_layout(B2MoveArgs& a, const B2Strided* lay, const char* name) {
   a.lay.nd = 0;
   a.in_blk_stride = 0;
@@ -991,12 +981,11 @@ static int set_layout(B2MoveArgs& a, const B2Strided* lay, const char* name) {
 
 static int move_common(B2Comm* c, B2MoveArgs& a, const char* name, cudaStream_t stream) {
   if (a.blk_bytes == 0) return 0;
-  int rc = check_stage(c, a.opcode, a.blk_bytes, name);
+  int grid;
+  int rc = plan_staged(c, a.opcode, a.blk_bytes, (const void*)b2_k_move, name, &a.chunk, &grid);
   if (rc) return rc;
   a.blk_stride = round_up(a.blk_bytes, 16);
   a.vec_ok = ((((uintptr_t)a.out) & 15) == 0 && (a.blk_bytes % 16 == 0 || a.nsrc <= 1)) ? 1 : 0;
-  int grid;
-  pick_chunks(c, a.blk_bytes, coresident_blocks(c, (const void*)b2_k_move), &a.chunk, &grid);
   b2_k_move<<<grid, B2_THREADS, 0, stream>>>(c->dev, a);
   return b2_launched(c, name);
 }
@@ -1004,9 +993,7 @@ static int move_common(B2Comm* c, B2MoveArgs& a, const char* name, cudaStream_t 
 extern "C" int b2_allgather(B2Comm* c, const void* in, void* out, size_t blk_bytes, const B2Strided* lay,
                             cudaStream_t stream) {
   B2DebugScope* dbg = b2_debug_begin(c, "Allgather", stream, "sending %zu bytes", blk_bytes);
-  B2MoveArgs a;
-  memset(&a, 0, sizeof a);
-  a.in = in; a.out = out; a.blk_bytes = blk_bytes; a.opcode = B2_OPC_ALLGATHER;
+  B2MoveArgs a = move_args(in, out, blk_bytes, B2_OPC_ALLGATHER);
   a.nin = 1;
   a.nsrc = c->dev.size;
   for (int q = 0; q < c->dev.size; ++q) { a.src_rank[q] = q; a.src_blk[q] = 0; a.dst_blk[q] = q; }
@@ -1019,9 +1006,7 @@ extern "C" int b2_allgather(B2Comm* c, const void* in, void* out, size_t blk_byt
 extern "C" int b2_alltoall(B2Comm* c, const void* in, void* out, size_t blk_bytes, const B2Strided* lay,
                            cudaStream_t stream) {
   B2DebugScope* dbg = b2_debug_begin(c, "Alltoall", stream, "sending %zu bytes per peer", blk_bytes);
-  B2MoveArgs a;
-  memset(&a, 0, sizeof a);
-  a.in = in; a.out = out; a.blk_bytes = blk_bytes; a.opcode = B2_OPC_ALLTOALL;
+  B2MoveArgs a = move_args(in, out, blk_bytes, B2_OPC_ALLTOALL);
   a.nin = c->dev.size;
   a.nsrc = c->dev.size;
   for (int q = 0; q < c->dev.size; ++q) {
@@ -1036,36 +1021,27 @@ extern "C" int b2_alltoall(B2Comm* c, const void* in, void* out, size_t blk_byte
 extern "C" int b2_bcast(B2Comm* c, const void* in, void* out, size_t nbytes, int root, const B2Strided* lay,
                         cudaStream_t stream) {
   B2DebugScope* dbg = b2_debug_begin(c, "Bcast", stream, "%zu bytes from root %d", nbytes, root);
-  int rc;
-  if (root < 0 || root >= c->dev.size) {
-    b2_set_error("bcast: invalid root %d", root);
-    rc = B2_ERR_BAD_ARG;
-  } else {
-    B2MoveArgs a;
-    memset(&a, 0, sizeof a);
-    a.in = in; a.out = out; a.blk_bytes = nbytes; a.opcode = B2_OPC_BCAST;
-    if (c->dev.rank == root) { a.nin = 1; a.nsrc = 0; }
-    else { a.nin = 0; a.nsrc = 1; a.src_rank[0] = root; a.src_blk[0] = 0; a.dst_blk[0] = 0; }
-    rc = set_layout(a, c->dev.rank == root ? lay : nullptr, "bcast");
-    // through the switch (one multimem.st stream from the root) once the root's links would be the
-    // bottleneck of P-1 pulls; contiguous 16-byte aligned root buffers only (every rank must take
-    // the same path: the decision uses sizes only, the root's layout is normalised by the caller)
-    const bool mc = c->dev.stage_mc != nullptr && c->dev.size > 2 && nbytes >= c->bcast_mc_min;
-    if (rc == 0 && mc && nbytes > 0) {
-      if ((rc = check_stage(c, a.opcode, a.blk_bytes, "bcast")) == 0) {
-        if (c->dev.rank == root && (a.lay.nd > 0 || (((uintptr_t)in) & 15) != 0)) {
-          b2_set_error("bcast: the multicast path needs a contiguous 16-byte aligned root buffer");
-          rc = B2_ERR_BAD_ARG;
-        } else {
-          int grid;
-          pick_chunks(c, a.blk_bytes, coresident_blocks(c, (const void*)b2_k_bcast_mc), &a.chunk, &grid);
-          b2_k_bcast_mc<<<grid, B2_THREADS, 0, stream>>>(c->dev, a, root);
-          rc = b2_launched(c, "bcast");
-        }
-      }
+  B2MoveArgs a = move_args(in, out, nbytes, B2_OPC_BCAST);
+  if (c->dev.rank == root) { a.nin = 1; a.nsrc = 0; }
+  else { a.nin = 0; a.nsrc = 1; a.src_rank[0] = root; a.src_blk[0] = 0; a.dst_blk[0] = 0; }
+  int rc = check_root(c, root, "bcast");
+  if (rc == 0) rc = set_layout(a, c->dev.rank == root ? lay : nullptr, "bcast");
+  // through the switch (one multimem.st stream from the root) once the root's links would be the
+  // bottleneck of P-1 pulls; contiguous 16-byte aligned root buffers only (every rank must take
+  // the same path: the decision uses sizes only, the root's layout is normalised by the caller)
+  const bool mc = c->dev.stage_mc != nullptr && c->dev.size > 2 && nbytes >= c->bcast_mc_min;
+  if (rc == 0 && mc && nbytes > 0) {
+    int grid;
+    rc = plan_staged(c, a.opcode, a.blk_bytes, (const void*)b2_k_bcast_mc, "bcast", &a.chunk, &grid);
+    if (rc == 0 && c->dev.rank == root && (a.lay.nd > 0 || (((uintptr_t)in) & 15) != 0)) {
+      b2_set_error("bcast: the multicast path needs a contiguous 16-byte aligned root buffer");
+      rc = B2_ERR_BAD_ARG;
     } else if (rc == 0) {
-      rc = move_common(c, a, "bcast", stream);
+      b2_k_bcast_mc<<<grid, B2_THREADS, 0, stream>>>(c->dev, a, root);
+      rc = b2_launched(c, "bcast");
     }
+  } else if (rc == 0) {
+    rc = move_common(c, a, "bcast", stream);
   }
   b2_debug_end(dbg, rc);
   return rc;
@@ -1074,22 +1050,15 @@ extern "C" int b2_bcast(B2Comm* c, const void* in, void* out, size_t nbytes, int
 extern "C" int b2_gather(B2Comm* c, const void* in, void* out, size_t blk_bytes, int root, const B2Strided* lay,
                          cudaStream_t stream) {
   B2DebugScope* dbg = b2_debug_begin(c, "Gather", stream, "sending %zu bytes to root %d", blk_bytes, root);
-  int rc;
-  if (root < 0 || root >= c->dev.size) {
-    b2_set_error("gather: invalid root %d", root);
-    rc = B2_ERR_BAD_ARG;
-  } else {
-    B2MoveArgs a;
-    memset(&a, 0, sizeof a);
-    a.in = in; a.out = out; a.blk_bytes = blk_bytes; a.opcode = B2_OPC_GATHER;
-    a.nin = 1;
-    if (c->dev.rank == root) {
-      a.nsrc = c->dev.size;
-      for (int q = 0; q < c->dev.size; ++q) { a.src_rank[q] = q; a.src_blk[q] = 0; a.dst_blk[q] = q; }
-    }
-    rc = set_layout(a, lay, "gather");
-    if (rc == 0) rc = move_common(c, a, "gather", stream);
+  B2MoveArgs a = move_args(in, out, blk_bytes, B2_OPC_GATHER);
+  a.nin = 1;
+  if (c->dev.rank == root) {
+    a.nsrc = c->dev.size;
+    for (int q = 0; q < c->dev.size; ++q) { a.src_rank[q] = q; a.src_blk[q] = 0; a.dst_blk[q] = q; }
   }
+  int rc = check_root(c, root, "gather");
+  if (rc == 0) rc = set_layout(a, lay, "gather");
+  if (rc == 0) rc = move_common(c, a, "gather", stream);
   b2_debug_end(dbg, rc);
   return rc;
 }
@@ -1097,20 +1066,13 @@ extern "C" int b2_gather(B2Comm* c, const void* in, void* out, size_t blk_bytes,
 extern "C" int b2_scatter(B2Comm* c, const void* in, void* out, size_t blk_bytes, int root, const B2Strided* lay,
                           cudaStream_t stream) {
   B2DebugScope* dbg = b2_debug_begin(c, "Scatter", stream, "%zu bytes per rank from root %d", blk_bytes, root);
-  int rc;
-  if (root < 0 || root >= c->dev.size) {
-    b2_set_error("scatter: invalid root %d", root);
-    rc = B2_ERR_BAD_ARG;
-  } else {
-    B2MoveArgs a;
-    memset(&a, 0, sizeof a);
-    a.in = in; a.out = out; a.blk_bytes = blk_bytes; a.opcode = B2_OPC_SCATTER;
-    a.nin = (c->dev.rank == root) ? c->dev.size : 0;
-    a.nsrc = 1;
-    a.src_rank[0] = root; a.src_blk[0] = c->dev.rank; a.dst_blk[0] = 0;
-    rc = set_layout(a, c->dev.rank == root ? lay : nullptr, "scatter");
-    if (rc == 0) rc = move_common(c, a, "scatter", stream);
-  }
+  B2MoveArgs a = move_args(in, out, blk_bytes, B2_OPC_SCATTER);
+  a.nin = (c->dev.rank == root) ? c->dev.size : 0;
+  a.nsrc = 1;
+  a.src_rank[0] = root; a.src_blk[0] = c->dev.rank; a.dst_blk[0] = 0;
+  int rc = check_root(c, root, "scatter");
+  if (rc == 0) rc = set_layout(a, c->dev.rank == root ? lay : nullptr, "scatter");
+  if (rc == 0) rc = move_common(c, a, "scatter", stream);
   b2_debug_end(dbg, rc);
   return rc;
 }
@@ -1119,11 +1081,9 @@ extern "C" int b2_scatter(B2Comm* c, const void* in, void* out, size_t blk_bytes
 // rows (the same everywhere) or, in alltoallv's reverse mode, nranks x its output rows (the forward's
 // input rows again).  The counts are read on the device, so the host never waits for them.
 static int rowsv_launch(B2Comm* c, B2AlltoallvArgs& a, const char* name, cudaStream_t stream) {
-  const size_t stage_bytes = a.max_rows * a.row_bytes;
-  int rc = check_stage(c, a.opcode, stage_bytes, name);
-  if (rc) return rc;
   int grid;
-  pick_chunks(c, stage_bytes, coresident_blocks(c, (const void*)b2_k_rowsv), &a.chunk, &grid);
+  int rc = plan_staged(c, a.opcode, a.max_rows * a.row_bytes, (const void*)b2_k_rowsv, name, &a.chunk, &grid);
+  if (rc) return rc;
   b2_k_rowsv<<<grid, B2_THREADS, 0, stream>>>(c->dev, a);
   return b2_launched(c, name);
 }
@@ -1176,26 +1136,20 @@ extern "C" int b2_reduce_scatterv(B2Comm* c, const void* in, void* out, size_t r
                                   int op, cudaStream_t stream) {
   B2DebugScope* dbg = b2_debug_begin(c, "Reduce_scatterv", stream, "with %zu rows of %zu bytes via pull", in_rows,
                                      row_bytes);
-  b2_ensure_tables();
-  int rc;
-  if (dtype < 0 || dtype >= B2_DTYPE_COUNT || op < 0 || op >= B2_OP_COUNT || b2_rsv_table[dtype][op] == nullptr) {
-    b2_set_error("reduce_scatterv: unsupported dtype/op combination (dtype=%d, op=%d)", dtype, op);
-    rc = B2_ERR_BAD_ARG;
-  } else if (send_counts == nullptr || recv_counts == nullptr) {
+  int rc = check_dtype_op(b2_rsv_table, dtype, op, "reduce_scatterv");
+  if (rc == 0 && (send_counts == nullptr || recv_counts == nullptr)) {
     b2_set_error("reduce_scatterv: send_counts and recv_counts must be device arrays of %d int64", c->dev.size);
     rc = B2_ERR_BAD_ARG;
-  } else if (row_bytes % b2_dtype_size(dtype) != 0) {
+  } else if (rc == 0 && row_bytes % b2_dtype_size(dtype) != 0) {
     b2_set_error("reduce_scatterv: %zu-byte rows are not whole elements of dtype %d", row_bytes, dtype);
     rc = B2_ERR_BAD_ARG;
-  } else {
+  } else if (rc == 0) {
     B2RsvArgs a;
     a.in = in; a.out = out; a.send_counts = send_counts; a.recv_counts = recv_counts;
     a.row_bytes = row_bytes; a.in_rows = in_rows; a.out_rows = out_rows; a.opcode = B2_OPC_REDUCE_SCATTERV;
-    const size_t blk_bytes = out_rows * row_bytes;
-    rc = check_stage(c, B2_OPC_REDUCE_SCATTERV, blk_bytes, "reduce_scatterv");
+    int grid;
+    rc = plan_staged(c, a.opcode, out_rows * row_bytes, b2_rsv_kernel[dtype][op], "reduce_scatterv", &a.chunk, &grid);
     if (rc == 0) {
-      int grid;
-      pick_chunks(c, blk_bytes, coresident_blocks(c, b2_rsv_kernel[dtype][op]), &a.chunk, &grid);
       b2_rsv_table[dtype][op](c->dev, a, grid, stream);
       rc = b2_launched(c, "reduce_scatterv");
     }

@@ -182,7 +182,8 @@ __device__ __forceinline__ void b2_barrier_wait(const B2DevComm& c, unsigned e, 
 // ticket: one value per kernel launch, identical on every CTA, advanced by the
 // LAST CTA TO FINISH (so every CTA has already read it).  Lives in local device
 // memory -> graph replays see fresh values without host involvement.
-// Usage:  unsigned t = b2_ticket_read(ptr);  ...  b2_ticket_finish(ptr, ctr, 1);
+// Usage:  unsigned t = b2_ticket_read(ptr);  ...  b2_finish_bump(ptr, ctr, 1, gridDim.x);
+// (staged kernels go through b2_staged_begin / b2_staged_end below)
 // ---------------------------------------------------------------------------
 __device__ __forceinline__ unsigned b2_ticket_read(const unsigned* ticket) {
   __shared__ unsigned s_ticket;
@@ -204,6 +205,38 @@ __device__ __forceinline__ void b2_finish_bump(unsigned* target, unsigned* ctr, 
       __threadfence();
     }
   }
+}
+
+// ---------------------------------------------------------------------------
+// staged launch: the protocol of every kernel that stages data and synchronises with the block-paired
+// barriers.  The ticket's parity picks the staging half, so a launch (or graph replay) never writes
+// staging that a peer may still be reading for the previous one; the CTA's epochs continue where its
+// previous launch stopped.  All threads call both:
+//   auto [par, e] = b2_staged_begin(c);  ... b2_barrier_all(c, ++e, ...) ...  b2_staged_end(c, e);
+// A kernel forms its own staging pointer, c.stage[c.rank] + par: formed in here, it changes the
+// register allocation of b2_k_rowsv and b2_k_reduce_root_nvls.
+// ---------------------------------------------------------------------------
+struct B2Staged {
+  size_t par;    // byte offset of this launch's staging half (into any rank's c.stage, and c.stage_mc)
+  unsigned e;    // the CTA's last barrier epoch
+};
+__device__ __forceinline__ B2Staged b2_staged_begin(const B2DevComm& c) {
+  B2Staged s;
+  s.par = (size_t)(b2_ticket_read(c.ticket) & 1u) * c.stage_half;
+  s.e = b2_ld_volatile(c.epoch + blockIdx.x);
+  return s;
+}
+// `e`: the CTA's last epoch.  The last CTA to finish advances the ticket.
+__device__ __forceinline__ void b2_staged_end(const B2DevComm& c, unsigned e) {
+  __syncthreads();
+  if (threadIdx.x == 0) b2_st_volatile(c.epoch + blockIdx.x, e);
+  b2_finish_bump(c.ticket, c.ticket + 1, 1u, gridDim.x);
+}
+
+// Bytes of chunk `ch` of a `total`-byte payload cut into `chunk`-byte chunks; chunk ch starts at byte
+// ch * chunk, which must be below `total`.
+__device__ __forceinline__ size_t b2_chunk_len(size_t total, size_t chunk, size_t ch) {
+  return total - ch * chunk < chunk ? total - ch * chunk : chunk;
 }
 
 // ---------------------------------------------------------------------------

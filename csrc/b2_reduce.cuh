@@ -39,9 +39,7 @@ struct B2ReduceArgs {
 template <typename T, int OP>
 __global__ void __launch_bounds__(B2_THREADS)
 b2_k_reduce_chunked(const B2DevComm c, const B2ReduceArgs a) {
-  const unsigned ticket = b2_ticket_read(c.ticket);
-  const size_t par = (size_t)(ticket & 1u) * c.stage_half;
-  unsigned e = b2_ld_volatile(c.epoch + blockIdx.x);
+  auto [par, e] = b2_staged_begin(c);
   const char* in = (const char*)a.in;
   char* out = (char*)a.out;
   char* mine = c.stage[c.rank] + par;
@@ -50,7 +48,7 @@ b2_k_reduce_chunked(const B2DevComm c, const B2ReduceArgs a) {
 
   for (size_t ch = blockIdx.x; ch < nchunks; ch += gridDim.x) {
     const size_t off = ch * a.chunk;
-    const size_t len = (a.nbytes - off < a.chunk) ? (a.nbytes - off) : a.chunk;
+    const size_t len = b2_chunk_len(a.nbytes, a.chunk, ch);
     const size_t nv = (len + 15) >> 4;        // vectors incl. a padded tail vector
     if (a.opcode == B2_OPC_REDUCE_SCATTER) {
       // reduce-scatter: nbytes is ONE block and chunks index into it.  Stage this chunk of all P
@@ -134,9 +132,7 @@ b2_k_reduce_chunked(const B2DevComm c, const B2ReduceArgs a) {
       if (a.has_out) b2_copy_bytes<true>(out + off, mine + off, len);
     }
   }
-  __syncthreads();
-  if (t == 0) b2_st_volatile(c.epoch + blockIdx.x, e);
-  b2_finish_bump(c.ticket, c.ticket + 1, 1u, gridDim.x);
+  b2_staged_end(c, e);
 }
 
 // ---------------------------------------------------------------------------
@@ -304,9 +300,7 @@ b2_k_reduce_scatterv(const B2DevComm c, const B2RsvArgs a) {
   __shared__ size_t s_len[B2_MAX_RANKS];                         // bytes of block `rank` staged by peer q
   __shared__ size_t s_cnt[B2_MAX_RANKS][B2_MAX_RANKS];           // [q][p]: min(s_q[p], N)
   __shared__ size_t s_fold, s_nch;
-  const unsigned ticket = b2_ticket_read(c.ticket);
-  const size_t par = (size_t)(ticket & 1u) * c.stage_half;
-  unsigned e = b2_ld_volatile(c.epoch + blockIdx.x);
+  auto [par, e] = b2_staged_begin(c);
   const int t = threadIdx.x, nt = blockDim.x, P = c.size, r = c.rank;
   const char* in = (const char*)a.in;
   char* out = (char*)a.out;
@@ -327,7 +321,7 @@ b2_k_reduce_scatterv(const B2DevComm c, const B2RsvArgs a) {
     }
   }
   __syncthreads();
-  // chunk ch of every block this rank sends
+  // chunk ch of every block this rank sends (n written out: b2_chunk_len changes this kernel's SASS)
   auto stage = [&](size_t ch) {
     const size_t off = ch * a.chunk;
     for (int p = 0; p < P; ++p)
@@ -382,9 +376,7 @@ b2_k_reduce_scatterv(const B2DevComm c, const B2RsvArgs a) {
   }
   // 4. rows nobody sends are zero: the output is fully written on every call
   a2av_zero(out, fold, a.out_rows * rb);
-  __syncthreads();
-  if (t == 0) b2_st_volatile(c.epoch + blockIdx.x, e);
-  b2_finish_bump(c.ticket, c.ticket + 1, 1u, gridDim.x);
+  b2_staged_end(c, e);
 }
 
 // ---------------------------------------------------------------------------
