@@ -11,6 +11,8 @@
   padded rows (alone and followed by a device-side compaction) and vs NCCL all_gather_into_tensor
 * reduce_scatterv bf16 rows, equal / skewed / small counts, 64 KiB - 256 MiB output per rank, vs the
   reduce_scatter of the zero-padded segments (with the padding gather) and vs NCCL reduce_scatter_tensor
+* gatherv / scatterv bf16 rows (root = last rank), full / half / skewed counts, 64 KiB - 256 MiB per rank, vs
+  gather / scatter of the padded blocks followed by the device-side compaction a user would otherwise write
 * bcast, reduce, gather, scatter (root = last rank) vs NCCL, scan (no NCCL counterpart)
 * sendrecv ring, halo exchange latency
 
@@ -46,6 +48,8 @@ ap.add_argument("--only-allreduce", action="store_true", help="stop after the al
 ap.add_argument("--only-p2p", action="store_true", help="only the p2p ring, barrier and halo lines")
 ap.add_argument("--only-allgatherv", action="store_true", help="only the allgatherv rows")
 ap.add_argument("--only-reduce-scatterv", action="store_true", help="only the reduce_scatterv rows")
+ap.add_argument("--only-gatherv", action="store_true", help="only the gatherv rows")
+ap.add_argument("--only-scatterv", action="store_true", help="only the scatterv rows")
 ap.add_argument("--max-blocks", type=int, default=0, help="override the collective grid cap")
 ap.add_argument("--nvls-pipeline", type=int, default=-1, help="0 / 1: software pipelining of the NVLS allreduce")
 ap.add_argument("--min-bytes", type=int, default=1 << 10)
@@ -227,6 +231,95 @@ def reduce_scatterv_rows():
             del x, padded
 
 
+# ----------------------------------------------------- gatherv / scatterv (root = last rank, 64 KiB - 256 MiB)
+# bf16 rows of hidden size 4096 (8 KiB).  gatherv: every rank holds N rows (nbytes) and contributes count_r of
+# them, "full" (N), "half" (N / 2) or "skewed" (N * (r + 1) / P).  scatterv: the root holds N rows and sends
+# s[q] to rank q, "full" (N / P each: all of them), "half" (N / 2P) or "skewed" (proportional to q + 1).  Next
+# to what a user writes without them: gather / scatter of (P, N, hidden) blocks with the counts, and the
+# device-side compaction on the receiving side (the root packs the gathered rows; the root pads its rows into
+# blocks before the scatter).  Both are capturable, with no host read.  Bandwidth: the rows that cross between
+# the root and the other ranks, times the row bytes, over the time.
+def gatherv_rows():
+    result["gatherv"] = {"full": {}, "half": {}, "skewed": {}}
+    hidden, root = 4096, size - 1
+    for nbytes in [b for b in sizes if (64 << 10) <= b <= (256 << 20)]:
+        n = nbytes // (hidden * 2)
+        for kind in ("full", "half", "skewed"):
+            counts = [n if kind == "full" else n // 2 if kind == "half" else n * (q + 1) // size for q in range(size)]
+            useful = (sum(counts) - counts[root]) * hidden * 2
+            bw = lambda us: round(useful / us / 1e3, 1) if useful else 0.0
+            x = torch.ones(n, hidden, dtype=torch.bfloat16, device=dev)
+            count = torch.tensor(counts[rank], dtype=torch.int64, device=dev)
+            reps = reps_for(nbytes * size // 2)
+            row = {}
+            us = time_graph(lambda: m.gatherv(x, count, root, comm=comm), reps)
+            row["ours"] = {"us": round(us, 2), "busbw": bw(us)}
+            rows = torch.arange(n, device=dev)
+
+            def gather_compact():
+                xs = m.gather(x, root, comm=comm)                                   # root: (P, N, hidden)
+                cs = m.gather(count.view(1), root, comm=comm)
+                if rank != root:
+                    return xs
+                cs = cs.view(size, 1)
+                dest = torch.where(rows < cs, torch.cumsum(cs, 0) - cs + rows, n * size)   # invalid -> pad row
+                out = torch.zeros(n * size + 1, hidden, dtype=x.dtype, device=dev)
+                return out.index_copy_(0, dest.view(-1), xs.view(-1, hidden))[: n * size]
+
+            us = time_graph(gather_compact, reps)
+            row["gather_compact"] = {"us": round(us, 2), "busbw": bw(us)}
+            result["gatherv"][kind][str(nbytes)] = row
+            if rank == 0:
+                print("gatherv", kind, nbytes, {k: (v["us"], v["busbw"]) for k, v in row.items()}, flush=True)
+            del x
+
+
+def scatterv_rows():
+    result["scatterv"] = {"full": {}, "half": {}, "skewed": {}}
+    hidden, root = 4096, size - 1
+    for nbytes in [b for b in sizes if (64 << 10) <= b <= (256 << 20)]:
+        n = nbytes // (hidden * 2)
+        for kind in ("full", "half", "skewed"):
+            counts = [n // size if kind == "full" else n // (2 * size) if kind == "half"
+                      else 2 * n * (q + 1) // (size * (size + 1)) for q in range(size)]
+            useful = (sum(counts) - counts[root]) * hidden * 2
+            bw = lambda us: round(useful / us / 1e3, 1) if useful else 0.0
+            x = torch.ones(n, hidden, dtype=torch.bfloat16, device=dev)
+            send = torch.tensor(counts, dtype=torch.int64, device=dev)
+            reps = reps_for(nbytes)
+            row = {}
+            us = time_graph(lambda: m.scatterv(x, send, root, comm=comm), reps)
+            row["ours"] = {"us": round(us, 2), "busbw": bw(us)}
+            i = torch.arange(n, device=dev)
+            idx = torch.where(i < send.view(size, 1), (torch.cumsum(send, 0) - send).view(size, 1) + i, n)
+            template = torch.empty(n, hidden, dtype=x.dtype, device=dev)
+
+            def pad_scatter():
+                if rank == root:
+                    padded = torch.cat([x, x.new_zeros(1, hidden)])[idx]                # (P, N, hidden)
+                    return m.scatter(padded, root, comm=comm), m.scatter(send.view(size, 1), root, comm=comm)
+                return m.scatter(template, root, comm=comm), m.scatter(send[:1], root, comm=comm)
+
+            us = time_graph(pad_scatter, reps)
+            row["pad_scatter"] = {"us": round(us, 2), "busbw": bw(us)}
+            result["scatterv"][kind][str(nbytes)] = row
+            if rank == 0:
+                print("scatterv", kind, nbytes, {k: (v["us"], v["busbw"]) for k, v in row.items()}, flush=True)
+            del x, template
+
+
+if ns.only_gatherv or ns.only_scatterv:
+    if ns.only_gatherv:
+        gatherv_rows()
+    else:
+        scatterv_rows()
+    if rank == 0:
+        os.makedirs(os.path.dirname(ns.out) or ".", exist_ok=True)
+        with open(ns.out, "w") as f:
+            json.dump(result, f, indent=1)
+    m.flush()
+    sys.exit(0)
+
 if ns.only_reduce_scatterv:
     reduce_scatterv_rows()
     if rank == 0:
@@ -403,6 +496,8 @@ for nbytes in [b for b in sizes if (64 << 10) <= b <= (256 << 20)]:
 
 allgatherv_rows()
 reduce_scatterv_rows()
+gatherv_rows()
+scatterv_rows()
 
 # ---------------------------------------------------------------- rooted ops + scan (per-rank payload = nbytes)
 result.update({"bcast": {}, "reduce": {}, "gather": {}, "scatter": {}, "scan": {}})

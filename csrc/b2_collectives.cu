@@ -270,8 +270,12 @@ b2_k_move(const __grid_constant__ B2DevComm c, const __grid_constant__ B2MoveArg
 // alltoallv: the header holds P send counts and the rows follow in destination order, so peer q's
 // segment for rank r starts after q's rows for the ranks below r.
 // allgatherv (`count` set, "gather mode"): the header holds one count in slot 0 and the rows are staged
-// once -- every rank reads the same segment, from source offset 0.  Only the header write and the
-// schedule (thread-0 code) know the mode; chunks, pulls and the zero fill are shared.
+// once -- every rank reads the same segment, from source offset 0.  gatherv is gather mode in which
+// only the root has output rows: the others pull nothing and write no zeros, but walk the same chunks.
+// scatterv (`root` >= 0, "rooted mode"): alltoallv in which only the root writes a header and stages
+// rows; the schedule reads the root's P counts and every rank pulls its one segment from the root.
+// Only the header code and the schedule (thread-0 code) know the mode; chunks, pulls and the zero fill
+// are shared.
 // ---------------------------------------------------------------------------
 struct B2AlltoallvArgs {
   const void* in;
@@ -279,13 +283,14 @@ struct B2AlltoallvArgs {
   const long long* send_counts;    // [P] rows to each rank (any value: clamped here)
   const long long* place_counts;   // [P] reverse mode: where the segments land (null: packed, forward)
   const long long* count;          // gather mode: the rows this rank sends to every rank (null: alltoallv)
-  long long* recv_counts;          // [P] rows written from each rank
+  long long* recv_counts;          // [P] rows written from each rank (rooted mode: [1], from the root)
   size_t row_bytes;
   size_t in_rows;
   size_t out_rows;
   size_t max_rows;                 // rows a rank may stage, the same on every rank (sizes the staging)
   size_t chunk;
   int opcode;
+  int root;                        // rooted mode: the only rank that sends (-1: every rank sends)
 };
 
 __global__ void __launch_bounds__(B2_THREADS, 1)
@@ -307,7 +312,9 @@ b2_k_rowsv(const __grid_constant__ B2DevComm c, const __grid_constant__ B2Alltoa
     const size_t n = a.in_rows < a.max_rows ? a.in_rows : a.max_rows;
     const long long* want = gather ? a.count : a.send_counts;
     size_t used = 0;
-    for (int q = 0; q < (gather ? 1 : P); ++q) {
+    // rooted mode: the other ranks neither read counts nor stage rows
+    const int nq = gather ? 1 : (a.root < 0 || a.root == r) ? P : 0;
+    for (int q = 0; q < nq; ++q) {
       size_t s = want[q] > 0 ? (size_t)want[q] : 0;
       if (s > n - used) s = n - used;
       used += s;
@@ -332,7 +339,9 @@ b2_k_rowsv(const __grid_constant__ B2DevComm c, const __grid_constant__ B2Alltoa
   if (gather) {
     if (t < P) s_cnt[t][0] = ((const volatile unsigned long long*)(c.stage[t] + par))[0];
   } else if (t < P * P) {
-    s_cnt[t / P][t % P] = ((const volatile unsigned long long*)(c.stage[t / P] + par))[t % P];
+    // rooted mode: only the root's header was written; the other ranks send nothing
+    const int q = t / P;
+    s_cnt[q][t % P] = (a.root < 0 || a.root == q) ? ((const volatile unsigned long long*)(c.stage[q] + par))[t % P] : 0;
   }
   __syncthreads();
   if (t == 0) {
@@ -370,7 +379,7 @@ b2_k_rowsv(const __grid_constant__ B2DevComm c, const __grid_constant__ B2Alltoa
         s_gap[ng][1] = (filled + slot) * rb;
         ++ng;
       }
-      if (blockIdx.x == 0) a.recv_counts[q] = (long long)k;
+      if (blockIdx.x == 0 && (a.root < 0 || a.root == q)) a.recv_counts[a.root < 0 ? q : 0] = (long long)k;
       filled += slot;
     }
     if (a.out_rows > filled) {
@@ -729,6 +738,8 @@ extern "C" size_t b2_stage_need(int opcode, int nranks, size_t blk_bytes) {
       return stride * (size_t)nranks + 4096;
     case B2_OPC_ALLTOALLV:                       // blk_bytes: the most bytes of rows a rank stages
     case B2_OPC_ALLGATHERV:
+    case B2_OPC_GATHERV:
+    case B2_OPC_SCATTERV:
       return B2_A2AV_HDR + stride + 4096;
     case B2_OPC_REDUCE_SCATTERV:                 // blk_bytes: the output rows N x row bytes, one block per rank
       return B2_A2AV_HDR + stride * (size_t)nranks + 4096;
@@ -1097,6 +1108,7 @@ extern "C" int b2_alltoallv(B2Comm* c, const void* in, void* out, size_t row_byt
   a.in = in; a.out = out; a.send_counts = send_counts; a.place_counts = place_counts; a.recv_counts = recv_counts;
   a.row_bytes = row_bytes; a.in_rows = in_rows; a.out_rows = out_rows; a.opcode = B2_OPC_ALLTOALLV;
   a.max_rows = place_counts == nullptr ? in_rows : (size_t)c->dev.size * out_rows;
+  a.root = -1;
   int rc;
   if (send_counts == nullptr || recv_counts == nullptr) {
     b2_set_error("alltoallv: send_counts and recv_counts must be device arrays of %d int64", c->dev.size);
@@ -1117,12 +1129,67 @@ extern "C" int b2_allgatherv(B2Comm* c, const void* in, void* out, size_t row_by
   a.in = in; a.out = out; a.count = count; a.place_counts = place_counts; a.recv_counts = recv_counts;
   a.row_bytes = row_bytes; a.in_rows = in_rows; a.out_rows = out_rows; a.opcode = B2_OPC_ALLGATHERV;
   a.max_rows = in_rows;
+  a.root = -1;
   int rc;
   if (count == nullptr || recv_counts == nullptr) {
     b2_set_error("allgatherv: count and recv_counts must be device arrays of 1 and %d int64", c->dev.size);
     rc = B2_ERR_BAD_ARG;
   } else {
     rc = rowsv_launch(c, a, "allgatherv", stream);
+  }
+  b2_debug_end(dbg, rc);
+  return rc;
+}
+
+// gather mode with output rows on the root only: every other rank stages its rows and walks the same
+// chunks (every rank makes the same arrive / wait sequence) but pulls nothing, writes no zeros and
+// reports zero rows received.
+extern "C" int b2_gatherv(B2Comm* c, const void* in, void* out, size_t row_bytes, size_t in_rows, size_t out_rows,
+                          size_t max_rows, const long long* count, long long* recv_counts,
+                          const long long* place_counts, int root, cudaStream_t stream) {
+  B2DebugScope* dbg = b2_debug_begin(c, "Gatherv", stream, "with %zu rows of %zu bytes to root %d", in_rows,
+                                     row_bytes, root);
+  const bool is_root = c->dev.rank == root;
+  B2AlltoallvArgs a;
+  memset(&a, 0, sizeof a);
+  a.in = in; a.out = out; a.count = count; a.recv_counts = recv_counts;
+  a.place_counts = is_root ? place_counts : nullptr;
+  a.row_bytes = row_bytes; a.in_rows = in_rows; a.out_rows = is_root ? out_rows : 0; a.opcode = B2_OPC_GATHERV;
+  a.max_rows = max_rows;
+  a.root = -1;
+  int rc = check_root(c, root, "gatherv");
+  if (rc == 0 && (count == nullptr || recv_counts == nullptr || (is_root && out == nullptr && out_rows > 0))) {
+    b2_set_error("gatherv: count and recv_counts must be device arrays of 1 and %d int64, and the root needs an "
+                 "output", c->dev.size);
+    rc = B2_ERR_BAD_ARG;
+  } else if (rc == 0) {
+    rc = rowsv_launch(c, a, "gatherv", stream);
+  }
+  b2_debug_end(dbg, rc);
+  return rc;
+}
+
+// alltoallv in rooted mode: the root's send counts, clamped in rank order to its rows, cut its rows into
+// one segment per rank; the other ranks stage nothing and read no counts.
+extern "C" int b2_scatterv(B2Comm* c, const void* in, void* out, size_t row_bytes, size_t in_rows, size_t out_rows,
+                           size_t max_rows, const long long* send_counts, long long* recv_count, int root,
+                           cudaStream_t stream) {
+  B2DebugScope* dbg = b2_debug_begin(c, "Scatterv", stream, "with %zu rows of %zu bytes from root %d", in_rows,
+                                     row_bytes, root);
+  const bool is_root = c->dev.rank == root;
+  B2AlltoallvArgs a;
+  memset(&a, 0, sizeof a);
+  a.in = in; a.out = out; a.send_counts = send_counts; a.recv_counts = recv_count;
+  a.row_bytes = row_bytes; a.in_rows = in_rows; a.out_rows = out_rows; a.opcode = B2_OPC_SCATTERV;
+  a.max_rows = max_rows;
+  a.root = root;
+  int rc = check_root(c, root, "scatterv");
+  if (rc == 0 && ((is_root && send_counts == nullptr) || recv_count == nullptr)) {
+    b2_set_error("scatterv: send_counts (on the root) and recv_count must be device arrays of %d and 1 int64",
+                 c->dev.size);
+    rc = B2_ERR_BAD_ARG;
+  } else if (rc == 0) {
+    rc = rowsv_launch(c, a, "scatterv", stream);
   }
   b2_debug_end(dbg, rc);
   return rc;

@@ -16,9 +16,9 @@
 #include <cstddef>
 #include <cstdint>
 
-#define B2_ABI_VERSION 16  // bump whenever a struct shared with Python or a C signature changes
+#define B2_ABI_VERSION 17  // bump whenever a struct shared with Python or a C signature changes
 #define B2_MAX_RANKS 16          // ranks per NVLink domain we support (8 on HGX H100)
-// bytes of the count header in front of the rows alltoallv / allgatherv / reduce_scatterv stage: one int64
+// bytes of the count header in front of the rows the variable-count collectives stage: one int64
 // per possible rank (keeps the rows 16-byte aligned)
 #define B2_A2AV_HDR ((size_t)B2_MAX_RANKS * sizeof(long long))
 #define B2_MAX_BLOCKS 1024       // max CTAs per collective launch (flag rows)
@@ -88,7 +88,7 @@ enum B2OpCode : int {
   B2_OPC_BARRIER = 0, B2_OPC_ALLREDUCE, B2_OPC_REDUCE, B2_OPC_SCAN, B2_OPC_ALLGATHER,
   B2_OPC_ALLTOALL, B2_OPC_BCAST, B2_OPC_GATHER, B2_OPC_SCATTER, B2_OPC_SEND, B2_OPC_RECV,
   B2_OPC_SENDRECV, B2_OPC_HALO, B2_OPC_REDUCE_SCATTER, B2_OPC_ALLTOALLV, B2_OPC_ALLGATHERV,
-  B2_OPC_REDUCE_SCATTERV, B2_OPC_COUNT
+  B2_OPC_REDUCE_SCATTERV, B2_OPC_GATHERV, B2_OPC_SCATTERV, B2_OPC_COUNT
 };
 
 static inline size_t b2_dtype_size(int dt) {

@@ -493,7 +493,8 @@ extern "C" long long b2_comm_get_option(B2Comm* c, const char* key) {
 static const char* opcode_name(int opc) {
   static const char* names[] = {"Barrier", "Allreduce", "Reduce", "Scan", "Allgather", "Alltoall",
                                 "Bcast", "Gather", "Scatter", "Send", "Recv", "Sendrecv", "Halo",
-                                "Reduce_scatter_block", "Alltoallv", "Allgatherv", "Reduce_scatterv"};
+                                "Reduce_scatter_block", "Alltoallv", "Allgatherv", "Reduce_scatterv", "Gatherv",
+                                "Scatterv"};
   if (opc < 0 || opc >= B2_OPC_COUNT) return "Unknown";
   return names[opc];
 }

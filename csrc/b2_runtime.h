@@ -169,6 +169,20 @@ int b2_alltoallv(B2Comm* c, const void* in, void* out, size_t row_bytes, size_t 
 int b2_allgatherv(B2Comm* c, const void* in, void* out, size_t row_bytes, size_t in_rows, size_t out_rows,
                   const long long* count, long long* recv_counts, const long long* place_counts,
                   cudaStream_t stream);
+// Variable-count gather whose counts stay on the device: b2_allgatherv with output rows on `root` only
+// (`out` and `place_counts` are read there only; the other ranks' recv_counts become zeros).  max_rows
+// bounds the rows any rank stages and must be the same on every rank: it sizes the staging and the
+// chunks; in_rows may differ.
+int b2_gatherv(B2Comm* c, const void* in, void* out, size_t row_bytes, size_t in_rows, size_t out_rows,
+               size_t max_rows, const long long* count, long long* recv_counts, const long long* place_counts,
+               int root, cudaStream_t stream);
+// Variable-count scatter whose counts stay on the device.  On `root`, `in` holds in_rows rows and
+// `send_counts` [nranks] int64, clamped in rank order to min(in_rows, max_rows); neither is read on the
+// other ranks.  Rank q receives its segment, packed from row 0 and clipped to its out_rows, zeros after
+// it; `recv_count`: one int64, the rows written.  max_rows: as for b2_gatherv.
+int b2_scatterv(B2Comm* c, const void* in, void* out, size_t row_bytes, size_t in_rows, size_t out_rows,
+                size_t max_rows, const long long* send_counts, long long* recv_count, int root,
+                cudaStream_t stream);
 // Variable-count reduce-scatter whose counts stay on the device.  `in`: in_rows rows of row_bytes bytes
 // (contiguous; in_rows may differ between ranks); `send_counts`: [nranks] int64, clamped in rank order
 // to in_rows; out_rows (N) must be the same on every rank.  Row i of `out` is `op` folded in rank order

@@ -22,6 +22,7 @@ from ._src import (  # noqa: F401
     comm_reserve,
     flush,
     gather,
+    gatherv,
     has_cuda_support,
     has_sycl_support,
     recv,
@@ -30,6 +31,7 @@ from ._src import (  # noqa: F401
     reduce_scatterv,
     scan,
     scatter,
+    scatterv,
     send,
     send_with_grad,
     sendrecv,
@@ -42,8 +44,9 @@ from ._src.compile_ops import compiled  # noqa: F401  (torch.library / torch.com
 effects_barrier = flush
 
 __all__ = [
-    "allgather", "allgatherv", "allreduce", "alltoall", "alltoallv", "barrier", "bcast", "gather", "recv", "reduce",
-    "reduce_scatter", "reduce_scatterv", "scan", "scatter", "send", "sendrecv", "has_cuda_support", "has_sycl_support",
+    "allgather", "allgatherv", "allreduce", "alltoall", "alltoallv", "barrier", "bcast", "gather", "gatherv", "recv",
+    "reduce", "reduce_scatter", "reduce_scatterv", "scan", "scatter", "scatterv", "send", "sendrecv", "has_cuda_support",
+    "has_sycl_support",
     "MPI", "jit", "compiled", "flush", "effects_barrier", "linear_transpose", "send_with_grad", "comm_reserve",
     "symmetric_empty", "allreduce_",
 ]

@@ -25,12 +25,14 @@ from .collective_ops.alltoallv import alltoallv  # noqa: E402,F401
 from .collective_ops.barrier import barrier  # noqa: E402,F401
 from .collective_ops.bcast import bcast  # noqa: E402,F401
 from .collective_ops.gather import gather  # noqa: E402,F401
+from .collective_ops.gatherv import gatherv  # noqa: E402,F401
 from .collective_ops.recv import recv  # noqa: E402,F401
 from .collective_ops.reduce import reduce  # noqa: E402,F401
 from .collective_ops.reduce_scatter import reduce_scatter  # noqa: E402,F401
 from .collective_ops.reduce_scatterv import reduce_scatterv  # noqa: E402,F401
 from .collective_ops.scan import scan  # noqa: E402,F401
 from .collective_ops.scatter import scatter  # noqa: E402,F401
+from .collective_ops.scatterv import scatterv  # noqa: E402,F401
 from .collective_ops.send import send, send_with_grad  # noqa: E402,F401
 from .collective_ops.sendrecv import sendrecv  # noqa: E402,F401
 

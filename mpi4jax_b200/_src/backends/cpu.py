@@ -247,6 +247,43 @@ def reduce_scatterv(comm: Comm, x: torch.Tensor, send_counts: torch.Tensor, out_
     return out, torch.tensor(recv, dtype=torch.int64)
 
 
+def gatherv(comm: Comm, x: torch.Tensor, count: torch.Tensor, root: int, out_rows: int, max_rows: int,
+            place_counts: Optional[torch.Tensor] = None):
+    """Same rules as the kernel's gather mode with output rows on the root only (csrc/b2_collectives.cu:
+    b2_k_rowsv): everybody gathers every rank's clamped count and rows, the root assembles its output
+    (correctness path).  The other ranks get ``(None, zeros)``."""
+    n = min(max(int(count), 0), x.shape[0], max_rows)
+    counts = _gather_stack(comm, torch.tensor(n, dtype=torch.int64)).tolist()
+    mine = torch.zeros((max(counts), *x.shape[1:]), dtype=x.dtype)
+    mine[:n] = x[:n]
+    stack = _gather_stack(comm, mine)
+    if comm.rank != root:
+        return None, torch.zeros(comm.size, dtype=torch.int64)
+    place = None if place_counts is None else _clamp_in_order(place_counts.tolist(), out_rows)
+    return _pack(stack, counts, [0] * comm.size, out_rows, place)
+
+
+def scatterv(comm: Comm, x: torch.Tensor, send_counts: Optional[torch.Tensor], root: int, out_rows: int,
+             max_rows: int):
+    """Same rules as the kernel's rooted mode (csrc/b2_collectives.cu: b2_k_rowsv): the root broadcasts its
+    send counts, clamped in rank order to its rows, then the rows they cover; each rank keeps its segment,
+    clipped to ``out_rows`` (correctness path)."""
+    P, r = comm.size, comm.rank
+    if r == root:
+        sent = torch.tensor(_clamp_in_order(send_counts.tolist(), min(x.shape[0], max_rows)), dtype=torch.int64)
+    else:
+        sent = torch.zeros(P, dtype=torch.int64)
+    sent = bcast(comm, sent, root).tolist()
+    width = sum(sent)
+    rows = x[:width] if r == root else torch.empty((width, *x.shape[1:]), dtype=x.dtype)
+    rows = bcast(comm, rows, root)
+    k = min(sent[r], out_rows)
+    out = torch.zeros((out_rows, *x.shape[1:]), dtype=x.dtype)
+    d = sum(sent[:r])
+    out[:k] = rows[d: d + k]
+    return out, torch.tensor(k, dtype=torch.int64)
+
+
 def bcast(comm: Comm, x: torch.Tensor, root: int) -> torch.Tensor:
     buf = _bytes_view(x).clone()
     if comm.size > 1:

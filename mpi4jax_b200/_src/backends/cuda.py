@@ -61,7 +61,8 @@ def stage_need(opcode: int, nranks: int, blk_bytes: int) -> int:
     """Staging bytes per parity that an op with ``blk_bytes`` per block needs: the Python twin of
     ``b2_stage_need`` (csrc/b2_collectives.cu), which validates every launch with the same formula."""
     stride = (blk_bytes + 15) & ~15
-    if opcode in (codes.OPC_ALLTOALLV, codes.OPC_ALLGATHERV):    # a header of the counts in front of the rows
+    if opcode in (codes.OPC_ALLTOALLV, codes.OPC_ALLGATHERV, codes.OPC_GATHERV, codes.OPC_SCATTERV):
+        # a header of the counts in front of the rows
         return ALLTOALLV_HEADER + stride + 4096
     if opcode == codes.OPC_REDUCE_SCATTERV:                        # the header, then one block per rank
         return ALLTOALLV_HEADER + stride * nranks + 4096
@@ -70,8 +71,8 @@ def stage_need(opcode: int, nranks: int, blk_bytes: int) -> int:
 
 
 #: bytes in front of the rows an alltoallv stages: the rank's clamped send counts, one int64 per possible
-#: rank (B2_A2AV_HDR; MAX_RANKS is checked against the library at import).  allgatherv reuses the slot
-#: for its one count, which keeps the rows 16-byte aligned
+#: rank (B2_A2AV_HDR; MAX_RANKS is checked against the library at import).  allgatherv and gatherv reuse the
+#: slot for their one count, which keeps the rows 16-byte aligned
 ALLTOALLV_HEADER = native.MAX_RANKS * 8
 
 
@@ -573,6 +574,47 @@ class NativeComm:
         return self._rowsv(_lib().b2_allgatherv, "Allgatherv", codes.OPC_ALLGATHERV, x.shape[0], x, out_rows, count,
                            None if place_counts is None else place_counts.data_ptr())
 
+    def gatherv(self, x: torch.Tensor, count: torch.Tensor, root: int, out_rows: int, max_rows: int,
+                place_counts: Optional[torch.Tensor] = None):
+        """``(out, recv_counts)``: allgatherv with output rows on ``root`` only (``collective_ops/gatherv.py``
+        states the rules); ``out`` is None elsewhere.  ``max_rows``: the rows any rank may stage, the same
+        on every rank.  ``place_counts`` (read on the root): the reverse mode, the adjoint of a scatterv
+        with these send counts."""
+        x = _prep(x)
+        is_root = self.comm.rank == root
+        row_bytes = math.prod(x.shape[1:]) * x.element_size()
+        out = torch.empty((out_rows, *x.shape[1:]), dtype=x.dtype, device=x.device) if is_root else None
+        recv_counts = torch.empty(self.comm.size, dtype=torch.int64, device=x.device)
+        count = count.to(torch.int64).contiguous()
+        if place_counts is not None and is_root:
+            place_counts = place_counts.to(torch.int64).contiguous()
+        else:
+            place_counts = None
+        self.ensure_stage(codes.OPC_GATHERV, max_rows * row_bytes)
+        rc = _lib().b2_gatherv(self.handle, x.data_ptr(), out.data_ptr() if is_root else None, row_bytes, x.shape[0],
+                               out_rows if is_root else 0, max_rows, count.data_ptr(), recv_counts.data_ptr(),
+                               None if place_counts is None else place_counts.data_ptr(), root, self._stream())
+        self._check(rc, "Gatherv")
+        return out, recv_counts
+
+    def scatterv(self, x: torch.Tensor, send_counts: Optional[torch.Tensor], root: int, out_rows: int,
+                 max_rows: int):
+        """``(out, recv_count)``: this rank's segment of the root's rows (``collective_ops/scatterv.py``
+        states the rules).  ``x`` and ``send_counts`` are read on the root only; ``max_rows``: the root
+        rows that may be sent, the same on every rank."""
+        is_root = self.comm.rank == root
+        row_bytes = math.prod(x.shape[1:]) * x.element_size()
+        out = torch.empty((out_rows, *x.shape[1:]), dtype=x.dtype, device=x.device)
+        recv_count = torch.empty((), dtype=torch.int64, device=x.device)
+        src = _prep(x) if is_root else None
+        counts = send_counts.to(torch.int64).contiguous() if is_root else None
+        self.ensure_stage(codes.OPC_SCATTERV, max_rows * row_bytes)
+        rc = _lib().b2_scatterv(self.handle, src.data_ptr() if is_root else None, out.data_ptr(), row_bytes,
+                                x.shape[0], out_rows, max_rows, counts.data_ptr() if is_root else None,
+                                recv_count.data_ptr(), root, self._stream())
+        self._check(rc, "Scatterv")
+        return out, recv_count
+
     def reduce_scatterv(self, x: torch.Tensor, send_counts: torch.Tensor, out_rows: int, op_code: int):
         """``(out, recv_counts)``: ``op`` over the ranks' segments for this rank, folded in rank order
         (``collective_ops/reduce_scatterv.py`` states the rules); the counts are read on the device."""
@@ -706,7 +748,8 @@ def _nvtx_wrap(name: str, fn):
 #: ``MPI4JAX_B200_NVTX=1``: one NVTX range per op (visible in Nsight Systems timelines); the
 #: methods are left untouched otherwise, so the fast path pays nothing (SURVEY 5.1)
 NVTX_OPS = ("barrier", "allreduce", "reduce", "scan", "allgather", "alltoall", "bcast", "gather", "scatter",
-            "send", "recv", "sendrecv", "reduce_scatter", "alltoallv", "allgatherv", "reduce_scatterv",
+            "send", "recv", "sendrecv", "reduce_scatter", "alltoallv", "allgatherv", "reduce_scatterv", "gatherv",
+            "scatterv",
             "gemm_allreduce",
             "halo_exchange")
 if env_flag("MPI4JAX_B200_NVTX", False):

@@ -103,6 +103,16 @@ class HostStagedComm:
         out, recv_counts = _cpu.reduce_scatterv(self.comm, self._down(x), self._down(send_counts), out_rows, op_code)
         return self._up(out, x), self._up(recv_counts, x)
 
+    def gatherv(self, x, count, root: int, out_rows: int, max_rows: int, place_counts=None):
+        out, recv_counts = _cpu.gatherv(self.comm, self._down(x), self._down(count), root, out_rows, max_rows,
+                                        None if place_counts is None else self._down(place_counts))
+        return self._up(out, x), self._up(recv_counts, x)
+
+    def scatterv(self, x, send_counts, root: int, out_rows: int, max_rows: int):
+        out, recv_count = _cpu.scatterv(self.comm, self._down(x), None if send_counts is None else
+                                        self._down(send_counts), root, out_rows, max_rows)
+        return self._up(out, x), self._up(recv_count, x)
+
     def bcast(self, x, root: int):
         out = _cpu.bcast(self.comm, self._down(x), root)
         return x if self.comm.rank == root else self._up(out, x)

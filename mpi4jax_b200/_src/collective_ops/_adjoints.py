@@ -53,6 +53,34 @@ def reduce_scatterv(F, g, comm, rows, send_counts):
     return F._allgatherv_reverse(g.contiguous(), send_counts, rows, comm)
 
 
+def gatherv(F, g, comm, root, rows, max_rows, recv_counts):
+    """The scatterv of the root's cotangent with its received counts as send counts, into the differentiated
+    call's ``rows`` input rows: each rank gets back what the root kept of its rows, and only those rows
+    travel.  The root's cotangent has the root's capacity in rows, which the other ranks do not know, so the
+    scatterv stages with the bound ``nproc * max_rows`` that every rank knows.  On the other ranks the
+    result was ``x`` itself, so their own cotangent adds (as for gather)."""
+    is_root = comm.Get_rank() == root
+    back = F._scatterv_bounded(g.contiguous(), recv_counts if is_root else None, root, rows,
+                               max_rows * comm.Get_size(), comm)
+    return back if is_root else back + g
+
+
+def gatherv_reverse(F, g, comm, root, rows, max_rows, place_counts):
+    """The forward scatterv that the reverse mode is the adjoint of: the root's cotangent by the place counts,
+    into each rank's ``rows`` input rows of the differentiated call.  The other ranks' result was zeros, so
+    their cotangent drops."""
+    is_root = comm.Get_rank() == root
+    return F._scatterv_bounded(g.contiguous(), place_counts if is_root else None, root, rows, max_rows, comm)
+
+
+def scatterv(F, g, comm, root, rows, max_rows, recv_count, send_counts):
+    """The reverse-mode gatherv of the cotangent: each rank's first ``recv_count`` rows land on the root where
+    they were taken from, in an output of the differentiated call's ``rows`` input rows; the other ranks'
+    inputs were templates and get zeros that are the gatherv's result, so that a second derivative runs
+    its adjoint, a scatterv from the root, on every rank."""
+    return F._gatherv_reverse(g.contiguous(), recv_count, send_counts, root, rows, max_rows, comm)
+
+
 def bcast(F, g, root, comm):
     """The sum of the cotangents on the root, zero elsewhere (the input there is only a template)."""
     total = F.reduce(g.contiguous(), SUM, root, comm=comm)

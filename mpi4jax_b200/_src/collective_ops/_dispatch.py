@@ -165,9 +165,9 @@ def as_counts(counts, x: torch.Tensor, scalar: bool = False) -> torch.Tensor:
 
 def check_rowsv_args(opname: str, comm: Comm, x: torch.Tensor, counts: torch.Tensor, out_rows: int,
                      name: str) -> None:
-    """Host-side checks of an alltoallv / allgatherv / reduce_scatterv call.  Every entry point (the op, its
-    ``compiled`` twin, the raw ``torch.ops`` op and its fake kernel, the backends) passes through them: the
-    kernel dereferences the counts as int64 values in x's device memory -- one for allgatherv's ``count``,
+    """Host-side checks of a variable-count call.  Every entry point (the op, its ``compiled`` twin, the raw
+    ``torch.ops`` op and its fake kernel, the backends) passes through them: the kernel dereferences the
+    counts as int64 values in x's device memory -- one for the ``count`` of allgatherv and gatherv,
     ``nproc`` for every other counts argument -- so anything else must be refused before the launch."""
     shape, shape_text = ((), "()") if name == "count" else ((comm.Get_size(),), "(nproc,)")
     check_rows(opname, x)
@@ -185,14 +185,14 @@ def check_rowsv_args(opname: str, comm: Comm, x: torch.Tensor, counts: torch.Ten
 
 def rowsv_capacity(opname: str, comm: Comm, x: torch.Tensor, counts: torch.Tensor, recv_capacity,
                    name: str):
-    """The output rows of a public alltoallv / allgatherv / reduce_scatterv call or its ``compiled`` twin,
-    after the checks: ``recv_capacity``, or by default the rows that never drop one -- ``N * nproc`` for the
-    gathering ops, ``N`` for reduce_scatterv (when every rank passes ``N`` rows)."""
+    """The output rows of a public variable-count call or its ``compiled`` twin, after the checks:
+    ``recv_capacity``, or by default the rows that never drop one -- ``N * nproc`` for the gathering ops,
+    ``N`` for reduce_scatterv (when every rank passes ``N`` rows) and scatterv."""
     check_rows(opname, x)
     if recv_capacity is not None:
         out_rows = recv_capacity
     else:
-        out_rows = x.shape[0] * (1 if opname == "Reduce_scatterv" else comm.Get_size())
+        out_rows = x.shape[0] * (1 if opname in ("Reduce_scatterv", "Scatterv") else comm.Get_size())
     check_rowsv_args(opname, comm, x, counts, out_rows, name)
     return out_rows
 
@@ -235,6 +235,50 @@ def reduce_scatterv(comm: Comm, x: torch.Tensor, send_counts: torch.Tensor, out_
     if x.is_cuda:
         return comm._native_comm().reduce_scatterv(x, send_counts, out_rows, op_code)
     return _cpu_rowsv("Reduce_scatterv", _cpu.reduce_scatterv, comm, x, send_counts, out_rows, op_code)
+
+
+def _cpu_rooted(opname: str, fn, comm: Comm, x: torch.Tensor, root: int, where: str, *args):
+    """``fn(comm, x, *args)``, the CPU backend's gatherv / scatterv, with its log line."""
+    row_bytes = math.prod(x.shape[1:]) * x.element_size()
+    done = _log(comm, opname, f"with {x.shape[0]} rows of {row_bytes} bytes {where} root {root}")
+    out = fn(comm, x, *args)
+    if done:
+        done()
+    return out
+
+
+def gatherv(comm: Comm, x: torch.Tensor, count: torch.Tensor, root: int, out_rows: int, max_rows: int,
+            place_counts: Optional[torch.Tensor] = None):
+    """``(out, recv_counts)``; ``out`` is None on the ranks other than ``root``, which read neither
+    ``out_rows`` nor ``place_counts``.  ``max_rows``: the rows any rank may contribute, the same on every
+    rank (it sizes the staging)."""
+    _plain(x)
+    is_root = comm.Get_rank() == root
+    check_rowsv_args("Gatherv", comm, x, count, out_rows, "count")
+    if place_counts is not None and is_root:
+        check_rowsv_args("Gatherv", comm, x, place_counts, out_rows, "place_counts")
+    if x.is_cuda:
+        return comm._native_comm().gatherv(x, count, root, out_rows, max_rows, place_counts)
+    return _cpu_rooted("Gatherv", _cpu.gatherv, comm, x, root, "to", count, root, out_rows, max_rows, place_counts)
+
+
+def scatterv(comm: Comm, x: torch.Tensor, send_counts: Optional[torch.Tensor], root: int, out_rows: int,
+             max_rows: int):
+    """``(out, recv_count)``.  ``x`` and ``send_counts`` are read on ``root`` only (elsewhere ``x`` gives
+    the row shape and dtype, and ``send_counts`` may be None); ``max_rows``: the root rows that may be
+    sent, the same on every rank (it sizes the staging)."""
+    _plain(x)
+    if send_counts is not None:
+        check_rowsv_args("Scatterv", comm, x, send_counts, out_rows, "send_counts")
+    elif comm.Get_rank() == root:
+        raise ValueError("Scatterv send_counts must be given on the root")
+    else:
+        check_rows("Scatterv", x)
+        if out_rows < 0:
+            raise ValueError(f"Scatterv recv_capacity must be >= 0 (got {out_rows})")
+    if x.is_cuda:
+        return comm._native_comm().scatterv(x, send_counts, root, out_rows, max_rows)
+    return _cpu_rooted("Scatterv", _cpu.scatterv, comm, x, root, "from", send_counts, root, out_rows, max_rows)
 
 
 def bcast(comm: Comm, x: torch.Tensor, root: int) -> torch.Tensor:

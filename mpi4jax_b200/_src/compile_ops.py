@@ -300,6 +300,103 @@ def _(x, root, comm_id):
     return torch.empty_like(x, memory_format=torch.contiguous_format)
 
 
+@custom_op("mpi4jax_b200::gatherv_root", mutates_args=())
+def _gatherv_root(x: torch.Tensor, count: torch.Tensor, root: int, out_rows: int, max_rows: int, comm_id: int,
+                  reverse: bool, place_counts: Optional[torch.Tensor] = None) -> tuple[torch.Tensor, torch.Tensor]:
+    # the root's output; in the reverse mode (scatterv's adjoint) also run on the other ranks, which get zeros
+    comm = _c(comm_id)
+    out, recv_counts = _dispatch.gatherv(comm, x.contiguous(), count, root, out_rows, max_rows, place_counts)
+    return (out if comm.Get_rank() == root else x.new_zeros((out_rows, *x.shape[1:]))), recv_counts
+
+
+@_gatherv_root.register_fake
+def _(x, count, root, out_rows, max_rows, comm_id, reverse, place_counts=None):
+    comm = _c(comm_id)
+    _dispatch.check_rowsv_args("Gatherv", comm, x, count, out_rows, "count")
+    if place_counts is not None:
+        _dispatch.check_rowsv_args("Gatherv", comm, x, place_counts, out_rows, "place_counts")
+    return x.new_empty((out_rows, *x.shape[1:])), x.new_empty((comm.Get_size(),), dtype=torch.int64)
+
+
+def _gatherv_root_setup(ctx, inputs, output):
+    x, _, ctx.root, _, ctx.max_rows, ctx.comm_id, ctx.reverse, place_counts = inputs
+    ctx.in_rows = x.shape[0]
+    ctx.save_for_backward(output[1], place_counts)
+
+
+def _gatherv_root_backward(ctx, g, _g_counts):
+    recv_counts, place_counts = ctx.saved_tensors
+    comm = _c(ctx.comm_id)
+    if ctx.reverse:
+        back = _adjoints.gatherv_reverse(compiled, g, comm, ctx.root, ctx.in_rows, ctx.max_rows, place_counts)
+    else:
+        back = _adjoints.gatherv(compiled, g, comm, ctx.root, ctx.in_rows, ctx.max_rows, recv_counts)
+    return back, None, None, None, None, None, None, None
+
+
+_gatherv_root.register_autograd(_gatherv_root_backward, setup_context=_gatherv_root_setup)
+
+
+@custom_op("mpi4jax_b200::gatherv_leaf", mutates_args=())
+def _gatherv_leaf(x: torch.Tensor, count: torch.Tensor, root: int, max_rows: int,
+                  comm_id: int) -> tuple[torch.Tensor, torch.Tensor]:
+    _, recv_counts = _dispatch.gatherv(_c(comm_id), x.contiguous(), count, root, 0, max_rows)
+    return x.clone(), recv_counts
+
+
+@_gatherv_leaf.register_fake
+def _(x, count, root, max_rows, comm_id):
+    comm = _c(comm_id)
+    _dispatch.check_rowsv_args("Gatherv", comm, x, count, 0, "count")
+    return torch.empty_like(x, memory_format=torch.contiguous_format), x.new_empty((comm.Get_size(),),
+                                                                                    dtype=torch.int64)
+
+
+def _gatherv_leaf_setup(ctx, inputs, output):
+    x, _, ctx.root, ctx.max_rows, ctx.comm_id = inputs
+    ctx.in_rows = x.shape[0]
+
+
+def _gatherv_leaf_backward(ctx, g, _g_counts):
+    back = _adjoints.gatherv(compiled, g, _c(ctx.comm_id), ctx.root, ctx.in_rows, ctx.max_rows, None)
+    return back, None, None, None, None
+
+
+_gatherv_leaf.register_autograd(_gatherv_leaf_backward, setup_context=_gatherv_leaf_setup)
+
+
+@custom_op("mpi4jax_b200::scatterv", mutates_args=())
+def _scatterv(x: torch.Tensor, send_counts: Optional[torch.Tensor], root: int, out_rows: int, max_rows: int,
+              comm_id: int) -> tuple[torch.Tensor, torch.Tensor]:
+    return _dispatch.scatterv(_c(comm_id), x.contiguous(), send_counts, root, out_rows, max_rows)
+
+
+@_scatterv.register_fake
+def _(x, send_counts, root, out_rows, max_rows, comm_id):
+    comm = _c(comm_id)
+    if send_counts is not None:
+        _dispatch.check_rowsv_args("Scatterv", comm, x, send_counts, out_rows, "send_counts")
+    elif comm.Get_rank() == root:
+        raise ValueError("Scatterv send_counts must be given on the root")
+    return x.new_empty((out_rows, *x.shape[1:])), x.new_empty((), dtype=torch.int64)
+
+
+def _scatterv_setup(ctx, inputs, output):
+    x, send_counts, ctx.root, _, ctx.max_rows, ctx.comm_id = inputs
+    ctx.in_rows = x.shape[0]
+    ctx.save_for_backward(send_counts, output[1])
+
+
+def _scatterv_backward(ctx, g, _g_count):
+    send_counts, recv_count = ctx.saved_tensors
+    back = _adjoints.scatterv(compiled, g, _c(ctx.comm_id), ctx.root, ctx.in_rows, ctx.max_rows, recv_count,
+                              send_counts)
+    return back, None, None, None, None, None
+
+
+_scatterv.register_autograd(_scatterv_backward, setup_context=_scatterv_setup)
+
+
 @custom_op("mpi4jax_b200::scatter", mutates_args=())
 def _scatter(x: torch.Tensor, root: int, comm_id: int, is_root: bool) -> torch.Tensor:
     shape = tuple(x.shape[1:]) if is_root else tuple(x.shape)
@@ -371,7 +468,7 @@ _sendrecv.register_autograd(_sendrecv_backward, setup_context=_sendrecv_setup)
 
 ALL_OPS = ("allreduce", "allgather", "alltoall", "bcast", "scan", "reduce", "gather_root", "gather_leaf",
            "scatter", "barrier", "send", "recv", "sendrecv", "reduce_scatter", "alltoallv", "allgatherv",
-           "reduce_scatterv")
+           "reduce_scatterv", "gatherv_root", "gatherv_leaf", "scatterv")
 ORDERED_EFFECT = False
 try:  # the ordered effect: AOTAutograd threads a token through these ops in program order
     from torch._higher_order_ops.effects import _EffectType, _register_effectful_op
@@ -441,6 +538,41 @@ class compiled:
         comm = comm or get_default_comm()
         cap = _dispatch.rowsv_capacity("Reduce_scatterv", comm, x, send_counts, recv_capacity, "send_counts")
         return torch.ops.mpi4jax_b200.reduce_scatterv(x, send_counts, cap, as_op(op).code, comm._id)
+
+    @staticmethod
+    def gatherv(x, count, root, *, recv_capacity=None, comm=None):
+        """``(out, recv_counts)`` of :func:`mpi4jax_b200.gatherv`; ``count`` must be an integer device tensor
+        of shape ``()``.  On the root the ``gatherv_root`` op, elsewhere ``gatherv_leaf``, whose result is a
+        copy of ``x``."""
+        comm = comm or get_default_comm()
+        if comm.Get_rank() == root:
+            cap = _dispatch.rowsv_capacity("Gatherv", comm, x, count, recv_capacity, "count")
+            return torch.ops.mpi4jax_b200.gatherv_root(x, count, int(root), cap, x.shape[0], comm._id, False)
+        return torch.ops.mpi4jax_b200.gatherv_leaf(x, count, int(root), x.shape[0], comm._id)
+
+    @staticmethod
+    def _gatherv_reverse(y, count, place_counts, root, rows, max_rows, comm):
+        # the counterpart of the eager gatherv_reverse, for scatterv's adjoint (collective_ops/_adjoints.py)
+        if comm.Get_rank() != root:
+            place_counts = None
+        return torch.ops.mpi4jax_b200.gatherv_root(y, count, root, rows, max_rows, comm._id, True, place_counts)[0]
+
+    @staticmethod
+    def scatterv(x, send_counts, root, *, recv_capacity=None, comm=None):
+        """``(out, recv_count)`` of :func:`mpi4jax_b200.scatterv`; ``send_counts`` must be a device tensor of
+        shape ``(nproc,)`` on the root (None or such a tensor elsewhere)."""
+        comm = comm or get_default_comm()
+        if send_counts is None:
+            cap = x.shape[0] if recv_capacity is None else recv_capacity
+            _dispatch.check_rows("Scatterv", x)
+        else:
+            cap = _dispatch.rowsv_capacity("Scatterv", comm, x, send_counts, recv_capacity, "send_counts")
+        return torch.ops.mpi4jax_b200.scatterv(x, send_counts, int(root), cap, x.shape[0], comm._id)
+
+    @staticmethod
+    def _scatterv_bounded(x, send_counts, root, rows, max_rows, comm):
+        # the counterpart of the eager scatterv_bounded, for gatherv's adjoint (collective_ops/_adjoints.py)
+        return torch.ops.mpi4jax_b200.scatterv(x, send_counts, root, rows, max_rows, comm._id)[0]
 
     @staticmethod
     def bcast(x, root, *, comm=None):

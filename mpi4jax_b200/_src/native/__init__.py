@@ -184,6 +184,15 @@ _SIGNATURES = {
         c_int,
         [c_void_p, c_void_p, c_void_p, c_size_t, c_size_t, c_size_t, c_void_p, c_void_p, c_void_p, c_void_p],
     ),
+    "b2_gatherv": (
+        c_int,
+        [c_void_p, c_void_p, c_void_p, c_size_t, c_size_t, c_size_t, c_size_t, c_void_p, c_void_p, c_void_p, c_int,
+         c_void_p],
+    ),
+    "b2_scatterv": (
+        c_int,
+        [c_void_p, c_void_p, c_void_p, c_size_t, c_size_t, c_size_t, c_size_t, c_void_p, c_void_p, c_int, c_void_p],
+    ),
     "b2_reduce_scatterv": (
         c_int,
         [c_void_p, c_void_p, c_void_p, c_size_t, c_size_t, c_size_t, c_void_p, c_void_p, c_int, c_int, c_void_p],
@@ -220,7 +229,7 @@ _SIGNATURES = {
 
 
 #: must equal B2_ABI_VERSION in csrc/b2_common.h
-ABI_VERSION = 16
+ABI_VERSION = 17
 #: must equal B2_MAX_RANKS in csrc/b2_common.h (ranks per communicator; sizes the alltoallv count header)
 MAX_RANKS = 16
 _ABI_FIELDS = ("abi_version", "sizeof_status_record", "sizeof_halo_desc", "sizeof_swe_params",

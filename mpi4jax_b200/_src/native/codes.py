@@ -45,5 +45,7 @@ OPC_REDUCE_SCATTER = 13
 OPC_ALLTOALLV = 14
 OPC_ALLGATHERV = 15
 OPC_REDUCE_SCATTERV = 16
+OPC_GATHERV = 17
+OPC_SCATTERV = 18
 
 ANY = -1  # ANY_SOURCE / ANY_TAG on the wire

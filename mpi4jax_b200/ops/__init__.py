@@ -2,8 +2,8 @@
 reference's one-MPI-call-per-op model (fused multi-field halo exchange)."""
 
 from .._src import (  # noqa: F401
-    allgather, allgatherv, allreduce, alltoall, alltoallv, barrier, bcast, gather, recv, reduce, reduce_scatter,
-    reduce_scatterv, scan, scatter, send, send_with_grad, sendrecv,
+    allgather, allgatherv, allreduce, alltoall, alltoallv, barrier, bcast, gather, gatherv, recv, reduce,
+    reduce_scatter, reduce_scatterv, scan, scatter, scatterv, send, send_with_grad, sendrecv,
 )
 from .halo import halo_exchange  # noqa: F401
 from .linear import linear_allreduce  # noqa: F401
