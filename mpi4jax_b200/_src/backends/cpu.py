@@ -196,6 +196,16 @@ def _pack(stack: torch.Tensor, counts: list, displs: list, out_rows: int, place:
     return out, torch.tensor(recv, dtype=torch.int64)
 
 
+def _gather_segments(comm: Comm, x: torch.Tensor, counts: list, n: int):
+    """Every rank's ``counts`` clamped in rank order to its first ``n`` rows, ``[q][p]``, and the rows they
+    cover, zero-padded to a common width, ``(P, width, *S)``."""
+    sent = _clamp_in_order(counts, n)
+    counts = _gather_stack(comm, torch.tensor(sent, dtype=torch.int64)).tolist()
+    mine = torch.zeros((max(sum(row) for row in counts), *x.shape[1:]), dtype=x.dtype)
+    mine[: sum(sent)] = x[: sum(sent)]
+    return counts, _gather_stack(comm, mine)
+
+
 def alltoallv(comm: Comm, x: torch.Tensor, send_counts: torch.Tensor, out_rows: int,
               place_counts: Optional[torch.Tensor] = None):
     """Same rules as the kernel (csrc/b2_collectives.cu: b2_k_rowsv): everybody gathers every
@@ -203,12 +213,7 @@ def alltoallv(comm: Comm, x: torch.Tensor, send_counts: torch.Tensor, out_rows: 
     P, r = comm.size, comm.rank
     rows = x.shape[0]
     max_rows = rows if place_counts is None else P * out_rows
-    sent = _clamp_in_order(send_counts.tolist(), min(rows, max_rows))
-    counts = _gather_stack(comm, torch.tensor(sent, dtype=torch.int64)).tolist()      # [q][p]
-    width = max(sum(row) for row in counts)
-    mine = torch.zeros((width, *x.shape[1:]), dtype=x.dtype)
-    mine[: sum(sent)] = x[: sum(sent)]
-    stack = _gather_stack(comm, mine)                                                   # (P, width, *S)
+    counts, stack = _gather_segments(comm, x, send_counts.tolist(), min(rows, max_rows))
     place = None if place_counts is None else _clamp_in_order(place_counts.tolist(), out_rows)
     return _pack(stack, [row[r] for row in counts], [sum(row[:r]) for row in counts], out_rows, place)
 
@@ -230,12 +235,7 @@ def reduce_scatterv(comm: Comm, x: torch.Tensor, send_counts: torch.Tensor, out_
     run of rows over the ranks whose segment reaches it, in rank order (correctness path)."""
     P, r = comm.size, comm.rank
     check_op(x.dtype, op_code)         # on every call, also when no row has two contributors
-    sent = _clamp_in_order(send_counts.tolist(), x.shape[0])
-    counts = _gather_stack(comm, torch.tensor(sent, dtype=torch.int64)).tolist()       # [q][p]
-    width = max(sum(row) for row in counts)
-    mine = torch.zeros((width, *x.shape[1:]), dtype=x.dtype)
-    mine[: sum(sent)] = x[: sum(sent)]
-    stack = _gather_stack(comm, mine)                                                   # (P, width, *S)
+    counts, stack = _gather_segments(comm, x, send_counts.tolist(), x.shape[0])
     recv = [min(row[r], out_rows) for row in counts]
     displ = [sum(row[:r]) for row in counts]
     out = torch.zeros((out_rows, *x.shape[1:]), dtype=x.dtype)
@@ -252,15 +252,11 @@ def gatherv(comm: Comm, x: torch.Tensor, count: torch.Tensor, root: int, out_row
     """Same rules as the kernel's gather mode with output rows on the root only (csrc/b2_collectives.cu:
     b2_k_rowsv): everybody gathers every rank's clamped count and rows, the root assembles its output
     (correctness path).  The other ranks get ``(None, zeros)``."""
-    n = min(max(int(count), 0), x.shape[0], max_rows)
-    counts = _gather_stack(comm, torch.tensor(n, dtype=torch.int64)).tolist()
-    mine = torch.zeros((max(counts), *x.shape[1:]), dtype=x.dtype)
-    mine[:n] = x[:n]
-    stack = _gather_stack(comm, mine)
+    counts, stack = _gather_segments(comm, x, [count], min(x.shape[0], max_rows))
     if comm.rank != root:
         return None, torch.zeros(comm.size, dtype=torch.int64)
     place = None if place_counts is None else _clamp_in_order(place_counts.tolist(), out_rows)
-    return _pack(stack, counts, [0] * comm.size, out_rows, place)
+    return _pack(stack, [n for (n,) in counts], [0] * comm.size, out_rows, place)
 
 
 def scatterv(comm: Comm, x: torch.Tensor, send_counts: Optional[torch.Tensor], root: int, out_rows: int,

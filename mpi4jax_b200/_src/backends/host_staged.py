@@ -51,6 +51,13 @@ class HostStagedComm:
             return None
         return y.to(like.device, non_blocking=False) if like.device.type != "cpu" else y
 
+    def _rowsv(self, fn, x, *args):
+        """``fn``, a variable-count op of the CPU backend, on host copies of ``x`` and of the tensor arguments;
+        its two outputs come back to ``x``'s device."""
+        out, counts = fn(self.comm, self._down(x), *[self._down(a) if isinstance(a, torch.Tensor) else a
+                                                      for a in args])
+        return self._up(out, x), self._up(counts, x)
+
     def _unsupported(self, what: str):
         raise MPIError(f"{what} needs the native NVLink transport, but this communicator uses host "
                        f"staging ({self.reason or 'requested'}); use the 15 primitives instead")
@@ -90,28 +97,19 @@ class HostStagedComm:
         return self._up(_cpu.alltoall(self.comm, self._down(x)), x)
 
     def alltoallv(self, x, send_counts, out_rows: int, place_counts=None):
-        out, recv_counts = _cpu.alltoallv(self.comm, self._down(x), self._down(send_counts), out_rows,
-                                          None if place_counts is None else self._down(place_counts))
-        return self._up(out, x), self._up(recv_counts, x)
+        return self._rowsv(_cpu.alltoallv, x, send_counts, out_rows, place_counts)
 
     def allgatherv(self, x, count, out_rows: int, place_counts=None):
-        out, recv_counts = _cpu.allgatherv(self.comm, self._down(x), self._down(count), out_rows,
-                                           None if place_counts is None else self._down(place_counts))
-        return self._up(out, x), self._up(recv_counts, x)
+        return self._rowsv(_cpu.allgatherv, x, count, out_rows, place_counts)
 
     def reduce_scatterv(self, x, send_counts, out_rows: int, op_code: int):
-        out, recv_counts = _cpu.reduce_scatterv(self.comm, self._down(x), self._down(send_counts), out_rows, op_code)
-        return self._up(out, x), self._up(recv_counts, x)
+        return self._rowsv(_cpu.reduce_scatterv, x, send_counts, out_rows, op_code)
 
     def gatherv(self, x, count, root: int, out_rows: int, max_rows: int, place_counts=None):
-        out, recv_counts = _cpu.gatherv(self.comm, self._down(x), self._down(count), root, out_rows, max_rows,
-                                        None if place_counts is None else self._down(place_counts))
-        return self._up(out, x), self._up(recv_counts, x)
+        return self._rowsv(_cpu.gatherv, x, count, root, out_rows, max_rows, place_counts)
 
     def scatterv(self, x, send_counts, root: int, out_rows: int, max_rows: int):
-        out, recv_count = _cpu.scatterv(self.comm, self._down(x), None if send_counts is None else
-                                        self._down(send_counts), root, out_rows, max_rows)
-        return self._up(out, x), self._up(recv_count, x)
+        return self._rowsv(_cpu.scatterv, x, send_counts, root, out_rows, max_rows)
 
     def bcast(self, x, root: int):
         out = _cpu.bcast(self.comm, self._down(x), root)

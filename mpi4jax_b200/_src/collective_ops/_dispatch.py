@@ -20,10 +20,17 @@ from ..comm import Comm, Status
 from ..native import codes
 
 
-def _log(comm: Comm, opname: str, details: str):
-    if native.get_logging():
-        return _cpu.log_call(comm.rank, opname, details)
-    return None
+def _on_cpu(comm: Comm, opname: str, details: str, fn, *args):
+    """``fn(comm, *args)``, a call of the CPU backend, between its ``MPI4JAX_DEBUG`` lines."""
+    done = _cpu.log_call(comm.rank, opname, details) if native.get_logging() else None
+    out = fn(comm, *args)
+    if done:
+        done()
+    return out
+
+
+def _rows_text(x: torch.Tensor) -> str:
+    return f"with {x.shape[0]} rows of {math.prod(x.shape[1:]) * x.element_size()} bytes"
 
 
 _is_wrapped = torch._C._functorch.is_functorch_wrapped_tensor
@@ -77,76 +84,50 @@ def barrier(comm: Comm) -> None:
     if comm.device.type == "cuda":
         comm._native_comm().barrier()
         return
-    done = _log(comm, "Barrier", "")
-    _cpu.barrier(comm)
-    if done:
-        done()
+    _on_cpu(comm, "Barrier", "", _cpu.barrier)
 
 
 def allreduce(comm: Comm, x: torch.Tensor, op_code: int, algo: int = codes.ALGO_AUTO) -> torch.Tensor:
     _plain(x)
     if x.is_cuda:
         return comm._native_comm().allreduce(x, op_code, algo)
-    done = _log(comm, "Allreduce", f"with {x.numel()} items")
-    out = _cpu.allreduce(comm, x, op_code)
-    if done:
-        done()
-    return out
+    return _on_cpu(comm, "Allreduce", f"with {x.numel()} items", _cpu.allreduce, x, op_code)
 
 
 def reduce(comm: Comm, x: torch.Tensor, op_code: int, root: int) -> Optional[torch.Tensor]:
     _plain(x)
     if x.is_cuda:
         return comm._native_comm().reduce(x, op_code, root)
-    done = _log(comm, "Reduce", f"with {x.numel()} items to root {root}")
-    out = _cpu.reduce(comm, x, op_code, root)
-    if done:
-        done()
-    return out
+    return _on_cpu(comm, "Reduce", f"with {x.numel()} items to root {root}", _cpu.reduce, x, op_code, root)
 
 
 def scan(comm: Comm, x: torch.Tensor, op_code: int) -> torch.Tensor:
     _plain(x)
     if x.is_cuda:
         return comm._native_comm().scan(x, op_code)
-    done = _log(comm, "Scan", f"with {x.numel()} items")
-    out = _cpu.scan(comm, x, op_code)
-    if done:
-        done()
-    return out
+    return _on_cpu(comm, "Scan", f"with {x.numel()} items", _cpu.scan, x, op_code)
 
 
 def reduce_scatter(comm: Comm, x: torch.Tensor, op_code: int) -> torch.Tensor:
     _plain(x)
     if x.is_cuda:
         return comm._native_comm().reduce_scatter(x, op_code)
-    done = _log(comm, "Reduce_scatter_block", f"with {x.numel() // x.shape[0]} items per block")
-    out = _cpu.reduce_scatter(comm, x, op_code)
-    if done:
-        done()
-    return out
+    return _on_cpu(comm, "Reduce_scatter_block", f"with {x.numel() // x.shape[0]} items per block",
+                   _cpu.reduce_scatter, x, op_code)
 
 
 def allgather(comm: Comm, x: torch.Tensor) -> torch.Tensor:
     _plain(x)
     if x.is_cuda:
         return comm._native_comm().allgather(x)
-    done = _log(comm, "Allgather", f"sending {x.numel() * x.element_size()} bytes")
-    out = _cpu.allgather(comm, x)
-    if done:
-        done()
-    return out
+    return _on_cpu(comm, "Allgather", f"sending {x.numel() * x.element_size()} bytes", _cpu.allgather, x)
 
 
 def alltoall(comm: Comm, x: torch.Tensor) -> torch.Tensor:
     _plain(x)
     if x.is_cuda:
         return comm._native_comm().alltoall(x)
-    done = _log(comm, "Alltoall", f"with {x.numel()} items")
-    out = _cpu.alltoall(comm, x)
-    if done:
-        done()
-    return out
+    return _on_cpu(comm, "Alltoall", f"with {x.numel()} items", _cpu.alltoall, x)
 
 
 def check_rows(opname: str, x: torch.Tensor) -> None:
@@ -184,27 +165,38 @@ def check_rowsv_args(opname: str, comm: Comm, x: torch.Tensor, counts: torch.Ten
 
 
 def rowsv_capacity(opname: str, comm: Comm, x: torch.Tensor, counts: torch.Tensor, recv_capacity,
-                   name: str):
+                   name: str, fan_in: int):
     """The output rows of a public variable-count call or its ``compiled`` twin, after the checks:
-    ``recv_capacity``, or by default the rows that never drop one -- ``N * nproc`` for the gathering ops,
-    ``N`` for reduce_scatterv (when every rank passes ``N`` rows) and scatterv."""
+    ``recv_capacity``, or by default ``fan_in * N``, the rows that never drop one -- ``fan_in`` is nproc for
+    the gathering ops, 1 for reduce_scatterv (when every rank passes ``N`` rows) and scatterv."""
     check_rows(opname, x)
-    if recv_capacity is not None:
-        out_rows = recv_capacity
-    else:
-        out_rows = x.shape[0] * (1 if opname in ("Reduce_scatterv", "Scatterv") else comm.Get_size())
+    out_rows = x.shape[0] * fan_in if recv_capacity is None else recv_capacity
     check_rowsv_args(opname, comm, x, counts, out_rows, name)
     return out_rows
 
 
-def _cpu_rowsv(opname: str, fn, comm: Comm, x: torch.Tensor, *args):
-    """``fn(comm, x, *args)``, the CPU backend's alltoallv / allgatherv / reduce_scatterv, with its log line."""
-    row_bytes = math.prod(x.shape[1:]) * x.element_size()
-    done = _log(comm, opname, f"with {x.shape[0]} rows of {row_bytes} bytes")
-    out = fn(comm, x, *args)
-    if done:
-        done()
-    return out
+def gatherv_capacity(comm: Comm, x: torch.Tensor, count: torch.Tensor, root: int, recv_capacity):
+    """gatherv's output rows after the checks: the capacity is read on the root only, the other ranks
+    receive nothing (0)."""
+    if comm.Get_rank() == root:
+        return rowsv_capacity("Gatherv", comm, x, count, recv_capacity, "count", comm.Get_size())
+    check_rowsv_args("Gatherv", comm, x, count, 0, "count")
+    return 0
+
+
+def scatterv_capacity(comm: Comm, x: torch.Tensor, send_counts: Optional[torch.Tensor], root: int,
+                      recv_capacity):
+    """scatterv's output rows after the checks: ``send_counts`` are required on the root and may be None
+    elsewhere; the capacity defaults to ``N`` and must be >= 0."""
+    if send_counts is not None:
+        return rowsv_capacity("Scatterv", comm, x, send_counts, recv_capacity, "send_counts", 1)
+    if comm.Get_rank() == root:
+        raise ValueError("Scatterv send_counts must be given on the root")
+    check_rows("Scatterv", x)
+    out_rows = x.shape[0] if recv_capacity is None else recv_capacity
+    if out_rows < 0:
+        raise ValueError(f"Scatterv recv_capacity must be >= 0 (got {out_rows})")
+    return out_rows
 
 
 def alltoallv(comm: Comm, x: torch.Tensor, send_counts: torch.Tensor, out_rows: int,
@@ -215,7 +207,7 @@ def alltoallv(comm: Comm, x: torch.Tensor, send_counts: torch.Tensor, out_rows: 
         check_rowsv_args("Alltoallv", comm, x, place_counts, out_rows, "place_counts")
     if x.is_cuda:
         return comm._native_comm().alltoallv(x, send_counts, out_rows, place_counts)
-    return _cpu_rowsv("Alltoallv", _cpu.alltoallv, comm, x, send_counts, out_rows, place_counts)
+    return _on_cpu(comm, "Alltoallv", _rows_text(x), _cpu.alltoallv, x, send_counts, out_rows, place_counts)
 
 
 def allgatherv(comm: Comm, x: torch.Tensor, count: torch.Tensor, out_rows: int,
@@ -226,7 +218,7 @@ def allgatherv(comm: Comm, x: torch.Tensor, count: torch.Tensor, out_rows: int,
         check_rowsv_args("Allgatherv", comm, x, place_counts, out_rows, "place_counts")
     if x.is_cuda:
         return comm._native_comm().allgatherv(x, count, out_rows, place_counts)
-    return _cpu_rowsv("Allgatherv", _cpu.allgatherv, comm, x, count, out_rows, place_counts)
+    return _on_cpu(comm, "Allgatherv", _rows_text(x), _cpu.allgatherv, x, count, out_rows, place_counts)
 
 
 def reduce_scatterv(comm: Comm, x: torch.Tensor, send_counts: torch.Tensor, out_rows: int, op_code: int):
@@ -234,17 +226,7 @@ def reduce_scatterv(comm: Comm, x: torch.Tensor, send_counts: torch.Tensor, out_
     check_rowsv_args("Reduce_scatterv", comm, x, send_counts, out_rows, "send_counts")
     if x.is_cuda:
         return comm._native_comm().reduce_scatterv(x, send_counts, out_rows, op_code)
-    return _cpu_rowsv("Reduce_scatterv", _cpu.reduce_scatterv, comm, x, send_counts, out_rows, op_code)
-
-
-def _cpu_rooted(opname: str, fn, comm: Comm, x: torch.Tensor, root: int, where: str, *args):
-    """``fn(comm, x, *args)``, the CPU backend's gatherv / scatterv, with its log line."""
-    row_bytes = math.prod(x.shape[1:]) * x.element_size()
-    done = _log(comm, opname, f"with {x.shape[0]} rows of {row_bytes} bytes {where} root {root}")
-    out = fn(comm, x, *args)
-    if done:
-        done()
-    return out
+    return _on_cpu(comm, "Reduce_scatterv", _rows_text(x), _cpu.reduce_scatterv, x, send_counts, out_rows, op_code)
 
 
 def gatherv(comm: Comm, x: torch.Tensor, count: torch.Tensor, root: int, out_rows: int, max_rows: int,
@@ -259,7 +241,8 @@ def gatherv(comm: Comm, x: torch.Tensor, count: torch.Tensor, root: int, out_row
         check_rowsv_args("Gatherv", comm, x, place_counts, out_rows, "place_counts")
     if x.is_cuda:
         return comm._native_comm().gatherv(x, count, root, out_rows, max_rows, place_counts)
-    return _cpu_rooted("Gatherv", _cpu.gatherv, comm, x, root, "to", count, root, out_rows, max_rows, place_counts)
+    return _on_cpu(comm, "Gatherv", f"{_rows_text(x)} to root {root}", _cpu.gatherv, x, count, root, out_rows,
+                   max_rows, place_counts)
 
 
 def scatterv(comm: Comm, x: torch.Tensor, send_counts: Optional[torch.Tensor], root: int, out_rows: int,
@@ -268,50 +251,32 @@ def scatterv(comm: Comm, x: torch.Tensor, send_counts: Optional[torch.Tensor], r
     the row shape and dtype, and ``send_counts`` may be None); ``max_rows``: the root rows that may be
     sent, the same on every rank (it sizes the staging)."""
     _plain(x)
-    if send_counts is not None:
-        check_rowsv_args("Scatterv", comm, x, send_counts, out_rows, "send_counts")
-    elif comm.Get_rank() == root:
-        raise ValueError("Scatterv send_counts must be given on the root")
-    else:
-        check_rows("Scatterv", x)
-        if out_rows < 0:
-            raise ValueError(f"Scatterv recv_capacity must be >= 0 (got {out_rows})")
+    scatterv_capacity(comm, x, send_counts, root, out_rows)
     if x.is_cuda:
         return comm._native_comm().scatterv(x, send_counts, root, out_rows, max_rows)
-    return _cpu_rooted("Scatterv", _cpu.scatterv, comm, x, root, "from", send_counts, root, out_rows, max_rows)
+    return _on_cpu(comm, "Scatterv", f"{_rows_text(x)} from root {root}", _cpu.scatterv, x, send_counts, root,
+                   out_rows, max_rows)
 
 
 def bcast(comm: Comm, x: torch.Tensor, root: int) -> torch.Tensor:
     _plain(x)
     if x.is_cuda:
         return comm._native_comm().bcast(x, root)
-    done = _log(comm, "Bcast", f"{x.numel()} items from root {root}")
-    out = _cpu.bcast(comm, x, root)
-    if done:
-        done()
-    return out
+    return _on_cpu(comm, "Bcast", f"{x.numel()} items from root {root}", _cpu.bcast, x, root)
 
 
 def gather(comm: Comm, x: torch.Tensor, root: int) -> Optional[torch.Tensor]:
     _plain(x)
     if x.is_cuda:
         return comm._native_comm().gather(x, root)
-    done = _log(comm, "Gather", f"{x.numel()} items to root {root}")
-    out = _cpu.gather(comm, x, root)
-    if done:
-        done()
-    return out
+    return _on_cpu(comm, "Gather", f"{x.numel()} items to root {root}", _cpu.gather, x, root)
 
 
 def scatter(comm: Comm, x: torch.Tensor, root: int, out_shape, dtype) -> torch.Tensor:
     _plain(x)
     if x.is_cuda:
         return comm._native_comm().scatter(x, root, out_shape, dtype)
-    done = _log(comm, "Scatter", f"from root {root}")
-    out = _cpu.scatter(comm, x, root, out_shape, dtype)
-    if done:
-        done()
-    return out
+    return _on_cpu(comm, "Scatter", f"from root {root}", _cpu.scatter, x, root, out_shape, dtype)
 
 
 def send(comm: Comm, x: torch.Tensor, dest: int, tag: int) -> None:
@@ -319,21 +284,15 @@ def send(comm: Comm, x: torch.Tensor, dest: int, tag: int) -> None:
     if x.is_cuda:
         comm._native_comm().send(x, dest, tag)
         return
-    done = _log(comm, "Send", f"{x.numel()} items to {dest} with tag {tag}")
-    _cpu.send(comm, x, dest, tag)
-    if done:
-        done()
+    _on_cpu(comm, "Send", f"{x.numel()} items to {dest} with tag {tag}", _cpu.send, x, dest, tag)
 
 
 def recv(comm: Comm, template: torch.Tensor, source: int, tag: int,
          status: Optional[Status]) -> torch.Tensor:
     if template.is_cuda:
         return comm._native_comm().recv(template, source, tag, status)
-    done = _log(comm, "Recv", f"{template.numel()} items from {source} with tag {tag}")
-    out = _cpu.recv(comm, template, source, tag, status)
-    if done:
-        done()
-    return out
+    return _on_cpu(comm, "Recv", f"{template.numel()} items from {source} with tag {tag}", _cpu.recv, template,
+                   source, tag, status)
 
 
 def sendrecv(comm: Comm, sendbuf: torch.Tensor, recv_template: torch.Tensor, source: int,
@@ -343,8 +302,5 @@ def sendrecv(comm: Comm, sendbuf: torch.Tensor, recv_template: torch.Tensor, sou
     if sendbuf.is_cuda:
         return comm._native_comm().sendrecv(sendbuf, recv_template, source, dest, sendtag,
                                             recvtag, status)
-    done = _log(comm, "Sendrecv", f"<{source} (tag {recvtag}) / >{dest} (tag {sendtag})")
-    out = _cpu.sendrecv(comm, sendbuf, recv_template, source, dest, sendtag, recvtag, status)
-    if done:
-        done()
-    return out
+    return _on_cpu(comm, "Sendrecv", f"<{source} (tag {recvtag}) / >{dest} (tag {sendtag})", _cpu.sendrecv,
+                   sendbuf, recv_template, source, dest, sendtag, recvtag, status)

@@ -32,49 +32,29 @@ import torch
 
 from .. import collective_ops
 from ..comm import Comm
-from ..utils import (NOTSET, as_tensor, check_dtype, get_default_comm, needs_autograd,
-                     raise_if_token_is_set)
+from ..utils import NOTSET, as_tensor, check_dtype, get_default_comm, raise_if_token_is_set
 from ..validation import enforce_types
 from . import _adjoints, _dispatch
+from ._rowsv import RowsvFunction
 
 
-class _Allgatherv(torch.autograd.Function):
+class _Allgatherv(RowsvFunction):
     """``place_counts`` None: the forward gather into ``out_rows`` packed rows.  Otherwise the reverse mode:
     ``place_counts`` are a reduce_scatterv's send counts and ``out_rows`` its input rows; the segment from
     rank q lands where that call took rank q's rows from."""
+
+    vmap_error = "allgatherv under vmap: the count must not be batched (one exchange moves every batch entry)"
 
     @staticmethod
     def forward(x, count, out_rows, place_counts, comm):
         return _dispatch.allgatherv(comm, x, count, out_rows, place_counts)
 
     @staticmethod
-    def setup_context(ctx, inputs, output):
-        x, ctx.count, ctx.out_rows, ctx.place_counts, ctx.comm = inputs
-        ctx.in_rows = x.shape[0]
-        ctx.mark_non_differentiable(output[1])
-        ctx.save_for_backward(output[1])
-
-    @staticmethod
     def backward(ctx, g, _g_counts):
+        _, _, place_counts, comm = ctx.args
         (recv_counts,) = ctx.saved_tensors
-        counts = recv_counts if ctx.place_counts is None else ctx.place_counts
-        return _adjoints.allgatherv(collective_ops.eager, g, ctx.comm, ctx.in_rows, counts), None, None, None, None
-
-    @staticmethod
-    def jvp(ctx, x_t, *_):
-        out_t, _counts = _Allgatherv.apply(x_t, ctx.count, ctx.out_rows, ctx.place_counts, ctx.comm)
-        return out_t, None
-
-    @staticmethod
-    def vmap(info, in_dims, x, count, out_rows, place_counts, comm):
-        if in_dims[1] is not None or in_dims[3] is not None:
-            raise ValueError("allgatherv under vmap: the count must not be batched (one exchange moves every "
-                             "batch entry)")
-        if in_dims[0] is None:
-            return _Allgatherv.apply(x, count, out_rows, place_counts, comm), (None, None)
-        # keep the row axis in front: (B, N, *S) -> (N, B, *S), gathered as one message of B-times larger rows
-        out, counts = _Allgatherv.apply(x.movedim(in_dims[0], 1).contiguous(), count, out_rows, place_counts, comm)
-        return (out, counts), (1, None)
+        counts = recv_counts if place_counts is None else place_counts
+        return _adjoints.allgatherv(collective_ops.eager, g, comm, ctx.in_rows, counts), None, None, None, None
 
 
 @enforce_types(recv_capacity=(type(None), np.integer), comm=(type(None), Comm))
@@ -102,10 +82,8 @@ def allgatherv(x, count, *, recv_capacity=None, comm=None, token=NOTSET):
     check_dtype(x)
     _dispatch.check_rows("Allgatherv", x)
     count = _dispatch.as_counts(count, x, scalar=True)
-    cap = int(_dispatch.rowsv_capacity("Allgatherv", comm, x, count, recv_capacity, "count"))
-    if not needs_autograd(x):
-        return _dispatch.allgatherv(comm, x, count, cap)
-    return _Allgatherv.apply(x, count, cap, None, comm)
+    cap = int(_dispatch.rowsv_capacity("Allgatherv", comm, x, count, recv_capacity, "count", comm.Get_size()))
+    return _Allgatherv.run(x, count, cap, None, comm)
 
 
 def allgatherv_reverse(y: torch.Tensor, place_counts: torch.Tensor, rows: int, comm: Comm) -> torch.Tensor:
@@ -116,6 +94,4 @@ def allgatherv_reverse(y: torch.Tensor, place_counts: torch.Tensor, rows: int, c
     place_counts = _dispatch.as_counts(place_counts, y)
     count = torch.full((), y.shape[0], dtype=torch.int64, device=y.device)
     _dispatch.check_rowsv_args("Allgatherv", comm, y, place_counts, rows, "place_counts")
-    if not needs_autograd(y):
-        return _dispatch.allgatherv(comm, y, count, rows, place_counts)[0]
-    return _Allgatherv.apply(y, count, rows, place_counts, comm)[0]
+    return _Allgatherv.run(y, count, rows, place_counts, comm)[0]

@@ -26,51 +26,29 @@ import torch
 
 from .. import collective_ops
 from ..comm import Comm
-from ..utils import (NOTSET, as_tensor, check_dtype, get_default_comm, needs_autograd,
-                     raise_if_token_is_set)
+from ..utils import NOTSET, as_tensor, check_dtype, get_default_comm, raise_if_token_is_set
 from ..validation import enforce_types
 from . import _adjoints, _dispatch
+from ._rowsv import RowsvFunction
 
 
-class _Alltoallv(torch.autograd.Function):
+class _Alltoallv(RowsvFunction):
     """``place_counts`` None: the forward exchange into ``out_rows`` packed rows.  Otherwise the reverse
     mode: ``send_counts`` are a forward's ``recv_counts``, ``place_counts`` its send counts and
     ``out_rows`` its input rows; each rank gets back the rows it sent, where it sent them from."""
+
+    vmap_error = "alltoallv under vmap: the counts must not be batched (one exchange moves every batch entry)"
 
     @staticmethod
     def forward(x, send_counts, out_rows, place_counts, comm):
         return _dispatch.alltoallv(comm, x, send_counts, out_rows, place_counts)
 
     @staticmethod
-    def setup_context(ctx, inputs, output):
-        x, ctx.send_counts, ctx.out_rows, ctx.place_counts, ctx.comm = inputs
-        ctx.in_rows = x.shape[0]
-        ctx.mark_non_differentiable(output[1])
-        ctx.save_for_backward(output[1])
-
-    @staticmethod
     def backward(ctx, g, _g_counts):
+        send_counts, _, place_counts, comm = ctx.args
         (recv_counts,) = ctx.saved_tensors
-        back = _adjoints.alltoallv(collective_ops.eager, g, ctx.comm, ctx.in_rows, ctx.send_counts, recv_counts,
-                                   ctx.place_counts)
+        back = _adjoints.alltoallv(collective_ops.eager, g, comm, ctx.in_rows, send_counts, recv_counts, place_counts)
         return back, None, None, None, None
-
-    @staticmethod
-    def jvp(ctx, x_t, *_):
-        out_t, _counts = _Alltoallv.apply(x_t, ctx.send_counts, ctx.out_rows, ctx.place_counts, ctx.comm)
-        return out_t, None
-
-    @staticmethod
-    def vmap(info, in_dims, x, send_counts, out_rows, place_counts, comm):
-        if in_dims[1] is not None or in_dims[3] is not None:
-            raise ValueError("alltoallv under vmap: the counts must not be batched (one exchange moves every "
-                             "batch entry)")
-        if in_dims[0] is None:
-            return _Alltoallv.apply(x, send_counts, out_rows, place_counts, comm), (None, None)
-        # keep the row axis in front: (B, N, *S) -> (N, B, *S), exchanged as one message of B-times larger rows
-        out, counts = _Alltoallv.apply(x.movedim(in_dims[0], 1).contiguous(), send_counts, out_rows,
-                                       place_counts, comm)
-        return (out, counts), (1, None)
 
 
 @enforce_types(recv_capacity=(type(None), np.integer), comm=(type(None), Comm))
@@ -100,10 +78,9 @@ def alltoallv(x, send_counts, *, recv_capacity=None, comm=None, token=NOTSET):
     check_dtype(x)
     _dispatch.check_rows("Alltoallv", x)
     send_counts = _dispatch.as_counts(send_counts, x)
-    cap = int(_dispatch.rowsv_capacity("Alltoallv", comm, x, send_counts, recv_capacity, "send_counts"))
-    if not needs_autograd(x):
-        return _dispatch.alltoallv(comm, x, send_counts, cap)
-    return _Alltoallv.apply(x, send_counts, cap, None, comm)
+    cap = int(_dispatch.rowsv_capacity("Alltoallv", comm, x, send_counts, recv_capacity, "send_counts",
+                                       comm.Get_size()))
+    return _Alltoallv.run(x, send_counts, cap, None, comm)
 
 
 def alltoallv_reverse(y: torch.Tensor, recv_counts: torch.Tensor, send_counts: torch.Tensor, rows: int,
@@ -115,6 +92,4 @@ def alltoallv_reverse(y: torch.Tensor, recv_counts: torch.Tensor, send_counts: t
     recv_counts, send_counts = _dispatch.as_counts(recv_counts, y), _dispatch.as_counts(send_counts, y)
     _dispatch.check_rowsv_args("Alltoallv", comm, y, recv_counts, rows, "recv_counts")
     _dispatch.check_rowsv_args("Alltoallv", comm, y, send_counts, rows, "send_counts")
-    if not needs_autograd(y):
-        return _dispatch.alltoallv(comm, y, recv_counts, rows, send_counts)[0]
-    return _Alltoallv.apply(y, recv_counts, rows, send_counts, comm)[0]
+    return _Alltoallv.run(y, recv_counts, rows, send_counts, comm)[0]

@@ -30,26 +30,29 @@ import torch
 
 from .. import collective_ops
 from ..comm import Comm
-from ..utils import (NOTSET, as_tensor, check_dtype, get_default_comm, needs_autograd,
-                     raise_if_token_is_set)
+from ..utils import NOTSET, as_tensor, check_dtype, get_default_comm, raise_if_token_is_set
 from ..validation import enforce_types
 from . import _adjoints, _dispatch
+from ._rowsv import RowsvFunction
 from .bcast import _check_root
 
 
 def _result(comm, x, out, root, out_rows, reverse):
-    """The root's output; elsewhere ``x`` (forward) or zeros of ``out_rows`` rows (reverse mode)."""
+    """The root's output; elsewhere ``x`` itself (forward; under autograd, ``apply`` returns a view of it) or
+    zeros of ``out_rows`` rows (reverse mode)."""
     if comm.Get_rank() == root:
         return out
-    return x.new_zeros((out_rows, *x.shape[1:])) if reverse else x.view_as(x)
+    return x.new_zeros((out_rows, *x.shape[1:])) if reverse else x
 
 
-class _Gatherv(torch.autograd.Function):
+class _Gatherv(RowsvFunction):
     """``reverse`` False: the forward gather into the root's ``out_rows`` packed rows.  Otherwise the reverse
     mode, the adjoint of a scatterv whose send counts were ``place_counts`` and whose input had
     ``out_rows`` rows on this rank: on the root the segment from rank q lands where that call took rank
     q's rows from; the other ranks get zeros.  ``max_rows``: the rows any rank may contribute, the same on
     every rank."""
+
+    vmap_error = "gatherv under vmap: the count must not be batched (one exchange moves every batch entry)"
 
     @staticmethod
     def forward(x, count, root, out_rows, max_rows, place_counts, reverse, comm):
@@ -57,39 +60,15 @@ class _Gatherv(torch.autograd.Function):
         return _result(comm, x, out, root, out_rows, reverse), recv_counts
 
     @staticmethod
-    def setup_context(ctx, inputs, output):
-        x, ctx.count, ctx.root, ctx.out_rows, ctx.max_rows, ctx.place_counts, ctx.reverse, ctx.comm = inputs
-        ctx.in_rows = x.shape[0]
-        ctx.mark_non_differentiable(output[1])
-        ctx.save_for_backward(output[1])
-
-    @staticmethod
     def backward(ctx, g, _g_counts):
-        F, comm = collective_ops.eager, ctx.comm
-        if ctx.reverse:
-            back = _adjoints.gatherv_reverse(F, g, comm, ctx.root, ctx.in_rows, ctx.max_rows, ctx.place_counts)
+        _, root, _, max_rows, place_counts, reverse, comm = ctx.args
+        F = collective_ops.eager
+        if reverse:
+            back = _adjoints.gatherv_reverse(F, g, comm, root, ctx.in_rows, max_rows, place_counts)
         else:
             (recv_counts,) = ctx.saved_tensors
-            back = _adjoints.gatherv(F, g, comm, ctx.root, ctx.in_rows, ctx.max_rows, recv_counts)
+            back = _adjoints.gatherv(F, g, comm, root, ctx.in_rows, max_rows, recv_counts)
         return back, None, None, None, None, None, None, None
-
-    @staticmethod
-    def jvp(ctx, x_t, *_):
-        out_t, _counts = _Gatherv.apply(x_t, ctx.count, ctx.root, ctx.out_rows, ctx.max_rows, ctx.place_counts,
-                                        ctx.reverse, ctx.comm)
-        return out_t, None
-
-    @staticmethod
-    def vmap(info, in_dims, x, count, root, out_rows, max_rows, place_counts, reverse, comm):
-        if in_dims[1] is not None or in_dims[5] is not None:
-            raise ValueError("gatherv under vmap: the count must not be batched (one exchange moves every "
-                             "batch entry)")
-        if in_dims[0] is None:
-            return _Gatherv.apply(x, count, root, out_rows, max_rows, place_counts, reverse, comm), (None, None)
-        # keep the row axis in front: (B, N, *S) -> (N, B, *S), gathered as one message of B-times larger rows
-        x = x.movedim(in_dims[0], 1).contiguous()
-        out, counts = _Gatherv.apply(x, count, root, out_rows, max_rows, place_counts, reverse, comm)
-        return (out, counts), (1, None)
 
 
 @enforce_types(root=(np.integer,), recv_capacity=(type(None), np.integer), comm=(type(None), Comm))
@@ -120,15 +99,8 @@ def gatherv(x, count, root, *, recv_capacity=None, comm=None, token=NOTSET):
     root = int(root)
     _dispatch.check_rows("Gatherv", x)
     count = _dispatch.as_counts(count, x, scalar=True)
-    if comm.Get_rank() == root:
-        cap = int(_dispatch.rowsv_capacity("Gatherv", comm, x, count, recv_capacity, "count"))
-    else:
-        cap = 0
-        _dispatch.check_rowsv_args("Gatherv", comm, x, count, cap, "count")
-    if not needs_autograd(x):
-        out, recv_counts = _dispatch.gatherv(comm, x, count, root, cap, x.shape[0])
-        return (out if comm.Get_rank() == root else x), recv_counts
-    return _Gatherv.apply(x, count, root, cap, x.shape[0], None, False, comm)
+    cap = int(_dispatch.gatherv_capacity(comm, x, count, root, recv_capacity))
+    return _Gatherv.run(x, count, root, cap, x.shape[0], None, False, comm)
 
 
 def gatherv_reverse(y: torch.Tensor, count: torch.Tensor, place_counts, root: int, rows: int, max_rows: int,
@@ -140,7 +112,4 @@ def gatherv_reverse(y: torch.Tensor, count: torch.Tensor, place_counts, root: in
     if comm.Get_rank() == root:
         place_counts = _dispatch.as_counts(place_counts, y)
         _dispatch.check_rowsv_args("Gatherv", comm, y, place_counts, rows, "place_counts")
-    if not needs_autograd(y):
-        out, _ = _dispatch.gatherv(comm, y, count, root, rows, max_rows, place_counts)
-        return _result(comm, y, out, root, rows, True)
-    return _Gatherv.apply(y, count, root, rows, max_rows, place_counts, True, comm)[0]
+    return _Gatherv.run(y, count, root, rows, max_rows, place_counts, True, comm)[0]

@@ -35,6 +35,7 @@ from ..utils import (NOTSET, as_tensor, check_dtype, get_default_comm, needs_aut
                      raise_if_token_is_set)
 from ..validation import enforce_types
 from . import _adjoints, _dispatch
+from ._rowsv import RowsvFunction
 
 
 def _require_sum(op: Op, what: str) -> None:
@@ -42,39 +43,24 @@ def _require_sum(op: Op, what: str) -> None:
         raise NotImplementedError(f"The {what} of reduce_scatterv for {op.name} is not defined")
 
 
-class _ReduceScatterv(torch.autograd.Function):
+class _ReduceScatterv(RowsvFunction):
+    vmap_error = "reduce_scatterv under vmap: the counts must not be batched (one exchange moves every batch entry)"
+
     @staticmethod
     def forward(x, send_counts, out_rows, op, comm):
         return _dispatch.reduce_scatterv(comm, x, send_counts, out_rows, op.code)
 
     @staticmethod
-    def setup_context(ctx, inputs, output):
-        x, ctx.send_counts, ctx.out_rows, ctx.op, ctx.comm = inputs
-        ctx.in_rows = x.shape[0]
-        ctx.mark_non_differentiable(output[1])
-
-    @staticmethod
     def backward(ctx, g, _g_counts):
-        _require_sum(ctx.op, "adjoint")
-        back = _adjoints.reduce_scatterv(collective_ops.eager, g, ctx.comm, ctx.in_rows, ctx.send_counts)
+        send_counts, _, op, comm = ctx.args
+        _require_sum(op, "adjoint")
+        back = _adjoints.reduce_scatterv(collective_ops.eager, g, comm, ctx.in_rows, send_counts)
         return back, None, None, None, None
 
-    @staticmethod
-    def jvp(ctx, x_t, *_):
-        _require_sum(ctx.op, "derivative")
-        out_t, _counts = _ReduceScatterv.apply(x_t, ctx.send_counts, ctx.out_rows, ctx.op, ctx.comm)
-        return out_t, None
-
-    @staticmethod
-    def vmap(info, in_dims, x, send_counts, out_rows, op, comm):
-        if in_dims[1] is not None:
-            raise ValueError("reduce_scatterv under vmap: the counts must not be batched (one exchange moves "
-                             "every batch entry)")
-        if in_dims[0] is None:
-            return _ReduceScatterv.apply(x, send_counts, out_rows, op, comm), (None, None)
-        # keep the row axis in front: (B, M, *S) -> (M, B, *S), reduced as one message of B-times larger rows
-        out, counts = _ReduceScatterv.apply(x.movedim(in_dims[0], 1).contiguous(), send_counts, out_rows, op, comm)
-        return (out, counts), (1, None)
+    @classmethod
+    def jvp(cls, ctx, x_t, *_):
+        _require_sum(ctx.args[2], "derivative")
+        return super().jvp(ctx, x_t)
 
 
 def _user_op(comm: Comm, x: torch.Tensor, send_counts: torch.Tensor, out_rows: int, op: Op):
@@ -135,11 +121,9 @@ def reduce_scatterv(x, send_counts, op, *, recv_capacity=None, comm=None, token=
     check_dtype(x)
     _dispatch.check_rows("Reduce_scatterv", x)
     send_counts = _dispatch.as_counts(send_counts, x)
-    cap = int(_dispatch.rowsv_capacity("Reduce_scatterv", comm, x, send_counts, recv_capacity, "send_counts"))
+    cap = int(_dispatch.rowsv_capacity("Reduce_scatterv", comm, x, send_counts, recv_capacity, "send_counts", 1))
     if op.code is None:
         if needs_autograd(x):
             raise NotImplementedError(f"The derivative of reduce_scatterv for {op.name} is not defined")
         return _user_op(comm, x.contiguous(), send_counts, cap, op)
-    if not needs_autograd(x):
-        return _dispatch.reduce_scatterv(comm, x, send_counts, cap, op.code)
-    return _ReduceScatterv.apply(x, send_counts, cap, op, comm)
+    return _ReduceScatterv.run(x, send_counts, cap, op, comm)

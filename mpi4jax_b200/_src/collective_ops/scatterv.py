@@ -30,50 +30,28 @@ import torch
 
 from .. import collective_ops
 from ..comm import Comm
-from ..utils import (NOTSET, as_tensor, check_dtype, get_default_comm, needs_autograd,
-                     raise_if_token_is_set)
+from ..utils import NOTSET, as_tensor, check_dtype, get_default_comm, raise_if_token_is_set
 from ..validation import enforce_types
 from . import _adjoints, _dispatch
+from ._rowsv import RowsvFunction
 from .bcast import _check_root
 
 
-class _Scatterv(torch.autograd.Function):
+class _Scatterv(RowsvFunction):
     """``max_rows``: the root rows that may be sent, the same on every rank (it sizes the staging)."""
+
+    vmap_error = "scatterv under vmap: the counts must not be batched (one exchange moves every batch entry)"
 
     @staticmethod
     def forward(x, send_counts, root, out_rows, max_rows, comm):
         return _dispatch.scatterv(comm, x, send_counts, root, out_rows, max_rows)
 
     @staticmethod
-    def setup_context(ctx, inputs, output):
-        x, ctx.send_counts, ctx.root, ctx.out_rows, ctx.max_rows, ctx.comm = inputs
-        ctx.in_rows = x.shape[0]
-        ctx.mark_non_differentiable(output[1])
-        ctx.save_for_backward(output[1])
-
-    @staticmethod
     def backward(ctx, g, _g_count):
+        send_counts, root, _, max_rows, comm = ctx.args
         (recv_count,) = ctx.saved_tensors
-        back = _adjoints.scatterv(collective_ops.eager, g, ctx.comm, ctx.root, ctx.in_rows, ctx.max_rows,
-                                  recv_count, ctx.send_counts)
+        back = _adjoints.scatterv(collective_ops.eager, g, comm, root, ctx.in_rows, max_rows, recv_count, send_counts)
         return back, None, None, None, None, None
-
-    @staticmethod
-    def jvp(ctx, x_t, *_):
-        out_t, _count = _Scatterv.apply(x_t, ctx.send_counts, ctx.root, ctx.out_rows, ctx.max_rows, ctx.comm)
-        return out_t, None
-
-    @staticmethod
-    def vmap(info, in_dims, x, send_counts, root, out_rows, max_rows, comm):
-        if in_dims[1] is not None:
-            raise ValueError("scatterv under vmap: the counts must not be batched (one exchange moves every "
-                             "batch entry)")
-        if in_dims[0] is None:
-            return _Scatterv.apply(x, send_counts, root, out_rows, max_rows, comm), (None, None)
-        # keep the row axis in front: (B, N, *S) -> (N, B, *S), scattered as one message of B-times larger rows
-        x = x.movedim(in_dims[0], 1).contiguous()
-        out, count = _Scatterv.apply(x, send_counts, root, out_rows, max_rows, comm)
-        return (out, count), (1, None)
 
 
 @enforce_types(root=(np.integer,), recv_capacity=(type(None), np.integer), comm=(type(None), Comm))
@@ -106,16 +84,8 @@ def scatterv(x, send_counts, root, *, recv_capacity=None, comm=None, token=NOTSE
     _dispatch.check_rows("Scatterv", x)
     if send_counts is not None:
         send_counts = _dispatch.as_counts(send_counts, x)
-        cap = int(_dispatch.rowsv_capacity("Scatterv", comm, x, send_counts, recv_capacity, "send_counts"))
-    elif comm.Get_rank() == root:
-        raise ValueError("Scatterv send_counts must be given on the root")
-    else:
-        cap = x.shape[0] if recv_capacity is None else int(recv_capacity)
-        if cap < 0:
-            raise ValueError(f"Scatterv recv_capacity must be >= 0 (got {cap})")
-    if not needs_autograd(x):
-        return _dispatch.scatterv(comm, x, send_counts, root, cap, x.shape[0])
-    return _Scatterv.apply(x, send_counts, root, cap, x.shape[0], comm)
+    cap = int(_dispatch.scatterv_capacity(comm, x, send_counts, root, recv_capacity))
+    return _Scatterv.run(x, send_counts, root, cap, x.shape[0], comm)
 
 
 def scatterv_bounded(x: torch.Tensor, send_counts, root: int, rows: int, max_rows: int, comm: Comm) -> torch.Tensor:
@@ -124,6 +94,4 @@ def scatterv_bounded(x: torch.Tensor, send_counts, root: int, rows: int, max_row
     gatherv's reverse mode)."""
     if comm.Get_rank() == root:
         send_counts = _dispatch.as_counts(send_counts, x)
-    if not needs_autograd(x):
-        return _dispatch.scatterv(comm, x, send_counts, root, rows, max_rows)[0]
-    return _Scatterv.apply(x, send_counts, root, rows, max_rows, comm)[0]
+    return _Scatterv.run(x, send_counts, root, rows, max_rows, comm)[0]

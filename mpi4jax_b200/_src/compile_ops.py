@@ -59,6 +59,19 @@ def _st(status_id: int):
     return st
 
 
+def _rowsv_fake(opname: str, comm: Comm, x, counts, name: str, out_rows: int, place_counts=None,
+                counts_shape=None):
+    """A variable-count op's fake kernel: the backends' checks of ``counts`` and ``place_counts`` (each when
+    given) against ``out_rows``, then ``(out, out_counts)``: ``out_rows`` rows like ``x`` and int64 counts of
+    ``counts_shape`` (default ``(nproc,)``)."""
+    if counts is not None:
+        _dispatch.check_rowsv_args(opname, comm, x, counts, out_rows, name)
+    if place_counts is not None:
+        _dispatch.check_rowsv_args(opname, comm, x, place_counts, out_rows, "place_counts")
+    counts_shape = (comm.Get_size(),) if counts_shape is None else counts_shape
+    return x.new_empty((out_rows, *x.shape[1:])), x.new_empty(counts_shape, dtype=torch.int64)
+
+
 # ---------------------------------------------------------------- op definitions
 @custom_op("mpi4jax_b200::allreduce", mutates_args=())
 def _allreduce(x: torch.Tensor, op: int, comm_id: int) -> torch.Tensor:
@@ -156,9 +169,7 @@ def _alltoallv(x: torch.Tensor, send_counts: torch.Tensor, out_rows: int, place_
 
 @_alltoallv.register_fake
 def _(x, send_counts, out_rows, place_counts, comm_id):
-    comm = _c(comm_id)
-    _dispatch.check_rowsv_args("Alltoallv", comm, x, send_counts, out_rows, "send_counts")
-    return x.new_empty((out_rows, *x.shape[1:])), x.new_empty((comm.Get_size(),), dtype=torch.int64)
+    return _rowsv_fake("Alltoallv", _c(comm_id), x, send_counts, "send_counts", out_rows)
 
 
 def _alltoallv_setup(ctx, inputs, output):
@@ -184,11 +195,7 @@ def _allgatherv(x: torch.Tensor, count: torch.Tensor, out_rows: int, comm_id: in
 
 @_allgatherv.register_fake
 def _(x, count, out_rows, comm_id, place_counts=None):
-    comm = _c(comm_id)
-    _dispatch.check_rowsv_args("Allgatherv", comm, x, count, out_rows, "count")
-    if place_counts is not None:
-        _dispatch.check_rowsv_args("Allgatherv", comm, x, place_counts, out_rows, "place_counts")
-    return x.new_empty((out_rows, *x.shape[1:])), x.new_empty((comm.Get_size(),), dtype=torch.int64)
+    return _rowsv_fake("Allgatherv", _c(comm_id), x, count, "count", out_rows, place_counts)
 
 
 def _allgatherv_setup(ctx, inputs, output):
@@ -214,9 +221,7 @@ def _reduce_scatterv(x: torch.Tensor, send_counts: torch.Tensor, out_rows: int, 
 
 @_reduce_scatterv.register_fake
 def _(x, send_counts, out_rows, op, comm_id):
-    comm = _c(comm_id)
-    _dispatch.check_rowsv_args("Reduce_scatterv", comm, x, send_counts, out_rows, "send_counts")
-    return x.new_empty((out_rows, *x.shape[1:])), x.new_empty((comm.Get_size(),), dtype=torch.int64)
+    return _rowsv_fake("Reduce_scatterv", _c(comm_id), x, send_counts, "send_counts", out_rows)
 
 
 def _reduce_scatterv_setup(ctx, inputs, output):
@@ -311,11 +316,7 @@ def _gatherv_root(x: torch.Tensor, count: torch.Tensor, root: int, out_rows: int
 
 @_gatherv_root.register_fake
 def _(x, count, root, out_rows, max_rows, comm_id, reverse, place_counts=None):
-    comm = _c(comm_id)
-    _dispatch.check_rowsv_args("Gatherv", comm, x, count, out_rows, "count")
-    if place_counts is not None:
-        _dispatch.check_rowsv_args("Gatherv", comm, x, place_counts, out_rows, "place_counts")
-    return x.new_empty((out_rows, *x.shape[1:])), x.new_empty((comm.Get_size(),), dtype=torch.int64)
+    return _rowsv_fake("Gatherv", _c(comm_id), x, count, "count", out_rows, place_counts)
 
 
 def _gatherv_root_setup(ctx, inputs, output):
@@ -346,10 +347,8 @@ def _gatherv_leaf(x: torch.Tensor, count: torch.Tensor, root: int, max_rows: int
 
 @_gatherv_leaf.register_fake
 def _(x, count, root, max_rows, comm_id):
-    comm = _c(comm_id)
-    _dispatch.check_rowsv_args("Gatherv", comm, x, count, 0, "count")
-    return torch.empty_like(x, memory_format=torch.contiguous_format), x.new_empty((comm.Get_size(),),
-                                                                                    dtype=torch.int64)
+    _, recv_counts = _rowsv_fake("Gatherv", _c(comm_id), x, count, "count", 0)
+    return torch.empty_like(x, memory_format=torch.contiguous_format), recv_counts
 
 
 def _gatherv_leaf_setup(ctx, inputs, output):
@@ -374,11 +373,8 @@ def _scatterv(x: torch.Tensor, send_counts: Optional[torch.Tensor], root: int, o
 @_scatterv.register_fake
 def _(x, send_counts, root, out_rows, max_rows, comm_id):
     comm = _c(comm_id)
-    if send_counts is not None:
-        _dispatch.check_rowsv_args("Scatterv", comm, x, send_counts, out_rows, "send_counts")
-    elif comm.Get_rank() == root:
-        raise ValueError("Scatterv send_counts must be given on the root")
-    return x.new_empty((out_rows, *x.shape[1:])), x.new_empty((), dtype=torch.int64)
+    _dispatch.scatterv_capacity(comm, x, send_counts, root, out_rows)
+    return _rowsv_fake("Scatterv", comm, x, send_counts, "send_counts", out_rows, counts_shape=())
 
 
 def _scatterv_setup(ctx, inputs, output):
@@ -509,7 +505,8 @@ class compiled:
         """``(out, recv_counts)`` of :func:`mpi4jax_b200.alltoallv`; ``send_counts`` must be a device
         tensor of shape ``(nproc,)``."""
         comm = comm or get_default_comm()
-        cap = _dispatch.rowsv_capacity("Alltoallv", comm, x, send_counts, recv_capacity, "send_counts")
+        cap = _dispatch.rowsv_capacity("Alltoallv", comm, x, send_counts, recv_capacity, "send_counts",
+                                       comm.Get_size())
         return torch.ops.mpi4jax_b200.alltoallv(x, send_counts, cap, None, comm._id)
 
     @staticmethod
@@ -522,7 +519,7 @@ class compiled:
         """``(out, recv_counts)`` of :func:`mpi4jax_b200.allgatherv`; ``count`` must be an integer device
         tensor of shape ``()``."""
         comm = comm or get_default_comm()
-        cap = _dispatch.rowsv_capacity("Allgatherv", comm, x, count, recv_capacity, "count")
+        cap = _dispatch.rowsv_capacity("Allgatherv", comm, x, count, recv_capacity, "count", comm.Get_size())
         return torch.ops.mpi4jax_b200.allgatherv(x, count, cap, comm._id)
 
     @staticmethod
@@ -536,7 +533,7 @@ class compiled:
         """``(out, recv_counts)`` of :func:`mpi4jax_b200.reduce_scatterv` for the built-in operators;
         ``send_counts`` must be a device tensor of shape ``(nproc,)``."""
         comm = comm or get_default_comm()
-        cap = _dispatch.rowsv_capacity("Reduce_scatterv", comm, x, send_counts, recv_capacity, "send_counts")
+        cap = _dispatch.rowsv_capacity("Reduce_scatterv", comm, x, send_counts, recv_capacity, "send_counts", 1)
         return torch.ops.mpi4jax_b200.reduce_scatterv(x, send_counts, cap, as_op(op).code, comm._id)
 
     @staticmethod
@@ -545,8 +542,8 @@ class compiled:
         of shape ``()``.  On the root the ``gatherv_root`` op, elsewhere ``gatherv_leaf``, whose result is a
         copy of ``x``."""
         comm = comm or get_default_comm()
+        cap = _dispatch.gatherv_capacity(comm, x, count, root, recv_capacity)
         if comm.Get_rank() == root:
-            cap = _dispatch.rowsv_capacity("Gatherv", comm, x, count, recv_capacity, "count")
             return torch.ops.mpi4jax_b200.gatherv_root(x, count, int(root), cap, x.shape[0], comm._id, False)
         return torch.ops.mpi4jax_b200.gatherv_leaf(x, count, int(root), x.shape[0], comm._id)
 
@@ -562,11 +559,8 @@ class compiled:
         """``(out, recv_count)`` of :func:`mpi4jax_b200.scatterv`; ``send_counts`` must be a device tensor of
         shape ``(nproc,)`` on the root (None or such a tensor elsewhere)."""
         comm = comm or get_default_comm()
-        if send_counts is None:
-            cap = x.shape[0] if recv_capacity is None else recv_capacity
-            _dispatch.check_rows("Scatterv", x)
-        else:
-            cap = _dispatch.rowsv_capacity("Scatterv", comm, x, send_counts, recv_capacity, "send_counts")
+        _dispatch.check_rows("Scatterv", x)
+        cap = _dispatch.scatterv_capacity(comm, x, send_counts, root, recv_capacity)
         return torch.ops.mpi4jax_b200.scatterv(x, send_counts, int(root), cap, x.shape[0], comm._id)
 
     @staticmethod
