@@ -18,6 +18,7 @@
 #include <cstring>
 
 #include "b2_reduce.cuh"
+#include "b2_reduce_loc.cuh"
 #include "b2_runtime.h"
 
 b2_reduce_launch_fn b2_reduce_table[B2_DTYPE_COUNT][B2_OP_COUNT];
@@ -32,6 +33,7 @@ static void b2_ensure_tables() {
   b2_register_reduce_group_1();
   b2_register_reduce_group_2();
   b2_register_reduce_group_3();
+  b2_register_reduce_loc();
   done = true;
 }
 
@@ -768,11 +770,12 @@ static int check_root(const B2Comm* c, int root, const char* name) {
   return B2_ERR_BAD_ARG;
 }
 
-// `table`: a typed launcher table of b2_reduce.cuh, nullptr where the dtype/op combination is invalid
-template <typename Fn>
-static int check_dtype_op(Fn (&table)[B2_DTYPE_COUNT][B2_OP_COUNT], int dtype, int op, const char* name) {
+// `table`: a typed launcher table of b2_reduce.cuh or b2_reduce_loc.cuh, nullptr where the dtype/op combination
+// is invalid; `op` indexes its columns
+template <typename Fn, int NOP>
+static int check_dtype_op(Fn (&table)[B2_DTYPE_COUNT][NOP], int dtype, int op, const char* name) {
   b2_ensure_tables();
-  if (dtype >= 0 && dtype < B2_DTYPE_COUNT && op >= 0 && op < B2_OP_COUNT && table[dtype][op] != nullptr) return 0;
+  if (dtype >= 0 && dtype < B2_DTYPE_COUNT && op >= 0 && op < NOP && table[dtype][op] != nullptr) return 0;
   b2_set_error("%s: unsupported dtype/op combination (dtype=%d, op=%d)", name, dtype, op);
   return B2_ERR_BAD_ARG;
 }
@@ -1219,6 +1222,52 @@ extern "C" int b2_reduce_scatterv(B2Comm* c, const void* in, void* out, size_t r
     if (rc == 0) {
       b2_rsv_table[dtype][op](c->dev, a, grid, stream);
       rc = b2_launched(c, "reduce_scatterv");
+    }
+  }
+  b2_debug_end(dbg, rc);
+  return rc;
+}
+
+// MAXLOC / MINLOC over (value, index) pairs (b2_reduce_loc.cu): `opcode` selects the collective -- the source
+// ranks, which ranks store a result and, for reduce-scatter, P blocks of `count` pairs per rank.  One
+// transport: stage the records, barrier, pull and fold (no LL, two-shot or in-switch path).
+extern "C" int b2_reduce_loc(B2Comm* c, const void* in_val, const void* in_idx, void* out_val, void* out_idx,
+                             size_t count, int val_dtype, int idx_bytes, int op, int opcode, int root,
+                             cudaStream_t stream) {
+  const bool rs = opcode == B2_OPC_REDUCE_SCATTER, red = opcode == B2_OPC_REDUCE, scan = opcode == B2_OPC_SCAN;
+  const char* opname = red ? "Reduce" : scan ? "Scan" : rs ? "Reduce_scatter_block" : "Allreduce";
+  const char* name = red ? "reduce" : scan ? "scan" : rs ? "reduce_scatter" : "allreduce";
+  B2DebugScope* dbg = red ? b2_debug_begin(c, opname, stream, "with %zu pairs to root %d via oneshot", count, root)
+                          : b2_debug_begin(c, opname, stream, "with %zu pairs%s via oneshot", count,
+                                           rs ? " per block" : "");
+  int rc = 0;
+  if (!(rs || red || scan || opcode == B2_OPC_ALLREDUCE)) {
+    b2_set_error("reduce_loc: opcode %d is not a reduction collective", opcode);
+    rc = B2_ERR_BAD_ARG;
+  } else if (op != B2_MAXLOC && op != B2_MINLOC) {
+    b2_set_error("%s: op %d is not MAXLOC or MINLOC", name, op);
+    rc = B2_ERR_BAD_ARG;
+  } else if (idx_bytes != 4 && idx_bytes != 8) {
+    b2_set_error("%s: indices must be int32 or int64 (got %d bytes)", name, idx_bytes);
+    rc = B2_ERR_BAD_ARG;
+  } else {
+    rc = check_dtype_op(b2_loc_table, val_dtype, op - B2_MAXLOC, name);
+  }
+  if (rc == 0 && red) rc = check_root(c, root, name);
+  if (rc == 0 && count > 0) {
+    B2LocArgs a;
+    a.in_val = in_val; a.in_idx = in_idx; a.out_val = out_val; a.out_idx = out_idx;
+    a.count = count; a.idx_bytes = idx_bytes; a.opcode = opcode;
+    a.src_lo = 0;
+    a.src_hi = scan ? c->dev.rank + 1 : c->dev.size;
+    a.has_out = red ? c->dev.rank == root : 1;
+    a.nblk = rs ? c->dev.size : 1;
+    int grid;
+    rc = plan_staged(c, opcode, count * B2_LOC_RECORD, b2_loc_kernel[val_dtype][op - B2_MAXLOC], name, &a.chunk,
+                     &grid);
+    if (rc == 0) {
+      b2_loc_table[val_dtype][op - B2_MAXLOC](c->dev, a, grid, stream);
+      rc = b2_launched(c, name);
     }
   }
   b2_debug_end(dbg, rc);

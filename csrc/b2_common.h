@@ -16,7 +16,7 @@
 #include <cstddef>
 #include <cstdint>
 
-#define B2_ABI_VERSION 17  // bump whenever a struct shared with Python or a C signature changes
+#define B2_ABI_VERSION 18  // bump whenever a struct shared with Python or a C signature changes
 #define B2_MAX_RANKS 16          // ranks per NVLink domain we support (8 on HGX H100)
 // bytes of the count header in front of the rows the variable-count collectives stage: one int64
 // per possible rank (keeps the rows 16-byte aligned)
@@ -40,7 +40,9 @@ enum B2Op : int {
   B2_SUM = 0, B2_PROD = 1, B2_MIN = 2, B2_MAX = 3,
   B2_LAND = 4, B2_LOR = 5, B2_LXOR = 6,
   B2_BAND = 7, B2_BOR = 8, B2_BXOR = 9,
-  B2_OP_COUNT = 10
+  B2_OP_COUNT = 10,
+  // value-index reductions (b2_reduce_loc.cu): outside B2_OP_COUNT, so the [dtype][op] tables keep their size
+  B2_MAXLOC = 10, B2_MINLOC = 11
 };
 
 // allreduce algorithm selector (B2_ALGO_AUTO = measured size table)

@@ -191,6 +191,13 @@ int b2_scatterv(B2Comm* c, const void* in, void* out, size_t row_bytes, size_t i
 int b2_reduce_scatterv(B2Comm* c, const void* in, void* out, size_t row_bytes, size_t in_rows, size_t out_rows,
                        const long long* send_counts, long long* recv_counts, int dtype, int op,
                        cudaStream_t stream);
+// MAXLOC / MINLOC (op) of (value, index) pairs for the reduction collective `opcode` (B2_OPC_ALLREDUCE,
+// _REDUCE, _SCAN or _REDUCE_SCATTER).  `in_val`: count pairs' values of dtype val_dtype (f32, f64, f16, bf16,
+// i16, i32 or i64), `in_idx`: their indices, idx_bytes 4 (int32) or 8 (int64); reduce-scatter: nranks blocks of
+// count pairs each.  `out_val` / `out_idx` (count pairs, the same dtypes) receive the winning pair, which is
+// always one of the inputs; reduce writes them on `root` only.  Pairs fold in rank order (see b2_reduce_loc.cu).
+int b2_reduce_loc(B2Comm* c, const void* in_val, const void* in_idx, void* out_val, void* out_idx, size_t count,
+                  int val_dtype, int idx_bytes, int op, int opcode, int root, cudaStream_t stream);
 
 // --- point to point ----------------------------------------------------------
 // source/tag may be -1 (ANY).  `status` is a host-mapped B2StatusRecord or null.

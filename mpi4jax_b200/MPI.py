@@ -20,7 +20,9 @@ from ._src.comm import (  # noqa: F401
     LOR,
     LXOR,
     MAX,
+    MAXLOC,
     MIN,
+    MINLOC,
     PROC_NULL,
     PROD,
     SUM,

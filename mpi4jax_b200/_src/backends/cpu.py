@@ -161,6 +161,23 @@ def reduce_scatter(comm: Comm, x: torch.Tensor, op_code: int) -> torch.Tensor:
     return reduce_stack(_gather_stack(comm, x)[:, comm.rank], op_code)
 
 
+def reduce_loc(comm: Comm, opcode: int, values: torch.Tensor, indices: torch.Tensor, op_code: int, root: int):
+    """MAXLOC / MINLOC: everybody gathers both tensors and folds the pairs of its source ranks in rank order
+    through ``Op.__call__`` (correctness path).  None off the root of a reduce."""
+    from ..comm import MAXLOC, MINLOC
+
+    op = MAXLOC if op_code == codes.MAXLOC else MINLOC
+    vals, idxs = _gather_stack(comm, values), _gather_stack(comm, indices)
+    if opcode == codes.OPC_REDUCE_SCATTER:
+        vals, idxs = vals[:, comm.rank], idxs[:, comm.rank]
+    if opcode == codes.OPC_REDUCE and comm.rank != root:
+        return None
+    acc = (vals[0], idxs[0])
+    for q in range(1, comm.rank + 1 if opcode == codes.OPC_SCAN else comm.size):
+        acc = op(acc, (vals[q], idxs[q]))
+    return acc[0].clone(), acc[1].clone()
+
+
 def allgather(comm: Comm, x: torch.Tensor) -> torch.Tensor:
     return _gather_stack(comm, x)
 

@@ -501,6 +501,24 @@ class NativeComm:
         self._check(rc, "Reduce_scatter_block")
         return out
 
+    def reduce_loc(self, opcode: int, values: torch.Tensor, indices: torch.Tensor, op_code: int, root: int):
+        """MAXLOC / MINLOC of ``(values, indices)`` pairs for the reduction collective ``opcode``
+        (``collective_ops/_loc.py`` states the rule): ``(values, indices)``, or None off the root of a reduce.
+        Each pair stages as one 16-byte record (csrc/b2_reduce_loc.cu)."""
+        values, indices = _prep(values), _prep(indices)
+        shape = values.shape[1:] if opcode == codes.OPC_REDUCE_SCATTER else values.shape
+        has_out = opcode != codes.OPC_REDUCE or self.comm.rank == root
+        out = ((torch.empty(shape, dtype=values.dtype, device=values.device),
+                torch.empty(shape, dtype=indices.dtype, device=values.device)) if has_out else None)
+        count = math.prod(shape)
+        self.ensure_stage(opcode, 16 * count)
+        rc = _lib().b2_reduce_loc(self.handle, values.data_ptr(), indices.data_ptr(),
+                                  out[0].data_ptr() if has_out else None, out[1].data_ptr() if has_out else None,
+                                  count, codes.DTYPE_CODE[values.dtype], indices.element_size(), op_code, opcode,
+                                  root, self._stream())
+        self._check(rc, codes.OPC_REDUCTION_NAME[opcode])
+        return out
+
     def allgather(self, x: torch.Tensor) -> torch.Tensor:
         x, lay = _layout(x)
         out = torch.empty((self.comm.size, *x.shape), dtype=x.dtype, device=x.device)
@@ -749,7 +767,7 @@ def _nvtx_wrap(name: str, fn):
 #: methods are left untouched otherwise, so the fast path pays nothing (SURVEY 5.1)
 NVTX_OPS = ("barrier", "allreduce", "reduce", "scan", "allgather", "alltoall", "bcast", "gather", "scatter",
             "send", "recv", "sendrecv", "reduce_scatter", "alltoallv", "allgatherv", "reduce_scatterv", "gatherv",
-            "scatterv",
+            "scatterv", "reduce_loc",
             "gemm_allreduce",
             "halo_exchange")
 if env_flag("MPI4JAX_B200_NVTX", False):

@@ -90,6 +90,10 @@ class HostStagedComm:
     def reduce_scatter(self, x, op_code: int):
         return self._up(_cpu.reduce_scatter(self.comm, self._down(x), op_code), x)
 
+    def reduce_loc(self, opcode: int, values, indices, op_code: int, root: int):
+        out = _cpu.reduce_loc(self.comm, opcode, self._down(values), self._down(indices), op_code, root)
+        return None if out is None else (self._up(out[0], values), self._up(out[1], values))
+
     def allgather(self, x):
         return self._up(_cpu.allgather(self.comm, self._down(x)), x)
 

@@ -116,6 +116,20 @@ def reduce_scatter(comm: Comm, x: torch.Tensor, op_code: int) -> torch.Tensor:
                    _cpu.reduce_scatter, x, op_code)
 
 
+def reduce_loc(comm: Comm, opcode: int, values: torch.Tensor, indices: torch.Tensor, op_code: int, root: int):
+    """MAXLOC / MINLOC of ``(values, indices)`` pairs for the reduction collective ``opcode`` (collective_ops/_loc.py
+    states the rule): ``(values, indices)``, or None off the root of a reduce."""
+    _plain(values)
+    _plain(indices)
+    if values.is_cuda:
+        return comm._native_comm().reduce_loc(opcode, values, indices, op_code, root)
+    n = values.numel() // values.shape[0] if opcode == codes.OPC_REDUCE_SCATTER else values.numel()
+    details = f"with {n} pairs" + (f" to root {root}" if opcode == codes.OPC_REDUCE else
+                                   " per block" if opcode == codes.OPC_REDUCE_SCATTER else "")
+    return _on_cpu(comm, codes.OPC_REDUCTION_NAME[opcode], details, _cpu.reduce_loc, opcode, values, indices, op_code,
+                   root)
+
+
 def allgather(comm: Comm, x: torch.Tensor) -> torch.Tensor:
     _plain(x)
     if x.is_cuda:

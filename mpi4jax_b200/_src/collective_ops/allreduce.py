@@ -16,7 +16,7 @@ from ..native import codes
 from ..utils import (NOTSET, as_tensor, check_dtype, fold, get_default_comm, needs_autograd,
                      raise_if_token_is_set)
 from ..validation import enforce_types
-from . import _dispatch
+from . import _dispatch, _loc
 
 
 def _require_sum(op: Op, what: str) -> None:
@@ -60,7 +60,8 @@ def allreduce(x, op, *, comm=None, token=NOTSET, algorithm="auto"):
     """Perform an allreduce operation.
 
     Arguments:
-        x: tensor, array or scalar input.
+        x: tensor, array or scalar input; with ``MPI.MAXLOC`` / ``MPI.MINLOC`` a pair
+            ``(values, indices)`` (see below).
         op: the reduction operator (e.g. ``mpi4jax_b200.MPI.SUM``).
         comm: the communicator (defaults to a clone of ``COMM_WORLD``).
         algorithm: GPU transport -- ``"auto"`` (size table), ``"ll"``, ``"oneshot"``,
@@ -68,11 +69,19 @@ def allreduce(x, op, *, comm=None, token=NOTSET, algorithm="auto"):
 
     Returns:
         Tensor: result of the allreduce (same shape and dtype as ``x``).
+
+    With ``op=MPI.MAXLOC`` or ``MPI.MINLOC``, ``x`` is a pair ``(values, indices)`` of one shape (values
+    float16, bfloat16, float32, float64, int16, int32 or int64; indices int32 or int64; elements may be
+    Python scalars) and the result is the pair ``(values, indices)`` of the extreme value over the ranks and
+    its index, elementwise: ties go to the smaller index, NaN wins (``collective_ops/_loc.py``).  Not
+    differentiable.
     """
     raise_if_token_is_set(token)
     if comm is None:
         comm = get_default_comm()
     op = as_op(op)
+    if _loc.is_loc(op):
+        return _loc.reduce_loc("allreduce", codes.OPC_ALLREDUCE, x, op, comm, algorithm=algorithm)
     x = as_tensor(x, comm)
     check_dtype(x)
     algo = codes.ALGO_BY_NAME[algorithm]

@@ -18,7 +18,8 @@ from ..comm import OP_TYPES, SUM, Comm, Op, as_op
 from ..utils import (NOTSET, as_tensor, check_dtype, fold, get_default_comm, needs_autograd,
                      raise_if_token_is_set)
 from ..validation import enforce_types
-from . import _dispatch
+from ..native import codes
+from . import _dispatch, _loc
 from .bcast import _check_root
 
 
@@ -48,12 +49,16 @@ def reduce(x, op, root, *, comm=None, token=NOTSET):
     """Perform a reduce operation.
 
     Returns:
-        Tensor: on the root the reduced data; on every other rank the input ``x``.
+        Tensor: on the root the reduced data; on every other rank the input ``x``.  With ``MPI.MAXLOC`` /
+        ``MPI.MINLOC``, ``x`` and the result are ``(values, indices)`` pairs (see ``allreduce``).
     """
     raise_if_token_is_set(token)
     if comm is None:
         comm = get_default_comm()
     op = as_op(op)
+    if _loc.is_loc(op):
+        _check_root(root, comm, "Reduce")
+        return _loc.reduce_loc("reduce", codes.OPC_REDUCE, x, op, comm, int(root))
     x = as_tensor(x, comm)
     check_dtype(x)
     _check_root(root, comm, "Reduce")

@@ -16,7 +16,8 @@ from ..comm import OP_TYPES, SUM, Comm, Op, as_op
 from ..utils import (NOTSET, as_tensor, check_dtype, fold, get_default_comm, needs_autograd,
                      raise_if_token_is_set)
 from ..validation import enforce_types
-from . import _adjoints, _dispatch
+from ..native import codes
+from . import _adjoints, _dispatch, _loc
 
 
 def _require_sum(op: Op, what: str) -> None:
@@ -59,12 +60,16 @@ def reduce_scatter(x, op, *, comm=None, token=NOTSET):
         comm: the communicator (defaults to a clone of ``COMM_WORLD``).
 
     Returns:
-        Tensor: ``op`` over all ranks of their block ``rank``, shape ``x.shape[1:]``, dtype of ``x``.
+        Tensor: ``op`` over all ranks of their block ``rank``, shape ``x.shape[1:]``, dtype of ``x``.  With
+        ``MPI.MAXLOC`` / ``MPI.MINLOC``, ``x`` is a pair ``(values, indices)`` of shape ``(nproc, ...)`` and the
+        result is the pair of this rank's blocks (see ``allreduce``).
     """
     raise_if_token_is_set(token)
     if comm is None:
         comm = get_default_comm()
     op = as_op(op)
+    if _loc.is_loc(op):
+        return _loc.reduce_loc("reduce_scatter", codes.OPC_REDUCE_SCATTER, x, op, comm)
     x = as_tensor(x, comm)
     check_dtype(x)
     if x.dim() == 0 or x.shape[0] != comm.Get_size():

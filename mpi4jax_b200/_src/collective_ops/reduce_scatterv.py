@@ -34,7 +34,7 @@ from ..comm import OP_TYPES, SUM, Comm, Op, as_op
 from ..utils import (NOTSET, as_tensor, check_dtype, get_default_comm, needs_autograd,
                      raise_if_token_is_set)
 from ..validation import enforce_types
-from . import _adjoints, _dispatch
+from . import _adjoints, _dispatch, _loc
 from ._rowsv import RowsvFunction
 
 
@@ -117,6 +117,7 @@ def reduce_scatterv(x, send_counts, op, *, recv_capacity=None, comm=None, token=
     if comm is None:
         comm = get_default_comm()
     op = as_op(op)
+    _loc.refuse(op, "reduce_scatterv")
     x = as_tensor(x, comm)
     check_dtype(x)
     _dispatch.check_rows("Reduce_scatterv", x)

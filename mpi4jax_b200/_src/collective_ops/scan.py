@@ -17,7 +17,7 @@ from ..native import codes
 from ..utils import (NOTSET, as_tensor, check_dtype, fold, get_default_comm, needs_autograd,
                      raise_if_token_is_set)
 from ..validation import enforce_types
-from . import _dispatch
+from . import _dispatch, _loc
 
 
 class _Scan(torch.autograd.Function):
@@ -46,11 +46,14 @@ class _Scan(torch.autograd.Function):
 
 @enforce_types(op=OP_TYPES, comm=(type(None), Comm))
 def scan(x, op, *, comm=None, token=NOTSET):
-    """Perform a scan operation (inclusive prefix reduction over the ranks)."""
+    """Perform a scan operation (inclusive prefix reduction over the ranks).  With ``MPI.MAXLOC`` /
+    ``MPI.MINLOC``, ``x`` and the result are ``(values, indices)`` pairs (see ``allreduce``)."""
     raise_if_token_is_set(token)
     if comm is None:
         comm = get_default_comm()
     op = as_op(op)
+    if _loc.is_loc(op):
+        return _loc.reduce_loc("scan", codes.OPC_SCAN, x, op, comm)
     x = as_tensor(x, comm)
     check_dtype(x)
     if op.code is None:                      # MPI.Op.Create: gather natively, fold ranks 0 .. r

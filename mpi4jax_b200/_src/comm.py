@@ -5,7 +5,7 @@ and forwards their C handles to its C++ bridge (/root/reference/mpi4jax/_src/uti
 60-153).  Neither mpi4py nor an MPI library exists on the target image, and the H100
 transport is not MPI at all, so this module supplies the small object model user code
 needs (``mpi4jax_b200.MPI``): ``COMM_WORLD``, ``Comm.Get_rank/Get_size/Clone/Split/
-Free/Barrier``, the ten predefined ``Op`` constants, ``Status`` with
+Free/Barrier``, the ten predefined elementwise ``Op`` constants and ``MAXLOC`` / ``MINLOC``, ``Status`` with
 ``Get_source/Get_tag/Get_count``, ``ANY_SOURCE``/``ANY_TAG``.
 
 Process model (same as the reference, README.rst:83-89): one OS process per rank, one
@@ -40,8 +40,9 @@ class MPIError(RuntimeError):
 
 
 class Op:
-    """A reduction operator (stand-in for ``mpi4py.MPI.Op``): one of the ten predefined ones
-    (``code`` selects the fused kernel instantiation) or a user-defined one made with
+    """A reduction operator (stand-in for ``mpi4py.MPI.Op``): one of the ten predefined elementwise ones
+    (``code`` selects the fused kernel instantiation), ``MAXLOC`` / ``MINLOC`` (which reduce
+    ``(values, indices)`` pairs, collective_ops/_loc.py), or a user-defined one made with
     :meth:`Op.Create` (``code is None``, ``function`` is applied on the device)."""
 
     __slots__ = ("name", "code", "function", "commute")
@@ -75,11 +76,17 @@ class Op:
 
     def python_function(self):
         """Binary Python function of the operator (used by the object collectives, like mpi4py's
-        ``comm.allreduce(obj, op)``)."""
+        ``comm.allreduce(obj, op)``).  MAXLOC / MINLOC fold ``(value, index)`` pairs of Python numbers, or of
+        tensors elementwise, by the rule of collective_ops/_loc.py."""
+        import functools
         import operator
 
         if self.function is not None:
             return self.function
+        if self.name in ("MAXLOC", "MINLOC"):
+            from .collective_ops import _loc
+
+            return functools.partial(_loc.fold, maxloc=self.name == "MAXLOC")
 
         return {
             "SUM": operator.add, "PROD": operator.mul, "MIN": min, "MAX": max,
@@ -107,7 +114,9 @@ LXOR = Op("LXOR", codes.LXOR)
 BAND = Op("BAND", codes.BAND)
 BOR = Op("BOR", codes.BOR)
 BXOR = Op("BXOR", codes.BXOR)
-_ALL_OPS = {o.name: o for o in (SUM, PROD, MIN, MAX, LAND, LOR, LXOR, BAND, BOR, BXOR)}
+MAXLOC = Op("MAXLOC", codes.MAXLOC)
+MINLOC = Op("MINLOC", codes.MINLOC)
+_ALL_OPS = {o.name: o for o in (SUM, PROD, MIN, MAX, LAND, LOR, LXOR, BAND, BOR, BXOR, MAXLOC, MINLOC)}
 
 
 def _op_by_name(name: str) -> Op:

@@ -27,7 +27,7 @@ import torch
 from torch.library import custom_op
 
 from . import comm as _comm_mod
-from .collective_ops import _adjoints, _dispatch
+from .collective_ops import _adjoints, _dispatch, _loc
 from .comm import ANY_SOURCE, ANY_TAG, SUM, Comm, as_op
 from .native import codes
 from .utils import get_default_comm
@@ -117,6 +117,21 @@ def _reduce_scatter_backward(ctx, g):
 
 
 _reduce_scatter.register_autograd(_reduce_scatter_backward, setup_context=_reduce_scatter_setup)
+
+
+@custom_op("mpi4jax_b200::reduce_loc", mutates_args=())
+def _reduce_loc(values: torch.Tensor, indices: torch.Tensor, op: int, kind: int, root: int,
+                comm_id: int) -> tuple[torch.Tensor, torch.Tensor]:
+    # MAXLOC / MINLOC of (values, indices) pairs; `kind`: the collective's opcode.  Off the root of a reduce:
+    # copies of the input pair.  No autograd rule: the eager op has none either.
+    out = _dispatch.reduce_loc(_c(comm_id), kind, values.contiguous(), indices.contiguous(), op, root)
+    return (values.clone(), indices.clone()) if out is None else out
+
+
+@_reduce_loc.register_fake
+def _(values, indices, op, kind, root, comm_id):
+    shape = values.shape[1:] if kind == codes.OPC_REDUCE_SCATTER else values.shape
+    return values.new_empty(shape), indices.new_empty(shape)
 
 
 @custom_op("mpi4jax_b200::allgather", mutates_args=())
@@ -464,7 +479,7 @@ _sendrecv.register_autograd(_sendrecv_backward, setup_context=_sendrecv_setup)
 
 ALL_OPS = ("allreduce", "allgather", "alltoall", "bcast", "scan", "reduce", "gather_root", "gather_leaf",
            "scatter", "barrier", "send", "recv", "sendrecv", "reduce_scatter", "alltoallv", "allgatherv",
-           "reduce_scatterv", "gatherv_root", "gatherv_leaf", "scatterv")
+           "reduce_scatterv", "gatherv_root", "gatherv_leaf", "scatterv", "reduce_loc")
 ORDERED_EFFECT = False
 try:  # the ordered effect: AOTAutograd threads a token through these ops in program order
     from torch._higher_order_ops.effects import _EffectType, _register_effectful_op
@@ -482,14 +497,22 @@ class compiled:
 
     @staticmethod
     def allreduce(x, op, *, comm=None):
-        return torch.ops.mpi4jax_b200.allreduce(x, as_op(op).code, _register(comm))
+        """With ``MPI.MAXLOC`` / ``MPI.MINLOC``, ``x`` and the result are ``(values, indices)`` pairs (the
+        ``reduce_loc`` op); the same holds for ``reduce``, ``scan`` and ``reduce_scatter``."""
+        op = as_op(op)
+        if _loc.is_loc(op):
+            return _loc.compiled_loc("allreduce", codes.OPC_ALLREDUCE, x, op, comm or get_default_comm())
+        return torch.ops.mpi4jax_b200.allreduce(x, op.code, _register(comm))
 
     @staticmethod
     def reduce_scatter(x, op, *, comm=None):
         comm = comm or get_default_comm()
+        op = as_op(op)
+        if _loc.is_loc(op):
+            return _loc.compiled_loc("reduce_scatter", codes.OPC_REDUCE_SCATTER, x, op, comm)
         if x.dim() == 0 or x.shape[0] != comm.Get_size():
             raise ValueError("Reduce_scatter input must have shape (nproc, ...)")
-        return torch.ops.mpi4jax_b200.reduce_scatter(x, as_op(op).code, comm._id)
+        return torch.ops.mpi4jax_b200.reduce_scatter(x, op.code, comm._id)
 
     @staticmethod
     def allgather(x, *, comm=None):
@@ -533,8 +556,10 @@ class compiled:
         """``(out, recv_counts)`` of :func:`mpi4jax_b200.reduce_scatterv` for the built-in operators;
         ``send_counts`` must be a device tensor of shape ``(nproc,)``."""
         comm = comm or get_default_comm()
+        op = as_op(op)
+        _loc.refuse(op, "reduce_scatterv")
         cap = _dispatch.rowsv_capacity("Reduce_scatterv", comm, x, send_counts, recv_capacity, "send_counts", 1)
-        return torch.ops.mpi4jax_b200.reduce_scatterv(x, send_counts, cap, as_op(op).code, comm._id)
+        return torch.ops.mpi4jax_b200.reduce_scatterv(x, send_counts, cap, op.code, comm._id)
 
     @staticmethod
     def gatherv(x, count, root, *, recv_capacity=None, comm=None):
@@ -574,11 +599,17 @@ class compiled:
 
     @staticmethod
     def scan(x, op, *, comm=None):
-        return torch.ops.mpi4jax_b200.scan(x, as_op(op).code, _register(comm))
+        op = as_op(op)
+        if _loc.is_loc(op):
+            return _loc.compiled_loc("scan", codes.OPC_SCAN, x, op, comm or get_default_comm())
+        return torch.ops.mpi4jax_b200.scan(x, op.code, _register(comm))
 
     @staticmethod
     def reduce(x, op, root, *, comm=None):
-        return torch.ops.mpi4jax_b200.reduce(x, as_op(op).code, int(root), _register(comm))
+        op = as_op(op)
+        if _loc.is_loc(op):
+            return _loc.compiled_loc("reduce", codes.OPC_REDUCE, x, op, comm or get_default_comm(), root)
+        return torch.ops.mpi4jax_b200.reduce(x, op.code, int(root), _register(comm))
 
     @staticmethod
     def gather(x, root, *, comm=None):

@@ -27,6 +27,7 @@ DTYPE_CODE = {
 
 # enum B2Op
 SUM, PROD, MIN, MAX, LAND, LOR, LXOR, BAND, BOR, BXOR = range(10)
+MAXLOC, MINLOC = 10, 11         # value-index reductions: not members of the [dtype][op] kernel tables
 
 # enum B2Algo
 ALGO_AUTO, ALGO_LL, ALGO_ONESHOT, ALGO_TWOSHOT, ALGO_NVLS = range(5)
@@ -47,5 +48,9 @@ OPC_ALLGATHERV = 15
 OPC_REDUCE_SCATTERV = 16
 OPC_GATHERV = 17
 OPC_SCATTERV = 18
+
+# MPI names of the reduction collectives (debug log lines, error messages)
+OPC_REDUCTION_NAME = {OPC_ALLREDUCE: "Allreduce", OPC_REDUCE: "Reduce", OPC_SCAN: "Scan",
+                      OPC_REDUCE_SCATTER: "Reduce_scatter_block"}
 
 ANY = -1  # ANY_SOURCE / ANY_TAG on the wire
