@@ -33,6 +33,7 @@ static void b2_ensure_tables() {
   b2_register_reduce_group_1();
   b2_register_reduce_group_2();
   b2_register_reduce_group_3();
+  b2_register_reduce_group_4();
   b2_register_reduce_loc();
   done = true;
 }

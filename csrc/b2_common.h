@@ -16,7 +16,7 @@
 #include <cstddef>
 #include <cstdint>
 
-#define B2_ABI_VERSION 18  // bump whenever a struct shared with Python or a C signature changes
+#define B2_ABI_VERSION 19  // bump whenever a struct shared with Python or a C signature changes
 #define B2_MAX_RANKS 16          // ranks per NVLink domain we support (8 on HGX H100)
 // bytes of the count header in front of the rows the variable-count collectives stage: one int64
 // per possible rank (keeps the rows 16-byte aligned)
@@ -33,7 +33,8 @@ enum B2DType : int {
   B2_I8 = 4, B2_I16 = 5, B2_I32 = 6, B2_I64 = 7,
   B2_U8 = 8, B2_U16 = 9, B2_U32 = 10, B2_U64 = 11,
   B2_BOOL = 12, B2_C64 = 13, B2_C128 = 14,
-  B2_DTYPE_COUNT = 15
+  B2_F8E4M3 = 15, B2_F8E5M2 = 16,   // float8 e4m3fn / e5m2: fp32 accumulation, rounded like torch's cast
+  B2_DTYPE_COUNT = 17
 };
 
 enum B2Op : int {
@@ -98,7 +99,7 @@ static inline size_t b2_dtype_size(int dt) {
     case B2_F32: case B2_I32: case B2_U32: return 4;
     case B2_F64: case B2_I64: case B2_U64: case B2_C64: return 8;
     case B2_F16: case B2_BF16: case B2_I16: case B2_U16: return 2;
-    case B2_I8: case B2_U8: case B2_BOOL: return 1;
+    case B2_I8: case B2_U8: case B2_BOOL: case B2_F8E4M3: case B2_F8E5M2: return 1;
     case B2_C128: return 16;
     default: return 0;
   }

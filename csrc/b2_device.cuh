@@ -5,8 +5,8 @@
 //   * the block-paired cross-GPU barrier (CTA b on every rank <-> CTA b)
 //   * the per-kernel ticket (staging parity + unique flag values, advanced on
 //     the device so CUDA-graph replays stay correct)
-//   * 16-byte vector movers and the typed reduction functors (10 ops x 15 dtypes,
-//     fp32 accumulation for f16/bf16)
+//   * 16-byte vector movers and the typed reduction functors (10 ops x 17 dtypes,
+//     fp32 accumulation for f16/bf16 and the two float8 formats)
 #pragma once
 
 #include <cuda_bf16.h>
@@ -309,6 +309,72 @@ template <> struct B2Traits<b2_boolean> {
   static __device__ __forceinline__ b2_boolean down(Acc v) { b2_boolean r; r.v = v; return r; }
 };
 
+// Hopper's float8 formats (tag types: the byte is the value).  Widening is exact: e4m3 through the hardware
+// f16x2 conversion, e5m2 as the top byte of an f16; the sign bit is or-ed back in, because the e4m3 conversion
+// makes every NaN the positive f16 NaN.  Narrowing is the hardware's round-to-nearest-even with satfinite
+// (one F2FP per pair), then a compare-select turns its clamp into torch's Tensor.to(float8) overflow:
+// e4m3fn |x| > 464, inf and NaN -> NaN; e5m2 |x| >= 61440 and inf -> inf, NaN -> NaN; the sign kept.
+struct b2_f8e4m3 { unsigned char v; };
+struct b2_f8e5m2 { unsigned char v; };
+
+template <typename F> struct B2F8;
+template <> struct B2F8<b2_f8e4m3> {
+  static __device__ __forceinline__ unsigned up2(unsigned short p) {     // two bytes -> f16x2
+    unsigned h2;
+    asm("cvt.rn.f16x2.e4m3x2 %0, %1;" : "=r"(h2) : "h"(p));
+    return h2;
+  }
+  static __device__ __forceinline__ unsigned short down2(float lo, float hi) {
+    unsigned short p;
+    asm("cvt.rn.satfinite.e4m3x2.f32 %0, %1, %2;" : "=h"(p) : "f"(hi), "f"(lo));
+    return p;
+  }
+  static __device__ __forceinline__ unsigned fix(float x, unsigned b) {
+    return fabsf(x) <= 464.f ? b : ((__float_as_uint(x) >> 24) & 0x80u) | 0x7Fu;
+  }
+};
+template <> struct B2F8<b2_f8e5m2> {
+  static __device__ __forceinline__ unsigned up2(unsigned short p) { return __byte_perm(p, 0u, 0x1404); }
+  static __device__ __forceinline__ unsigned short down2(float lo, float hi) {
+    unsigned short p;
+    asm("cvt.rn.satfinite.e5m2x2.f32 %0, %1, %2;" : "=h"(p) : "f"(hi), "f"(lo));
+    return p;
+  }
+  static __device__ __forceinline__ unsigned fix(float x, unsigned b) {
+    return fabsf(x) < 61440.f ? b : ((__float_as_uint(x) >> 24) & 0x80u) | (x != x ? 0x7Fu : 0x7Cu);
+  }
+};
+// bytes 0 and 1 of `w` (k = 0) or 2 and 3 (k = 1), widened
+template <typename F>
+__device__ __forceinline__ float2 b2_f8x2_up(unsigned w, int k) {
+  const unsigned h2 = B2F8<F>::up2((unsigned short)(w >> (16 * k)));
+  const float2 f = __half22float2(*reinterpret_cast<const __half2*>(&h2));
+  return make_float2(__uint_as_float(__float_as_uint(f.x) | ((w << (24 - 16 * k)) & 0x80000000u)),
+                     __uint_as_float(__float_as_uint(f.y) | ((w << (16 - 16 * k)) & 0x80000000u)));
+}
+template <typename F>
+__device__ __forceinline__ unsigned b2_f8x2_down(float lo, float hi) {
+  const unsigned p = B2F8<F>::down2(lo, hi);
+  return B2F8<F>::fix(lo, p & 0xFFu) | (B2F8<F>::fix(hi, p >> 8) << 8);
+}
+template <> struct B2Traits<b2_f8e4m3> {
+  using Acc = float;
+  static __device__ __forceinline__ Acc up(b2_f8e4m3 v) { return b2_f8x2_up<b2_f8e4m3>(v.v, 0).x; }
+  static __device__ __forceinline__ b2_f8e4m3 down(Acc v) {
+    b2_f8e4m3 r; r.v = (unsigned char)b2_f8x2_down<b2_f8e4m3>(v, 0.f); return r;
+  }
+};
+template <> struct B2Traits<b2_f8e5m2> {
+  using Acc = float;
+  static __device__ __forceinline__ Acc up(b2_f8e5m2 v) { return b2_f8x2_up<b2_f8e5m2>(v.v, 0).x; }
+  static __device__ __forceinline__ b2_f8e5m2 down(Acc v) {
+    b2_f8e5m2 r; r.v = (unsigned char)b2_f8x2_down<b2_f8e5m2>(v, 0.f); return r;
+  }
+};
+template <typename T> struct b2_is_fp8 { static constexpr bool value = false; };
+template <> struct b2_is_fp8<b2_f8e4m3> { static constexpr bool value = true; };
+template <> struct b2_is_fp8<b2_f8e5m2> { static constexpr bool value = true; };
+
 template <typename A> struct b2_is_complex { static constexpr bool value = false; };
 template <> struct b2_is_complex<b2_c64> { static constexpr bool value = true; };
 template <> struct b2_is_complex<b2_c128> { static constexpr bool value = true; };
@@ -366,6 +432,41 @@ template <typename T> struct B2Vec {
     return *reinterpret_cast<const uint4*>(tmp);
   }
 };
+
+// float8: 16 elements per vector, widened and narrowed in pairs (8 packed conversions each way).  `a` stays
+// addressable per element for rsv_fold.
+template <typename F> struct B2Vec8 {
+  static constexpr int N = 16;
+  using Acc = float;
+  Acc a[N];
+  __device__ __forceinline__ void load(uint4 v) {
+    const unsigned w[4] = {v.x, v.y, v.z, v.w};
+#pragma unroll
+    for (int i = 0; i < 8; ++i) {
+      const float2 f = b2_f8x2_up<F>(w[i >> 1], i & 1);
+      a[2 * i] = f.x;
+      a[2 * i + 1] = f.y;
+    }
+  }
+  template <int OP> __device__ __forceinline__ void accumulate(uint4 v) {
+    const unsigned w[4] = {v.x, v.y, v.z, v.w};
+#pragma unroll
+    for (int i = 0; i < 8; ++i) {
+      const float2 f = b2_f8x2_up<F>(w[i >> 1], i & 1);
+      a[2 * i] = b2_apply<OP, Acc>(a[2 * i], f.x);
+      a[2 * i + 1] = b2_apply<OP, Acc>(a[2 * i + 1], f.y);
+    }
+  }
+  __device__ __forceinline__ uint4 store() const {
+    unsigned w[4];
+#pragma unroll
+    for (int j = 0; j < 4; ++j)
+      w[j] = b2_f8x2_down<F>(a[4 * j], a[4 * j + 1]) | (b2_f8x2_down<F>(a[4 * j + 2], a[4 * j + 3]) << 16);
+    return make_uint4(w[0], w[1], w[2], w[3]);
+  }
+};
+template <> struct B2Vec<b2_f8e4m3> : B2Vec8<b2_f8e4m3> {};
+template <> struct B2Vec<b2_f8e5m2> : B2Vec8<b2_f8e5m2> {};
 
 // Store the first `nbytes` (<16) bytes of a vector to an arbitrary address.
 __device__ __forceinline__ void b2_store_partial(void* dst, uint4 v, int nbytes) {

@@ -106,6 +106,8 @@ b2_k_reduce_chunked(const B2DevComm c, const B2ReduceArgs a) {
             if (q < c.size) v[q] = b2_ld_peer16(c.stage[q] + par + off + (i << 4));
           B2Vec<T> acc;
           acc.load(v[0]);
+          // float8 rounds every result, rank 0's single contribution too (a non-canonical e5m2 NaN)
+          if constexpr (b2_is_fp8<T>::value) b2_st16(c.stage[0] + par + off + (i << 4), acc.store());
 #pragma unroll
           for (int q = 1; q < B2_MAX_RANKS; ++q)
             if (q < c.size) {
@@ -410,6 +412,7 @@ void b2_register_reduce_group_0();
 void b2_register_reduce_group_1();
 void b2_register_reduce_group_2();
 void b2_register_reduce_group_3();
+void b2_register_reduce_group_4();
 
 #define B2_REG(DT, T, OP)                                                \
   b2_reduce_table[DT][OP] = &b2_launch_reduce<T, OP>;                    \

@@ -36,6 +36,8 @@ def _bytes_view(x: torch.Tensor) -> torch.Tensor:
 def reduce_stack(stack: torch.Tensor, op_code: int) -> torch.Tensor:
     """Reduce ``stack`` (P, *shape) over dim 0 with MPI op semantics, in rank order."""
     dt = stack.dtype
+    if dt in codes.FP8_DTYPE_CODE:
+        return _reduce_fp8(stack, op_code)
     if stack.shape[0] == 1:
         return stack[0].clone()     # a single contribution passes through unchanged (as in MPI)
     if dt == torch.bool:
@@ -93,6 +95,26 @@ def reduce_stack(stack: torch.Tensor, op_code: int) -> torch.Tensor:
         else:
             acc ^= wide[q]
     return acc.to(dt)
+
+
+def _reduce_fp8(stack: torch.Tensor, op_code: int) -> torch.Tensor:
+    """The float8 rule of the kernels (csrc/b2_device.cuh): widen exactly to fp32, fold in rank order with
+    ``b2_apply`` (the later NaN wins MIN / MAX), round once with torch's cast -- a single contribution too.
+    A NaN that SUM or PROD computes is the positive NaN, as the GPU's fp32 arithmetic makes it."""
+    check_op(stack.dtype, op_code)
+    wide = stack.to(torch.float32)
+    acc = wide[0]
+    for b in wide[1:]:
+        if op_code == codes.SUM:
+            acc = acc + b
+        elif op_code == codes.PROD:
+            acc = acc * b
+        else:
+            wins = b < acc if op_code == codes.MIN else b > acc
+            acc = torch.where(wins | b.isnan(), b, acc)
+    if op_code in (codes.SUM, codes.PROD) and stack.shape[0] > 1:
+        acc = torch.where(acc.isnan(), float("nan"), acc)
+    return acc.to(stack.dtype)
 
 
 def check_op(dtype: torch.dtype, op_code: int) -> None:

@@ -838,9 +838,9 @@ _BOOL_OP = {
 
 def _prep_reduce(x: torch.Tensor, op_code: int):
     x = _prep(x)
-    if x.dtype not in codes.DTYPE_CODE:
+    if x.dtype not in codes.WIRE_DTYPE_CODE:
         raise TypeError(f"dtype {x.dtype} is not supported by mpi4jax_b200 reductions")
-    dt = codes.DTYPE_CODE[x.dtype]
+    dt = codes.WIRE_DTYPE_CODE[x.dtype]
     if x.dtype == torch.bool:
         op_code = _BOOL_OP[op_code]
     elif x.dtype.is_complex and op_code not in (codes.SUM, codes.PROD):

@@ -233,7 +233,7 @@ _SIGNATURES = {
 
 
 #: must equal B2_ABI_VERSION in csrc/b2_common.h
-ABI_VERSION = 18
+ABI_VERSION = 19
 #: must equal B2_MAX_RANKS in csrc/b2_common.h (ranks per communicator; sizes the alltoallv count header)
 MAX_RANKS = 16
 _ABI_FIELDS = ("abi_version", "sizeof_status_record", "sizeof_halo_desc", "sizeof_swe_params",

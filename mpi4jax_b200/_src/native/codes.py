@@ -25,6 +25,17 @@ DTYPE_CODE = {
     torch.complex128: C128,
 }
 
+# Hopper's two 8-bit float formats (no MPI predefined datatype): every data-movement collective moves them
+# as bytes, the reductions widen to fp32, fold, and round once (csrc/b2_device.cuh)
+F8E4M3, F8E5M2 = 15, 16
+FP8_DTYPE_CODE = {
+    torch.float8_e4m3fn: F8E4M3,
+    torch.float8_e5m2: F8E5M2,
+}
+
+# every dtype with a wire representation
+WIRE_DTYPE_CODE = {**DTYPE_CODE, **FP8_DTYPE_CODE}
+
 # enum B2Op
 SUM, PROD, MIN, MAX, LAND, LOR, LXOR, BAND, BOR, BXOR = range(10)
 MAXLOC, MINLOC = 10, 11         # value-index reductions: not members of the [dtype][op] kernel tables

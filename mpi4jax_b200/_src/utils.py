@@ -60,12 +60,13 @@ def raise_if_token_is_set(token: Any) -> None:
 
 # dtypes with a wire representation.  The reference supports 14 numpy dtypes and NOT
 # float16/bfloat16 (utils.py:101-128); both 16-bit floats are supported here (fp32
-# accumulation inside the fused reduce kernels); float128 has no GPU representation.
-SUPPORTED_DTYPES = tuple(codes.DTYPE_CODE)
+# accumulation inside the fused reduce kernels), and so are Hopper's two float8 formats
+# (e4m3fn, e5m2: fp32 accumulation, one rounding); float128 has no GPU representation.
+SUPPORTED_DTYPES = tuple(codes.WIRE_DTYPE_CODE)
 
 
 def check_dtype(t: torch.Tensor) -> None:
-    if t.dtype not in codes.DTYPE_CODE:
+    if t.dtype not in codes.WIRE_DTYPE_CODE:
         raise RuntimeError(f"Unknown MPI type for dtype {t.dtype}")
 
 

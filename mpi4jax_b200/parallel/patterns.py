@@ -10,6 +10,7 @@ import torch
 from .. import _src as ops
 from .._src.collective_ops.alltoallv import alltoallv_reverse
 from .._src.comm import SUM, Comm
+from .._src.native import codes
 from .._src.utils import get_default_comm
 
 
@@ -88,7 +89,9 @@ def expert_dispatch(x: torch.Tensor, dest_rank: torch.Tensor, capacity: Optional
     # counts from the sorted keys: torch.bincount would read its maximum back to the host
     bounds = torch.searchsorted(key[order], torch.arange(n + 1, device=key.device))
     send_counts = bounds.diff()
-    rows, recv_counts = ops.alltoallv(x[order], send_counts, recv_capacity=capacity, comm=comm)
+    # float8 tokens are gathered as their bytes: torch's index kernels do not all take float8
+    picked = x.view(torch.uint8)[order].view(x.dtype) if x.dtype in codes.FP8_DTYPE_CODE else x[order]
+    rows, recv_counts = ops.alltoallv(picked, send_counts, recv_capacity=capacity, comm=comm)
     return rows, recv_counts, ExpertPlan(order, send_counts, recv_counts, comm)
 
 
