@@ -7,6 +7,9 @@ gradient correctness), data-parallel and tensor-parallel, eager and under ``mpi4
   calls ``mpi4jax.allreduce`` / ``bcast`` (README.rst:59-96, tests/collective_ops/test_allreduce.py:141-223).
 * tp: first layer column-sharded, second layer row-sharded; in bf16 the row-parallel GEMM and its
   allreduce are ONE wgmma + multimem kernel (csrc/b2_gemm.cu).
+* sp: batch sharded, weights sharded as in tp; the rows are all-gathered before the first layer and the
+  row-parallel GEMM and its reduce-scatter are ONE wgmma kernel in bf16 (csrc/b2_gemm_rs.cu).  Rank q
+  uses data(q), so its gradient shards are checked against the single-process gradient as for dp.
 
 Device-timed (CUDA events on the launching stream, barrier + synchronize before, max over ranks).
 
@@ -76,10 +79,10 @@ def data(q, dtype):
 
 
 result = {"world": size, "shape": [ns.d_in, ns.d_hidden, ns.d_out], "batch_per_rank": ns.batch}
-for mode, dtype in (("dp", torch.float32), ("tp", torch.float32), ("tp", torch.bfloat16)):
+for mode, dtype in (("dp", torch.float32), ("tp", torch.float32), ("tp", torch.bfloat16), ("sp", torch.bfloat16)):
     name = f"{mode}_{'bf16' if dtype == torch.bfloat16 else 'fp32'}"
     mlp = ParallelMLP(ns.d_in, ns.d_hidden, ns.d_out, comm=comm, device=dev, dtype=dtype, mode=mode)
-    x, y = data(rank if mode == "dp" else 0, dtype)           # tp: every rank sees the same batch
+    x, y = data(rank if mode != "tp" else 0, dtype)           # tp: every rank sees the same batch
     # ---- gradient correctness against the single-process loss -----------------------------
     for p in mlp.parameters():
         p.grad = None
@@ -92,6 +95,13 @@ for mode, dtype in (("dp", torch.float32), ("tp", torch.float32), ("tp", torch.b
         if rank == 0:       # the root's parameters receive the gradient summed over ranks (reduce-to-root)
             row["grad_rel_err"] = max(((mlp.w1.grad - g1).norm() / g1.norm()).item(),
                                       ((mlp.w2.grad - g2).norm() / g2.norm()).item())
+    elif mode == "sp":      # every rank holds its column / row shard of the single-process gradient
+        ref_loss, g1, g2 = reference_grads(dtype)
+        k = ns.d_hidden // size
+        s1, s2 = g1[:, rank * k:(rank + 1) * k], g2[rank * k:(rank + 1) * k]
+        row["loss_rel_err"] = abs(loss.item() - ref_loss.item()) / abs(ref_loss.item())
+        row["grad_rel_err"] = max(((mlp.w1.grad - s1).float().norm() / s1.float().norm()).item(),
+                                  ((mlp.w2.grad - s2).float().norm() / s2.float().norm()).item())
     else:
         row["loss_finite"] = bool(torch.isfinite(loss).item())
     # ---- step time: eager and as one CUDA graph --------------------------------------------
@@ -111,7 +121,7 @@ for mode, dtype in (("dp", torch.float32), ("tp", torch.float32), ("tp", torch.b
                             / (size if mode == "tp" else 1))
     row["tflops_per_gpu_jit"] = round(flops / row.get("jit_us", row["eager_us"]) / 1e6, 2)
     errs = comm.allgather(row.get("grad_rel_err"))
-    row["grad_rel_err"] = next((v for v in errs if v is not None), None)
+    row["grad_rel_err"] = max((v for v in errs if v is not None), default=None)
     result[name] = row
     if rank == 0:
         print(name, row, flush=True)

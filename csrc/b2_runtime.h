@@ -213,6 +213,10 @@ int b2_sendrecv(B2Comm* c, const void* sendbuf, size_t send_bytes, int dest, int
 // --- tensor-parallel linear: wgmma GEMM + in-switch allreduce in one kernel (b2_gemm.cu) ---
 int b2_gemm_allreduce(B2Comm* c, const void* A, const void* B, void* out, int M, int N, int K,
                       cudaStream_t stream);
+// ... and its sequence-parallel twin: GEMM + reduce-scatter over the rows (M % size == 0), this rank's
+// (M / size) x N shard of the sum; pull-and-fold epilogue, no multicast
+int b2_gemm_reduce_scatter(B2Comm* c, const void* A, const void* B, void* out, int M, int N, int K,
+                           cudaStream_t stream);
 
 // --- fused halo exchange + shallow-water stencils (see b2_halo.cu, b2_swe.cu) --
 struct B2HaloDesc {

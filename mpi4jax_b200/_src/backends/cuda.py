@@ -712,7 +712,7 @@ class NativeComm:
         self._bind_status(status, rec, out.element_size())
         return out
 
-    # -- tensor-parallel linear: wgmma GEMM + in-switch allreduce (csrc/b2_gemm.cu) ------------
+    # -- row-parallel linear: wgmma GEMM + allreduce / reduce-scatter (csrc/b2_gemm*.cu) ------------
     def gemm_allreduce(self, x: torch.Tensor, weight: torch.Tensor) -> torch.Tensor:
         """``allreduce_SUM(x @ weight.T)`` for bf16 ``x (M, K)``, ``weight (N, K)`` in ONE kernel."""
         M, K = x.shape
@@ -725,6 +725,22 @@ class NativeComm:
         rc = _lib().b2_gemm_allreduce(self.handle, x.data_ptr(), weight.data_ptr(), out.data_ptr(), M, N, K,
                                       self._stream())
         self._check(rc, "Allreduce")
+        return out
+
+    def gemm_reduce_scatter(self, x: torch.Tensor, weight: torch.Tensor) -> torch.Tensor:
+        """This rank's ``(M / size, N)`` row shard of ``sum over ranks (x @ weight.T)`` for bf16 ``x (M, K)``,
+        ``weight (N, K)`` in ONE kernel (csrc/b2_gemm_rs.cu); no multicast needed."""
+        M, K = x.shape
+        N = weight.shape[0]
+        P = self.comm.size
+        if M % P:
+            raise ValueError(f"gemm_reduce_scatter: M = {M} is not divisible by the {P} ranks")
+        out = torch.empty((M // P, N), dtype=torch.bfloat16, device=x.device)
+        if P > 1:
+            self.ensure_stage(codes.OPC_REDUCE_SCATTER, M * N * 2 // P)      # M*N*2 bytes per parity
+        rc = _lib().b2_gemm_reduce_scatter(self.handle, x.data_ptr(), weight.data_ptr(), out.data_ptr(), M, N, K,
+                                           self._stream())
+        self._check(rc, "Reduce_scatter_block")
         return out
 
     # -- fused halo exchange ---------------------------------------------------------
@@ -768,7 +784,7 @@ def _nvtx_wrap(name: str, fn):
 NVTX_OPS = ("barrier", "allreduce", "reduce", "scan", "allgather", "alltoall", "bcast", "gather", "scatter",
             "send", "recv", "sendrecv", "reduce_scatter", "alltoallv", "allgatherv", "reduce_scatterv", "gatherv",
             "scatterv", "reduce_loc",
-            "gemm_allreduce",
+            "gemm_allreduce", "gemm_reduce_scatter",
             "halo_exchange")
 if env_flag("MPI4JAX_B200_NVTX", False):
     for _name in NVTX_OPS:

@@ -10,8 +10,9 @@ fallback, never the default on one node:
 * forced by ``MPI4JAX_B200_TRANSPORT=host`` or the reference's ``MPI4JAX_USE_CUDA_MPI=0``.
 
 Same method surface as ``backends.cuda.NativeComm`` for the 15 ops; the fused / H100-only entry
-points (halo exchange, GEMM+allreduce) raise.  Ops synchronise the stream and block the host, so
-they cannot be captured into CUDA graphs: ``mpi4jax_b200.jit`` runs such functions eagerly.
+points (halo exchange, GEMM + allreduce, GEMM + reduce-scatter) raise.  Ops synchronise the stream and
+block the host, so they cannot be captured into CUDA graphs: ``mpi4jax_b200.jit`` runs such functions
+eagerly.
 """
 
 from __future__ import annotations
@@ -141,6 +142,9 @@ class HostStagedComm:
     # -- H100-only entry points ---------------------------------------------------------
     def gemm_allreduce(self, *a, **k):
         self._unsupported("the fused GEMM + allreduce kernel")
+
+    def gemm_reduce_scatter(self, *a, **k):
+        self._unsupported("the fused GEMM + reduce-scatter kernel")
 
     def halo_exchange(self, *a, **k):
         self._unsupported("the fused halo-exchange kernel")

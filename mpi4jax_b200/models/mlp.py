@@ -4,7 +4,9 @@ BASELINE.json config 5 ("grad through allreduce+bcast on a jitted MLP loss"): pa
 are created on rank 0 and broadcast (``bcast``, whose VJP is a reduce-to-root), the loss
 is averaged with ``allreduce`` (VJP = identity), hidden activations of the tensor-parallel
 variant are summed with ``allreduce`` exactly like the reference's column-sharded mat-vec
-pattern (/root/reference/tests/collective_ops/test_allreduce_matvec.py:41-65).
+pattern (/root/reference/tests/collective_ops/test_allreduce_matvec.py:41-65).  The sequence-parallel
+variant gathers the sharded rows before the first layer (``allgather``, whose VJP is a reduce-scatter)
+and reduce-scatters them after the second (``linear_reduce_scatter``, whose VJP is an allgather).
 """
 
 from __future__ import annotations
@@ -20,7 +22,10 @@ from .._src.utils import get_default_comm
 
 class ParallelMLP:
     """``mode="dp"``: replicated weights, batch sharded, gradients all-reduced.
-    ``mode="tp"``: first layer column-sharded, second layer row-sharded + allreduce."""
+    ``mode="tp"``: first layer column-sharded, second layer row-sharded + allreduce.
+    ``mode="sp"``: batch sharded and weights sharded as in ``"tp"``; the rows are all-gathered before the
+    column-parallel first layer and reduce-scattered back to their rank after the row-parallel second
+    layer, so each rank's output holds the rows of its own batch."""
 
     def __init__(self, d_in: int, d_hidden: int, d_out: int, comm: Optional[Comm] = None,
                  device=None, dtype=torch.float32, mode: str = "dp", seed: int = 0):
@@ -31,7 +36,7 @@ class ParallelMLP:
         gen = torch.Generator().manual_seed(seed)
         w1 = torch.randn(d_in, d_hidden, generator=gen, dtype=torch.float32) / d_in**0.5
         w2 = torch.randn(d_hidden, d_out, generator=gen, dtype=torch.float32) / d_hidden**0.5
-        if mode == "tp":
+        if mode in ("tp", "sp"):
             if d_hidden % P:
                 raise ValueError("d_hidden must be divisible by the number of ranks")
             k = d_hidden // P
@@ -54,6 +59,13 @@ class ParallelMLP:
 
                 return linear_allreduce(h, w2_.t(), comm=self.comm)
             return ops.allreduce(h @ w2_, SUM, comm=self.comm)       # row-parallel + sum
+        if self.mode == "sp":
+            from ..ops.linear import linear_reduce_scatter
+
+            xs = ops.allgather(x, comm=self.comm).reshape(-1, x.shape[-1])     # every rank's rows, in rank order
+            h = torch.tanh(xs @ w1_)                          # column-parallel
+            # row-parallel GEMM + reduce-scatter over the rows: one wgmma kernel for bf16 tile-aligned shapes
+            return linear_reduce_scatter(h, w2_.t(), comm=self.comm)
         w1 = ops.bcast(w1_, 0, comm=self.comm)                # parameters live on the root
         w2 = ops.bcast(w2_, 0, comm=self.comm)
         return torch.tanh(x @ w1) @ w2

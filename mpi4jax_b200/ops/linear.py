@@ -1,4 +1,4 @@
-"""Row-parallel linear layer with the allreduce fused into the GEMM kernel.
+"""Row-parallel linear layers with the allreduce or the reduce-scatter fused into the GEMM kernel.
 
 ``linear_allreduce(x, weight)`` = ``allreduce(x @ weight.T, SUM)`` where every rank holds a
 K-shard of both operands -- the tensor-parallel pattern of the reference's matvec tests
@@ -14,6 +14,13 @@ The K shards may differ between ranks, in length and in memory layout.  The fuse
 of every rank in its epilogue, so either every rank runs it or none does: the choice depends only on
 what all ranks share (M, N, the dtype, the transport and NVLS), and each rank then brings its own
 operands into the form the kernel needs (:func:`_kernel_operands`).
+
+``linear_reduce_scatter(x, weight)`` is the sequence-parallel twin: rank r keeps only rows
+``[r M/P, (r+1) M/P)`` of the same sum, ``reduce_scatter((x @ weight.T).reshape(P, M/P, N), SUM)``.
+Its kernel (csrc/b2_gemm_rs.cu) shares the GEMM and reduces each group of tiles by pulling every rank's
+staged partial, with no multicast, so it also runs where NVLS is off or the ranks share a GPU.  The
+adjoint of a reduce-scatter is an allgather: with ``G = allgather(g)``, ``grad_x = G @ weight`` and
+``grad_weight = G.T @ x``.
 """
 
 from __future__ import annotations
@@ -27,16 +34,22 @@ from .._src.collective_ops import _dispatch
 from .._src.comm import SUM, Comm
 from .._src.utils import get_default_comm, needs_autograd
 
-_BM, _BN, _BK = 128, 128, 64     # tile of csrc/b2_gemm.cu
+_BM, _BN, _BK = 128, 128, 64     # tile of csrc/b2_gemm_body.cuh
 
 
-def _fuse(x: torch.Tensor, w: torch.Tensor, comm: Comm) -> bool:
-    """Whether to run the fused kernel; the same answer on every rank of ``comm``."""
+def _kernel_shape(x: torch.Tensor, w: torch.Tensor, comm: Comm) -> bool:
+    """bf16 CUDA operands with tile-aligned M and N on the native transport: what both kernels need.
+    The same answer on every rank of ``comm``."""
     if not (x.is_cuda and w.is_cuda and x.dtype == torch.bfloat16 and w.dtype == torch.bfloat16
             and x.dim() == 2 and w.dim() == 2):
         return False
     M, N = x.shape[0], w.shape[0]
-    if M == 0 or N == 0 or M % _BM or N % _BN or comm.transport != "native":
+    return not (M == 0 or N == 0 or M % _BM or N % _BN or comm.transport != "native")
+
+
+def _fuse(x: torch.Tensor, w: torch.Tensor, comm: Comm) -> bool:
+    """Whether to run the fused allreduce kernel; the same answer on every rank of ``comm``."""
+    if not _kernel_shape(x, w, comm):
         return False
     return comm.Get_size() == 1 or comm._native_comm().has_nvls
 
@@ -86,3 +99,45 @@ def linear_allreduce(x: torch.Tensor, weight: torch.Tensor, *, comm: Optional[Co
     if not needs_autograd(x, weight):
         return _forward(x, weight, comm)
     return _LinearAllreduce.apply(x, weight, comm)
+
+
+def _forward_rs(x: torch.Tensor, w: torch.Tensor, comm: Comm) -> torch.Tensor:
+    P = comm.Get_size()
+    if _kernel_shape(x, w, comm):
+        nc = comm._native_comm()
+        xk, wk = _kernel_operands(x, w)
+        # one rank: the reduce-scatter is the identity and the kernel the stand-alone GEMM
+        return nc.gemm_allreduce(xk, wk) if P == 1 else nc.gemm_reduce_scatter(xk, wk)
+    y = (x @ w.t()).contiguous()
+    return _dispatch.reduce_scatter(comm, y.reshape(P, y.shape[0] // P, y.shape[1]), SUM.code)
+
+
+class _LinearReduceScatter(torch.autograd.Function):
+    @staticmethod
+    def forward(x, w, comm):
+        return _forward_rs(x, w, comm)
+
+    @staticmethod
+    def setup_context(ctx, inputs, output):
+        x, w, ctx.comm = inputs
+        ctx.save_for_backward(x, w)
+
+    @staticmethod
+    def backward(ctx, g):
+        x, w = ctx.saved_tensors
+        G = _dispatch.allgather(ctx.comm, g.contiguous()).reshape(x.shape[0], g.shape[1])
+        return G @ w, G.t() @ x, None
+
+
+def linear_reduce_scatter(x: torch.Tensor, weight: torch.Tensor, *, comm: Optional[Comm] = None) -> torch.Tensor:
+    """Rows ``[r M/P, (r+1) M/P)`` of ``x (M, K_local) @ weight (N, K_local).T`` summed over the P ranks of
+    ``comm``, on rank r: shape ``(M / P, N)``.  ``M`` must be divisible by P."""
+    comm = comm or get_default_comm()
+    P = comm.Get_size()
+    if x.dim() != 2 or weight.dim() != 2:
+        raise ValueError(f"linear_reduce_scatter: x and weight must be 2-D (got {x.dim()}-D and {weight.dim()}-D)")
+    if x.shape[0] % P:
+        raise ValueError(f"linear_reduce_scatter: M = {x.shape[0]} rows are not divisible by the {P} ranks")
+    if not needs_autograd(x, weight):
+        return _forward_rs(x, weight, comm)
+    return _LinearReduceScatter.apply(x, weight, comm)

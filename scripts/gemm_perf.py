@@ -1,4 +1,5 @@
-"""Fused wgmma GEMM+allreduce vs cuBLAS GEMM followed by an allreduce (ours / NCCL)."""
+"""Fused wgmma GEMM+allreduce vs cuBLAS GEMM followed by an allreduce (ours / NCCL), and for M divisible by
+the world size the same for GEMM+reduce-scatter over the rows."""
 import os
 import sys
 
@@ -8,7 +9,7 @@ import torch.distributed as dist  # noqa: E402
 
 import mpi4jax_b200 as m  # noqa: E402
 from mpi4jax_b200 import MPI  # noqa: E402
-from mpi4jax_b200.ops import linear_allreduce  # noqa: E402
+from mpi4jax_b200.ops import linear_allreduce, linear_reduce_scatter  # noqa: E402
 from mpi4jax_b200.utils import max_over_ranks  # noqa: E402
 
 comm = MPI.COMM_WORLD
@@ -44,6 +45,17 @@ for (M, N, K) in [(4096, 4096, 4096 // size), (8192, 8192, 8192 // size), (8192,
             dist.all_reduce(y, group=nccl)
             return y
         rows["cublas + nccl allreduce"] = timeit(f)
+    if M % size == 0:
+        rows["fused wgmma+reduce-scatter (one kernel)"] = timeit(lambda: linear_reduce_scatter(x, w, comm=comm))
+        rows["cublas + our reduce_scatter"] = timeit(
+            lambda: m.reduce_scatter((x @ w.t()).reshape(size, M // size, N), MPI.SUM, comm=comm))
+        if nccl is not None:
+            def g():
+                y = x @ w.t()
+                out = torch.empty(M // size, N, device=dev, dtype=y.dtype)
+                dist.reduce_scatter_tensor(out, y, group=nccl)
+                return out
+            rows["cublas + nccl reduce_scatter_tensor"] = timeit(g)
     rows["cublas gemm only"] = timeit(lambda: x @ w.t())
     if rank == 0:
         print(f"M={M} N={N} K/rank={K} (bf16 out {M * N * 2 / 2**20:.0f} MiB): " +
