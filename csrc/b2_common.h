@@ -16,7 +16,7 @@
 #include <cstddef>
 #include <cstdint>
 
-#define B2_ABI_VERSION 19  // bump whenever a struct shared with Python or a C signature changes
+#define B2_ABI_VERSION 20  // bump whenever a struct shared with Python or a C signature changes
 #define B2_MAX_RANKS 16          // ranks per NVLink domain we support (8 on HGX H100)
 // bytes of the count header in front of the rows the variable-count collectives stage: one int64
 // per possible rank (keeps the rows 16-byte aligned)

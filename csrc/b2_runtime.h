@@ -249,13 +249,15 @@ struct B2SweParams {
 
 // Device pointers of a model's fields (mirrored by ctypes in _src/native/__init__.py; the layout
 // is part of the ABI checked at import).  h0/h1, u/u1, v/v1, du/du1 and dv/dv1 are ping-pong pairs;
-// the first of each pair holds the state between calls.
+// the first of each holds the state between calls.  The communication-avoiding step rotates three
+// sets (h0, u, v, dh, du, dv), (h1, u1, ..., dh1, ...) and (h2, u2, ..., dh2, ...).
 struct B2SweState {
   float *h0, *h1, *u, *v, *dh, *du, *dv, *fe, *fn, *q, *ke, *fe2, *fn2;
   float* u1;
   float* v1;
   float* du1;
   float* dv1;
+  float *h2, *u2, *v2, *dh1, *dh2, *du2, *dv2;
 };
 
 // "ext" arrays of the communication-avoiding step (b2_swe_ca_body.cuh): [(ny + 4) x epitch] floats,

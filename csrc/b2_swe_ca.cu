@@ -6,13 +6,13 @@
 //   stream s  (bulk) :  S  flux + tendency + friction of the bulk, one pass ---------------> next step
 //   stream s2 (frame):  A (tendencies, frame band) -> X (deep halo exchange) -> D (friction, frame + ext)
 //
-// S writes only bulk cells, A / X / D own the frame.  h, u, v, du and dv are ping-pong pairs: every
-// kernel reads this step's buffers and writes the next step's, and dh is updated cell by cell by the
-// kernel that owns the cell.  So the streams meet only at the step boundary: S(t+1) reads what D(t)
+// S writes only bulk cells, A / X / D own the frame.  Every kernel reads this step's buffer set and
+// writes the next step's.  So the streams meet only at the step boundary: S(t+1) reads what D(t)
 // wrote next to the bulk, A(t+1) what S(t) wrote next to the frame.  Seven arrays are read once and
 // written once per step (12 array passes instead of the stand-alone path's 32; at 8 GPUs, 2 M cells
 // per rank, the step's working set is larger than the 50 MB L2 of an H100, so passes are HBM traffic),
-// one exchange instead of three, and the NVLink round of X is hidden behind S.  Under CUDA-graph
+// one exchange instead of three, and the NVLink round of X is hidden behind S.  Pairs of steps advance
+// the bulk twice per pass (S2, see b2_swe_multistep_ca).  Under CUDA-graph
 // capture (mpi4jax_b200.jit) the event fork / join becomes graph edges.
 
 #include "b2_device.cuh"
@@ -123,6 +123,7 @@ __global__ void __launch_bounds__(CA_THREADS) swe_ca_init_ext(const B2SweParams 
 }
 
 // ---- S: the bulk, one pass per step (b2_swe_ca_bulk.cuh) ----------------------------------------
+// Also the ring launch of the pair schedule: the same kernel over narrower store windows.
 __global__ void __launch_bounds__(CA_BULK_WARPS * 32)
 swe_ca_bulk_step(const CABulkArgs a, const CAStamp ts) {
   ca_stamp_begin(ts);
@@ -138,6 +139,74 @@ swe_ca_bulk_step(const CABulkArgs a, const CAStamp ts) {
       const float uw2 = __shfl_up_sync(0xffffffffu, L.upn[2], 1), uw3 = __shfl_up_sync(0xffffffffu, L.upn[3], 1);
       const float ue = __shfl_down_sync(0xffffffffu, L.upn[0], 1), ve = __shfl_down_sync(0xffffffffu, L.vpn[0], 1);
       ca_bulk_fric(a, L, t, uw2, uw3, ue, ve, t == s, t > s);
+    }
+  }
+  ca_stamp_end(ts);
+}
+
+// ---- S2: two steps of the bulk in one pass (b2_swe_ca_bulk.cuh) ---------------------------------
+// A PAIR of warps owns a strip of the inner bulk (`b`: rows [8, ny-7) x groups [1, ng-1)) and a segment
+// of its rows [s, e).  The step-1 warp walks rows [s-4, e+3) of step t exactly as swe_ca_bulk_step does
+// (`a`: state t in, state t+1 out) and puts its rows of state t+1 into the pair's shared-memory row
+// ring; the step-2 warp walks rows [s, e) of step t+1 four rows behind it, reading state t+1 from the
+// ring and writing state t+2.  One step's dependency cone is 4 rows south (row s-4 feeds the fluxes of
+// row s-2), 3 north (row e+2 feeds the u' of row e) and 3 columns (one lane either side, each of which
+// needs its own neighbour lanes for the friction), so step 2 needs nothing the frame kernels write.
+//
+// Lanes: step-1 friction is valid on lanes 1..30 (lanes 0, 31 lack a neighbour's u'); step-2 reads
+// the ring columns of its lane and both neighbour lanes, so its tendency is valid on lanes 2..29 and its
+// friction on 3..28: a strip stores 26 groups (`halo` 3).
+// Lockstep: round k runs step-1 row k and step-2 row k-4, then the pair meets at a named barrier.  Row
+// k-4 of step 2 needs rows up to k-1 of step 1 (its tendency reads row k-2, whose u'' is finished by
+// step-1 row k-1); in round k step 2 reads ring rows k-5 .. k-2 and step 1 writes rows k-1, k, so eight
+// ring slots leave every row in place until it has been read.
+// Step 1 also stores state t+1 to the arrays where the ring launch and the frame kernels of step t+1
+// read it (ca_pair_band).
+#define CA_PAIR_WARPS 4              // warps per CTA: two pairs
+#define CA_PAIR_CTAS 3               // CTAs per SM: 6 pairs, 3 x 2 rings of shared memory
+#define CA_PAIR_SMEM (2 * CA_RING_FLOATS * (int)sizeof(float))
+__global__ void __launch_bounds__(CA_PAIR_WARPS * 32, CA_PAIR_CTAS)
+swe_ca_bulk_pair(const CABulkArgs a, const CABulkArgs b, const CAStamp ts) {
+  ca_stamp_begin(ts);
+  extern __shared__ float4 ca_ring_mem[];
+  const int pair = (int)(threadIdx.x >> 6), lane = threadIdx.x & 31;
+  const bool second = (threadIdx.x >> 5) & 1;
+  float* const ring = reinterpret_cast<float*>(ca_ring_mem) + pair * CA_RING_FLOATS;
+  const int w = (int)blockIdx.x * (CA_PAIR_WARPS / 2) + pair;
+  if (w < ca_bulk_warps(b)) {                          // (whole pairs: both warps meet at every barrier)
+    const int seg = w / b.wcols, wc = w % b.wcols;
+    int s, e;
+    ca_bulk_rows(b, seg, s, e);
+    CABulkLane L;
+    const bool own = ca_bulk_lane(b, wc, lane, L.i0);
+    L.ic = 4 + 4 * lane;
+    const int s1 = s - 4, e1 = e + 3;
+    if (!second) {
+      const CAPairBand band = ca_pair_band(b, seg, wc, lane, own, L);
+      ca_bulk_begin(a, L, s1);
+      for (int k = s1 - 2; k <= e + 4; ++k) {
+        if (k <= e1) {
+          ca_bulk_tend<false, true>(a, L, k, k >= s1 && k < e1, ring, ca_pair_hbm(band, a.p.ny, k));
+          const float uw2 = __shfl_up_sync(0xffffffffu, L.upn[2], 1), uw3 = __shfl_up_sync(0xffffffffu, L.upn[3], 1);
+          const float ue = __shfl_down_sync(0xffffffffu, L.upn[0], 1), ve = __shfl_down_sync(0xffffffffu, L.vpn[0], 1);
+          ca_bulk_fric<true>(a, L, k, uw2, uw3, ue, ve, k == s1, k > s1, ring, ca_pair_hbm(band, a.p.ny, k - 1));
+        }
+        asm volatile("bar.sync %0, 64;" ::"r"(1 + pair) : "memory");
+      }
+    } else {
+      L.store = own;
+      for (int k = s1 - 2; k <= e + 4; ++k) {
+        const int t = k - 4;
+        if (k == s + 1) {
+          ca_bulk_begin<true>(b, L, s, ring);
+        } else if (t >= s - 2) {
+          ca_bulk_tend<true, false>(b, L, t, t >= s && t < e, ring);
+          const float uw2 = __shfl_up_sync(0xffffffffu, L.upn[2], 1), uw3 = __shfl_up_sync(0xffffffffu, L.upn[3], 1);
+          const float ue = __shfl_down_sync(0xffffffffu, L.upn[0], 1), ve = __shfl_down_sync(0xffffffffu, L.vpn[0], 1);
+          ca_bulk_fric(b, L, t, uw2, uw3, ue, ve, t == s, t > s);
+        }
+        asm volatile("bar.sync %0, 64;" ::"r"(1 + pair) : "memory");
+      }
     }
   }
   ca_stamp_end(ts);
@@ -246,25 +315,20 @@ static CAStamp ca_slot(int step, int kernel) {
   return s;
 }
 
-// Rows per segment of the bulk kernel: about two waves of warps on this GPU, so that the frame chain's
-// CTAs find free slots while the bulk runs, and at least 16 rows (a segment evaluates the tendencies of
-// three rows beyond its own).
-static int ca_bulk_rows_per_segment(const B2SweParams& p, int cb1) {
-  static int slot_warps = 0;
-  if (slot_warps == 0) {
-    int dev = 0, sms = 0, per_sm = 0;
-    cudaGetDevice(&dev);
-    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-    cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, swe_ca_bulk_step, CA_BULK_WARPS * 32, 0);
-    slot_warps = sms * per_sm * CA_BULK_WARPS;
-    if (slot_warps <= 0) slot_warps = 132 * 16;
-  }
-  CABulkArgs g;
-  g.p = p;
-  ca_bulk_geometry(p, cb1, 1, g);
-  const int nseg = (2 * slot_warps) / g.wcols > 1 ? (2 * slot_warps) / g.wcols : 1;
-  const int rows = (p.ny - 8 + nseg - 1) / nseg;
+// Rows per segment of a bulk launch: about two waves of warps (pairs) on this GPU, so that the frame
+// chain's CTAs find free slots while the bulk runs, and at least 16 rows (a segment evaluates the
+// tendencies of three rows beyond its own, the pair kernel's step 1 of seven).
+static int ca_rows_per_segment(int slots, int wcols, int rows_total) {
+  const int nseg = (2 * slots) / wcols > 1 ? (2 * slots) / wcols : 1;
+  const int rows = (rows_total + nseg - 1) / nseg;
   return rows < 16 ? 16 : rows;
+}
+static int ca_slots(const void* kernel, int threads, int smem, int per_cta) {
+  int dev = 0, sms = 0, per_sm = 0;
+  cudaGetDevice(&dev);
+  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+  cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, threads, smem);
+  return sms * per_sm * per_cta > 0 ? sms * per_sm * per_cta : 132 * per_cta;
 }
 
 static int ca_exchange(B2Comm* c, const B2HaloDesc& topo, const B2SweParams& p, const B2SweCA& x, float* f0,
@@ -318,6 +382,21 @@ int b2_swe_ca_init(B2Comm* c, const B2SweParams* p0, const B2SweState* st, const
   return b2_launched(c, "swe_ca_init_ext");
 }
 
+// Schedule.  A step is the bulk kernel S on stream s next to the frame chain A -> X -> D on stream s2.
+// Pairs of steps (t, t+1) after the first (Euler) step advance the bulk twice per pass over the arrays:
+//
+//   s :  S2 (step t on the bulk, t+1 on the inner bulk) ------------> ring (t+1) ----------> next
+//   s2:  A X D (t) ----------------------------------------------> A X D (t+1) ------------> next
+//                                   (ring waits for D (t), A X D (t+1) for S2)
+//
+// The ring launches are swe_ca_bulk_step on the four windows around the inner bulk: rows [4, 8) and
+// [ny-7, ny-4), groups 0 and ng-1 between them; they are the only part of step t+1 that needs the frame's
+// state t+1.  An odd step left over runs the one-step schedule.  h, u, v, du and dv rotate through three
+// buffer sets: a step reads one and writes another; S2 reads set c (state t), stores the band of state
+// t+1 into set n, where A X D (t) write the frame's, and state t+2 into set m (a segment's step 1 reads
+// rows that a neighbouring segment's step 2 overwrites, so ping-pong is not enough).  dh stays in place
+// through a one-step launch and moves to another of its three buffers with a pair, for the same reason.
+// Each launch picks its output sets so that the call ends in the home buffers (`target`).
 int b2_swe_multistep_ca(B2Comm* c, const B2SweParams* p0, const B2SweState* st, const B2SweCA* x0,
                         const B2HaloDesc* topo, int nsteps, int first_step, cudaStream_t s) {
   // blocks too small for the bulk / frame split, or no friction step: the stand-alone kernels
@@ -330,67 +409,137 @@ int b2_swe_multistep_ca(B2Comm* c, const B2SweParams* p0, const B2SweState* st, 
   if (int rc = ca_streams()) return rc;
   const cudaStream_t s2 = g_side;
   const cudaEvent_t e0 = g_ev[0], eS = g_ev[1], eD = g_ev[2];
-  // ping-pong pairs: [cur] = this step's, [nxt] = the next step's; the flux arrays of the stand-alone
-  // path are free here: fe / fn hold u', v' of the frame band between kernels A, X and D
-  float* H[2] = {st->h0, st->h1};
-  float* U[2] = {st->u, st->u1};
-  float* V[2] = {st->v, st->v1};
-  float* DU[2] = {st->du, st->du1};
-  float* DV[2] = {st->dv, st->dv1};
+  // [k] = buffer set k; the flux arrays of the stand-alone path are free here: fe / fn hold u', v' of
+  // the frame band between kernels A, X and D
+  float* const H[3] = {st->h0, st->h1, st->h2};
+  float* const U[3] = {st->u, st->u1, st->u2};
+  float* const V[3] = {st->v, st->v1, st->v2};
+  float* const DU[3] = {st->du, st->du1, st->du2};
+  float* const DV[3] = {st->dv, st->dv1, st->dv2};
+  float* const DH[3] = {st->dh, st->dh1, st->dh2};
   float* const upf = st->fe;
   float* const vpf = st->fn;
-  CABulkArgs sa;
-  sa.p = p;
-  ca_bulk_geometry(p, x.cb1, ca_bulk_rows_per_segment(p, x.cb1), sa);
-  const unsigned bulk_blocks = ca_blocks(ca_bulk_warps(sa), CA_BULK_WARPS);
+  static int slot_warps = 0, slot_pairs = 0;
+  if (slot_warps == 0) {
+    if (int rc = b2_cuda_check(cudaFuncSetAttribute(swe_ca_bulk_pair, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                                    CA_PAIR_SMEM), "swe_multistep_ca: shared memory of the pair kernel"))
+      return rc;
+    slot_warps = ca_slots((const void*)swe_ca_bulk_step, CA_BULK_WARPS * 32, 0, CA_BULK_WARPS);
+    slot_pairs = ca_slots((const void*)swe_ca_bulk_pair, CA_PAIR_WARPS * 32, CA_PAIR_SMEM, CA_PAIR_WARPS / 2);
+  }
+  const int ng = (x.cb1 >> 2) - 1, ny = p.ny;
+  CABulkArgs sa = {};                                   // one step, whole bulk
+  ca_bulk_geometry(p, x.cb1, 1, sa);
+  ca_bulk_geometry(p, x.cb1, ca_rows_per_segment(slot_warps, sa.wcols, ny - 8), sa);
+  // pairs: S2's inner bulk (step 1 walks its segments), the ring's four windows; two rows per segment
+  // there: the ring launches are exposed and move little data, so a warp's walk (its rows + 3 tendency
+  // rows, each a round trip to HBM) is kept short
+  const bool pairs = ny - 7 > 8 && ng >= 3;
+  CABulkArgs pa = {}, pb = {}, ring[4] = {};
+  if (pairs) {
+    ca_bulk_window(x.cb1, 8, ny - 7, 1, ng - 1, 3, 1, pb);
+    ca_bulk_window(x.cb1, 8, ny - 7, 1, ng - 1, 3, ca_rows_per_segment(slot_pairs, pb.wcols, ny - 15), pb);
+    pa.ng = pb.ng;
+    ca_bulk_window(x.cb1, 4, 8, 0, ng, 1, 2, ring[0]);
+    ca_bulk_window(x.cb1, ny - 7, ny - 4, 0, ng, 1, 2, ring[1]);
+    ca_bulk_window(x.cb1, 8, ny - 7, 0, 1, 1, 2, ring[2]);
+    ca_bulk_window(x.cb1, 8, ny - 7, ng - 1, ng, 1, 2, ring[3]);
+  }
   const CAFrame fa = ca_frame(p, 5, x.cb1 - 2), fd = ca_frame(p, 3, x.cb1);
   const unsigned tend_blocks = ca_blocks(fa.total, CA_CELLS);
   const unsigned fric_blocks = ca_blocks(fd.total + ca_ext_total(p), CA_CELLS);
   int rc = 0;
 #define CA_RT(call) \
   if (rc == 0) rc = b2_cuda_check((call), "swe_multistep_ca: %s failed", #call);
+  // sets `in` -> `out`; dh from dh_in (null: in place) to dh_out
+  auto io = [&](CABulkArgs& a, int in, int out, const float* dh_in, float* dh_out) {
+    a.p = p;
+    a.h = H[in]; a.u = U[in]; a.v = V[in]; a.du = DU[in]; a.dv = DV[in];
+    a.h_o = H[out]; a.u_o = U[out]; a.v_o = V[out]; a.du_o = DU[out]; a.dv_o = DV[out];
+    a.dh = dh_out; a.dh_src = dh_in;
+  };
+  auto frame = [&](int it, int in, int out, const float* dh_in, float* dh_out) -> int {
+    CACtx ctx;
+    ctx.p = p; ctx.x = x;
+    ctx.h = H[in]; ctx.hn = H[out];
+    ctx.ua = U[in]; ctx.va = V[in];
+    ctx.dh = dh_out; ctx.dh_src = dh_in;
+    ctx.du = DU[in]; ctx.dv = DV[in];
+    ctx.du_o = DU[out]; ctx.dv_o = DV[out];
+    ctx.upf = upf; ctx.vpf = vpf;
+    swe_ca_tend_frame<<<tend_blocks, CA_CELLS * CA_TEND_WARPS, 0, s2>>>(ctx, fa, ca_slot(it, 0));
+    if (int r = b2_launched(c, "swe_ca_tend_frame")) return r;
+    if (int r = ca_exchange(c, *topo, p, x, H[out], upf, vpf, s2, ca_slot(it, 2))) return r;
+    swe_ca_fric_frame<<<fric_blocks, CA_CELLS * 3, 0, s2>>>(ctx, fd, U[out], V[out], ca_slot(it, 3));
+    if (int r = b2_launched(c, "swe_ca_fric_frame")) return r;
+    return b2_cuda_check(cudaEventRecord(eD, s2), "swe_multistep_ca: cudaEventRecord failed");
+  };
+  // h .. dv move to another set with every one-step or pair launch, dh with every pair launch; the last
+  // move goes to the home set and the one before it elsewhere, so only a call of a single move (of dh:
+  // a single pair) ends with copies
+  const int lead = (first_step && nsteps > 0) ? 1 : 0;
+  const int npairs = pairs ? (nsteps - lead) / 2 : 0;
+  const int moves = nsteps - npairs;
+  auto target = [](int mv, int n, int cur) {
+    if (mv == n - 1 && cur != 0) return 0;
+    return mv == n - 2 ? (cur == 1 ? 2 : 1) : (cur + 1) % 3;
+  };
   CA_RT(cudaEventRecord(e0, s));
   CA_RT(cudaStreamWaitEvent(s2, e0, 0));
-  int cur = 0;
-  for (int it = 0; it < nsteps && rc == 0; ++it) {
-    const int nxt = cur ^ 1;
+  int cur = 0, dc = 0;
+  for (int it = 0, mv = 0, pv = 0; it < nsteps && rc == 0; ++mv) {
     p.first_step = (first_step && it == 0) ? 1 : 0;
-    // ---- frame stream: needs the bulk kernel of the previous step (u'', v'', h next to the frame);
+    const bool pair = pairs && !p.first_step && nsteps - it >= 2;
+    // single step: cur -> nxt; pair: cur -> nxt (band of step t+1, frame) -> third
+    const int third = target(mv, moves, cur), nxt = pair ? 3 - cur - third : third;
+    // ---- frame stream: needs the bulk launches of the previous step (state next to the frame);
     // enqueued before this step's bulk kernel re-records eS
     if (it > 0) CA_RT(cudaStreamWaitEvent(s2, eS, 0));
     // ---- bulk stream: needs D of the previous step (u'', v'' of the frame, the arrays' halos)
     if (it > 0) CA_RT(cudaStreamWaitEvent(s, eD, 0));
     if (rc) break;
-    sa.p = p;
-    sa.h = H[cur]; sa.u = U[cur]; sa.v = V[cur]; sa.du = DU[cur]; sa.dv = DV[cur];
-    sa.h_o = H[nxt]; sa.u_o = U[nxt]; sa.v_o = V[nxt]; sa.du_o = DU[nxt]; sa.dv_o = DV[nxt];
-    sa.dh = st->dh;
-    swe_ca_bulk_step<<<bulk_blocks, CA_BULK_WARPS * 32, 0, s>>>(sa, ca_slot(it, 1));
-    if ((rc = b2_launched(c, "swe_ca_bulk_step"))) break;
+    if (!pair) {
+      io(sa, cur, nxt, nullptr, DH[dc]);
+      swe_ca_bulk_step<<<ca_blocks(ca_bulk_warps(sa), CA_BULK_WARPS), CA_BULK_WARPS * 32, 0, s>>>(sa, ca_slot(it, 1));
+      if ((rc = b2_launched(c, "swe_ca_bulk_step"))) break;
+      CA_RT(cudaEventRecord(eS, s));
+      if (rc || (rc = frame(it, cur, nxt, nullptr, DH[dc]))) break;
+      cur = nxt;
+      ++it;
+      continue;
+    }
+    const int dm = target(pv++, npairs, dc), dn = 3 - dc - dm;
+    io(pa, cur, nxt, DH[dc], DH[dn]);
+    io(pb, nxt, third, nullptr, DH[dm]);
+    swe_ca_bulk_pair<<<ca_blocks(ca_bulk_warps(pb), CA_PAIR_WARPS / 2), CA_PAIR_WARPS * 32, CA_PAIR_SMEM, s>>>(
+        pa, pb, ca_slot(it, 1));
+    if ((rc = b2_launched(c, "swe_ca_bulk_pair"))) break;
     CA_RT(cudaEventRecord(eS, s));
-    CACtx ctx;
-    ctx.p = p; ctx.x = x;
-    ctx.h = H[cur]; ctx.hn = H[nxt];
-    ctx.ua = U[cur]; ctx.va = V[cur];
-    ctx.dh = st->dh; ctx.du = DU[cur]; ctx.dv = DV[cur];
-    ctx.du_o = DU[nxt]; ctx.dv_o = DV[nxt];
-    ctx.upf = upf; ctx.vpf = vpf;
-    swe_ca_tend_frame<<<tend_blocks, CA_CELLS * CA_TEND_WARPS, 0, s2>>>(ctx, fa, ca_slot(it, 0));
-    if ((rc = b2_launched(c, "swe_ca_tend_frame"))) break;
-    if ((rc = ca_exchange(c, *topo, p, x, H[nxt], upf, vpf, s2, ca_slot(it, 2)))) break;
-    swe_ca_fric_frame<<<fric_blocks, CA_CELLS * 3, 0, s2>>>(ctx, fd, U[nxt], V[nxt], ca_slot(it, 3));
-    if ((rc = b2_launched(c, "swe_ca_fric_frame"))) break;
-    CA_RT(cudaEventRecord(eD, s2));
-    cur = nxt;
+    if (rc || (rc = frame(it, cur, nxt, DH[dc], DH[dn]))) break;
+    // ring (t+1): needs D (t); A X D (t+1): needs S2 (eS, recorded before the ring re-records it)
+    CA_RT(cudaStreamWaitEvent(s, eD, 0));
+    CA_RT(cudaStreamWaitEvent(s2, eS, 0));
+    for (int k = 0; k < 4 && rc == 0; ++k) {
+      io(ring[k], nxt, third, DH[dn], DH[dm]);
+      swe_ca_bulk_step<<<ca_blocks(ca_bulk_warps(ring[k]), CA_BULK_WARPS), CA_BULK_WARPS * 32, 0, s>>>(
+          ring[k], ca_slot(it + 1, 1));
+      rc = b2_launched(c, "swe_ca_bulk_step");
+    }
+    if (rc || (rc = frame(it + 1, nxt, third, DH[dn], DH[dm]))) break;
+    CA_RT(cudaEventRecord(eS, s));
+    cur = third;
+    dc = dm;
+    it += 2;
   }
   CA_RT(cudaStreamWaitEvent(s, eD, 0));           // join (also required to end a stream capture)
-  // odd step count: the state goes back to its home buffers
+  // the state goes back to its home buffers
   const size_t bytes = (size_t)p.ny * p.pitch * sizeof(float);
-  if (cur != 0)
-    for (int k = 0; k < 5 && rc == 0; ++k) {
-      float* const pair[5][2] = {{H[0], H[1]}, {U[0], U[1]}, {V[0], V[1]}, {DU[0], DU[1]}, {DV[0], DV[1]}};
-      CA_RT(cudaMemcpyAsync(pair[k][0], pair[k][1], bytes, cudaMemcpyDeviceToDevice, s));
-    }
+  if (cur != 0) {
+    float* const* set[5] = {H, U, V, DU, DV};
+    for (int k = 0; k < 5 && rc == 0; ++k)
+      CA_RT(cudaMemcpyAsync(set[k][0], set[k][cur], bytes, cudaMemcpyDeviceToDevice, s));
+  }
+  if (dc != 0) CA_RT(cudaMemcpyAsync(DH[0], DH[dc], bytes, cudaMemcpyDeviceToDevice, s));
 #undef CA_RT
   return rc;
 }

@@ -28,7 +28,9 @@
 // (tests/test_swe_host_emulation.py runs both on 1x1 .. 2x4 process grids).
 //
 // Storage.  The main (ny, pitch) arrays keep their meaning (1-cell halo; u, v halos stale).  h, u, v,
-// du and dv are ping-pong pairs: every kernel of a step reads one buffer and writes the other.
+// du and dv come in three buffer sets: every kernel of a step reads one set and writes another
+// (b2_swe_ca.cu: two sets per step, the third for the pair schedule that advances the bulk two steps).
+// dh is updated in place by a one-step schedule and moves between three buffers with a pair of steps.
 // Five "ext" arrays [(ny + 4) x epitch], cell (j, i) at (j + 2) * epitch + (i + 2), hold what
 // lies beyond: hx (h, layers 1..2), upx / vpx (u', v': layers 1..3 and a mirror of this rank's
 // own ring cells, i.e. every STALE value a view can ask for), uppx / vppx (u'', v'' of the
@@ -53,9 +55,10 @@ struct CACtx {
   float *hn;                      // h' (ping-pong partner of h)
   const float *ua, *va;           // u'', v'' of the previous step (interior; wall rows constant); kernel D
                                   // writes this step's into the partners
-  float *dh;                      // read (previous step) and written (this step) cell by cell
+  float *dh;                      // the next step's dh (frame cells)
+  const float *dh_src = nullptr;  // this step's dh; null: dh, updated cell by cell in place
   const float *du, *dv;           // du, dv of this step (the previous step's tendencies)
-  float *du_o, *dv_o;             // their ping-pong partners: the bulk kernel reads du, dv while kernel A runs
+  float *du_o, *dv_o;             // their partners: the bulk kernel reads du, dv while kernel A runs
   float *upf, *vpf;               // u', v' of the frame band (cells within 5 of the edge) and, after X, their halo
 };
 
@@ -225,8 +228,8 @@ __device__ __forceinline__ void swe_ca_tend_finish(const CACtx& c, int j, int i,
   in.h_c = c.h[off]; in.h_e = ca_h(c, j, i + 1); in.h_n = ca_h(c, j + 1, i);
   in.u_o = c.ua[off]; in.v_o = c.va[off];
   const bool frame = ca_is_frame(p, c.x.cb1, j, i);
-  // not read for a band-only cell: the bulk kernel updates that cell's dh in place meanwhile
-  in.dh_o = (p.first_step || !frame) ? 0.f : c.dh[off];
+  // (a band-only cell's h' and dh are the bulk kernel's: its old dh is not needed)
+  in.dh_o = (p.first_step || !frame) ? 0.f : (c.dh_src != nullptr ? c.dh_src : c.dh)[off];
   in.du_o = p.first_step ? 0.f : c.du[off];
   in.dv_o = p.first_step ? 0.f : c.dv[off];
   SweK2Out o = swe_k2_cell(p, in);

@@ -14,10 +14,12 @@
 // The u' a lane needs beyond its own four columns (two to the west, one to the east) come from its
 // neighbour lanes, so lanes 0 and 31 only supply them: a warp stores 30 groups.  A segment also
 // evaluates u', v' of the two rows above and the one row below it (and, at the bulk's edge, of the band
-// cells at distance 2 and 3): nothing it reads is written by another warp in the same step, because u,
-// v, du and dv are ping-pong pairs (the segment reads this step's arrays and writes the partners).  dh
-// is updated in place: a cell's new dh is needed only where the cell's h' is stored, and only the
-// owning lane reads it.
+// cells at distance 2 and 3): nothing it reads is written by another warp in the same step, because the
+// segment reads this step's buffer set and writes another.
+//
+// The same functions serve the pair kernel (swe_ca_bulk_pair, b2_swe_ca.cu), whose step-2 warp reads its
+// rows from the step-1 warp's shared-memory ring instead of the arrays: the row addressing is a template
+// parameter (IN_RING / OUT_RING), the arithmetic is the same code.
 //
 // Bit-compatibility with the stand-alone kernels: the quantities are the shared explicit-rounding
 // helpers of b2_swe_body.cuh (swe_fe .. swe_ke, swe_k2_cell, swe_friction_u, swe_visc_flux,
@@ -29,7 +31,6 @@
 #include "b2_swe_body.cuh"
 
 #define CA_BULK_WARPS 4              // warps per CTA (independent: no shared memory, no barrier)
-#define CA_BULK_LANES 30             // groups a warp stores; lanes 0 and 31 supply their neighbours' u', v'
 
 // Row of six with index d + 1 for column offset d = -1 .. 4 relative to the group start.
 struct Row6A {
@@ -42,32 +43,54 @@ __device__ __forceinline__ Row6A ld_row_a(const float* __restrict__ x, int j, in
   return o;
 }
 
+// The pair kernel's shared-memory row ring (swe_ca_bulk_pair, b2_swe_ca.cu): the step-1 warp's rows of
+// h, u, v, dh, du, dv, CA_RING_SLOTS rows per field, row j in slot j % CA_RING_SLOTS.  A ring row is the
+// warp strip's 128 columns with 4 floats of padding on each side (lane l's group at 4 + 4 l), so that the
+// west / east neighbours of lanes 0 and 31 are addressable.
+#define CA_RING_SLOTS 8
+#define CA_RING_PITCH 136
+#define CA_RING_FIELD (CA_RING_SLOTS * CA_RING_PITCH)
+#define CA_RING_FLOATS (6 * CA_RING_FIELD)
+enum { CA_RH = 0, CA_RU, CA_RV, CA_RDH, CA_RDU, CA_RDV };
+
 struct CABulkArgs {
   B2SweParams p;
   int ng;                                            // bulk groups per row: columns [4, 4 + 4 ng)
+  int r0, r1, g0, g1;                                // store window: rows [r0, r1) x groups [g0, g1)
+  int halo;                                          // lanes on each side of a strip that do not store
   int rows;                                          // rows per segment
   int wcols;                                         // warp strips per row of segments
-  int nseg;                                          // segments: bulk rows [4, ny - 4)
+  int nseg;                                          // segments: window rows [r0, r1)
   const float *h, *u, *v, *du, *dv;                  // this step
-  float *h_o, *u_o, *v_o, *du_o, *dv_o;              // the next step (ping-pong partners)
-  float* dh;                                         // read, then updated in place (own cell only)
+  float *h_o, *u_o, *v_o, *du_o, *dv_o;              // the next step
+  float* dh;                                         // the next step's dh (own cells only)
+  const float* dh_src = nullptr;                     // this step's dh; null: dh, updated in place
 };
 
-// geometry of the launch: a warp's (segment, strip), a lane's group
-__host__ __device__ inline void ca_bulk_geometry(const B2SweParams& p, int cb1, int rows, CABulkArgs& a) {
+// geometry of a launch over the window [r0, r1) x [g0, g1): a warp's (segment, strip), a lane's group.
+// The one-step kernel over the whole bulk is the window [4, ny - 4) x [0, ng) with halo 1.
+__host__ __device__ inline void ca_bulk_window(int cb1, int r0, int r1, int g0, int g1, int halo, int rows,
+                                               CABulkArgs& a) {
   a.ng = (cb1 >> 2) - 1;
+  a.r0 = r0; a.r1 = r1; a.g0 = g0; a.g1 = g1; a.halo = halo;
   a.rows = rows;
-  a.wcols = (a.ng + CA_BULK_LANES - 1) / CA_BULK_LANES;
-  a.nseg = (p.ny - 8 + rows - 1) / rows;
+  a.wcols = (g1 - g0 + 32 - 2 * halo - 1) / (32 - 2 * halo);
+  a.nseg = (r1 - r0 + rows - 1) / rows;
+}
+__host__ __device__ inline void ca_bulk_geometry(const B2SweParams& p, int cb1, int rows, CABulkArgs& a) {
+  ca_bulk_window(cb1, 4, p.ny - 4, 0, (cb1 >> 2) - 1, 1, rows, a);
 }
 __host__ __device__ inline long long ca_bulk_warps(const CABulkArgs& a) { return (long long)a.wcols * a.nseg; }
-// group index of `lane` in strip `wc` (-1 = the group west of the bulk, ng = the one east of it;
-// lanes beyond that repeat it); the lane stores when it returns true
+// group index of `lane` in strip `wc`; lanes beyond the groups the window's stored lanes need repeat the
+// last of them (at most ng, the group east of the bulk), so a narrow window loads few distinct columns;
+// the lane stores when it returns true
 __host__ __device__ inline bool ca_bulk_lane(const CABulkArgs& a, int wc, int lane, int& i0) {
-  int g = wc * CA_BULK_LANES + lane - 1;
-  if (g > a.ng) g = a.ng;
+  int g = a.g0 + wc * (32 - 2 * a.halo) + lane - a.halo;
+  const int ghi = a.g1 + a.halo - 1 < a.ng ? a.g1 + a.halo - 1 : a.ng;
+  if (g > ghi) g = ghi;
+  if (g < -1) g = -1;
   i0 = 4 + 4 * g;
-  return lane >= 1 && lane <= CA_BULK_LANES && g < a.ng;
+  return lane >= a.halo && lane < 32 - a.halo && g < a.g1;
 }
 
 // the four flux quantities of row k from rows k-1 (v only), k and k+1 (swe_k1_body's expressions)
@@ -91,7 +114,8 @@ __device__ __forceinline__ void ca_bulk_fluxes(const B2SweParams& p, float cor, 
 // everything a lane carries from one row to the next
 struct CABulkLane {
   int i0;
-  bool store;                                        // this lane's group is a bulk group
+  int ic;                                            // the lane's group in a ring row (pair kernel)
+  bool store;                                        // this lane's group is stored to the arrays
   Row6A H[3], U[3], V[3];                            // rows t, t+1 and (loaded ahead) t+2
   CAFluxRow Fm, Fc;                                  // fluxes of rows t-1, t
   float4 dh4, du4, dv4;                              // old tendencies of row t
@@ -104,17 +128,75 @@ struct CABulkLane {
 // rows [s, e) of segment `seg`; its tendency rows are s-2 .. e (rows s-2, s-1 and e only feed the
 // friction of rows s .. e-1)
 __host__ __device__ inline void ca_bulk_rows(const CABulkArgs& a, int seg, int& s, int& e) {
-  s = 4 + seg * a.rows;
-  e = s + a.rows < a.p.ny - 4 ? s + a.rows : a.p.ny - 4;
+  s = a.r0 + seg * a.rows;
+  e = s + a.rows < a.r1 ? s + a.rows : a.r1;
+}
+
+// The pair kernel's step-1 lane (segment `seg`, strip `wc` of the inner bulk `b`) also stores state t+1
+// to the arrays where the ring launch and the frame kernels of step t+1 read it: rows < 10 and >= ny-11
+// (the ring launch's row windows [4, 8) and [ny-7, ny-4) reach 2 rows north, 4 south) and groups 0, 1,
+// ng-2, ng-1 (the side windows' groups and their neighbours).  Each such cell is stored by one lane: the
+// owner of its row and group under step 2's partition, extended to rows [4, 8) for the first segment, to
+// rows [ny-7, ny-4) for the last, and to groups 0 and ng-1 for the outer strips.  Sets L.store.
+struct CAPairBand {
+  bool band_g;                                       // the lane's group is a band group
+  int lo, hi;                                        // rows the lane owns
+};
+__host__ __device__ inline CAPairBand ca_pair_band(const CABulkArgs& b, int seg, int wc, int lane, bool own,
+                                                   CABulkLane& L) {
+  const int g = (L.i0 - 4) >> 2;
+  L.store = own || (g == 0 && wc == 0 && lane == 2) || (g == b.g1 && wc == b.wcols - 1);
+  int s, e;
+  ca_bulk_rows(b, seg, s, e);
+  CAPairBand r;
+  r.band_g = g < 2 || g >= b.ng - 2;
+  r.lo = seg == 0 ? s - 4 : s;
+  r.hi = seg == b.nseg - 1 ? e + 3 : e;
+  return r;
+}
+__host__ __device__ __forceinline__ bool ca_pair_hbm(const CAPairBand& B, int ny, int r) {
+  return r >= B.lo && r < B.hi && (B.band_g || r < 10 || r >= ny - 11);
+}
+
+// Row j of an input field: from the (ny, pitch) array `x` or (RING) from field `f` of the ring.
+__host__ __device__ __forceinline__ int ca_ring_off(const CABulkLane& L, int f, int j) {
+  return f * CA_RING_FIELD + (j & (CA_RING_SLOTS - 1)) * CA_RING_PITCH + L.ic;
+}
+template <bool RING>
+__device__ __forceinline__ Row6A ca_ld_row(const CABulkArgs& a, const CABulkLane& L, const float* x,
+                                           const float* ring, int f, int j) {
+  if (!RING) return ld_row_a(x, j, L.i0, a.p.pitch);
+  const int o = ca_ring_off(L, f, j);
+  const float4 c = ld4(ring, o);
+  Row6A r;
+  r.a[0] = ring[o - 1]; r.a[1] = c.x; r.a[2] = c.y; r.a[3] = c.z; r.a[4] = c.w; r.a[5] = ring[o + 4];
+  return r;
+}
+// (`off`: the lane's group in row j of the arrays)
+template <bool RING>
+__device__ __forceinline__ float4 ca_ld4(const CABulkLane& L, const float* x, size_t off, const float* ring, int f,
+                                         int j) {
+  return RING ? ld4(ring, ca_ring_off(L, f, j)) : ld4(x, off);
+}
+// Row j of an output field: to the array `x` where `hbm` (and the lane stores), and (RING) to the ring.
+template <bool RING>
+__device__ __forceinline__ void ca_st4(const CABulkLane& L, float* x, size_t off, float* ring, int f, int j,
+                                       bool hbm, float4 v) {
+  if (RING) st4(ring, ca_ring_off(L, f, j), v);
+  if (hbm && L.store) st4(x, off, v);
 }
 
 // rows s-4 .. s-1 and the fluxes of rows s-3, s-2 of the segment starting at row s
-__device__ __forceinline__ void ca_bulk_begin(const CABulkArgs& a, CABulkLane& L, int s) {
-  const int P = a.p.pitch, t = s - 2;
-  const Row6A Vs = ld_row_a(a.v, t - 2, L.i0, P);
-  L.H[0] = ld_row_a(a.h, t - 1, L.i0, P); L.U[0] = ld_row_a(a.u, t - 1, L.i0, P); L.V[0] = ld_row_a(a.v, t - 1, L.i0, P);
-  L.H[1] = ld_row_a(a.h, t, L.i0, P); L.U[1] = ld_row_a(a.u, t, L.i0, P); L.V[1] = ld_row_a(a.v, t, L.i0, P);
-  L.H[2] = ld_row_a(a.h, t + 1, L.i0, P); L.U[2] = ld_row_a(a.u, t + 1, L.i0, P); L.V[2] = ld_row_a(a.v, t + 1, L.i0, P);
+template <bool IN_RING = false>
+__device__ __forceinline__ void ca_bulk_begin(const CABulkArgs& a, CABulkLane& L, int s, const float* ring = nullptr) {
+  const int t = s - 2;
+  const Row6A Vs = ca_ld_row<IN_RING>(a, L, a.v, ring, CA_RV, t - 2);
+  L.H[0] = ca_ld_row<IN_RING>(a, L, a.h, ring, CA_RH, t - 1); L.U[0] = ca_ld_row<IN_RING>(a, L, a.u, ring, CA_RU, t - 1);
+  L.V[0] = ca_ld_row<IN_RING>(a, L, a.v, ring, CA_RV, t - 1);
+  L.H[1] = ca_ld_row<IN_RING>(a, L, a.h, ring, CA_RH, t); L.U[1] = ca_ld_row<IN_RING>(a, L, a.u, ring, CA_RU, t);
+  L.V[1] = ca_ld_row<IN_RING>(a, L, a.v, ring, CA_RV, t);
+  L.H[2] = ca_ld_row<IN_RING>(a, L, a.h, ring, CA_RH, t + 1); L.U[2] = ca_ld_row<IN_RING>(a, L, a.u, ring, CA_RU, t + 1);
+  L.V[2] = ca_ld_row<IN_RING>(a, L, a.v, ring, CA_RV, t + 1);
   ca_bulk_fluxes(a.p, a.p.coriolis[t - 1], L.H[0], L.U[0], L.V[0], L.H[1], L.U[1], Vs, L.Fm);
   ca_bulk_fluxes(a.p, a.p.coriolis[t], L.H[1], L.U[1], L.V[1], L.H[2], L.U[2], L.V[0], L.Fc);
   // slots 0, 1 = rows t, t+1 (ca_bulk_tend loads row t+2 into slot 2)
@@ -124,15 +206,20 @@ __device__ __forceinline__ void ca_bulk_begin(const CABulkArgs& a, CABulkLane& L
 }
 
 // phase 1 of row t: load row t+2 and the old tendencies, fluxes of row t+1, tendency + update of row t;
-// stores h', dh, du, dv when `out` (row t is one of the segment's rows)
-__device__ __forceinline__ void ca_bulk_tend(const CABulkArgs& a, CABulkLane& L, int t, bool out) {
+// stores h', dh, du, dv when `out` (row t is one of the segment's rows): to the ring (OUT_RING), and to
+// the arrays where `hbm` as well
+template <bool IN_RING = false, bool OUT_RING = false>
+__device__ __forceinline__ void ca_bulk_tend(const CABulkArgs& a, CABulkLane& L, int t, bool out,
+                                             float* ring = nullptr, bool hbm = true) {
   const B2SweParams& p = a.p;
-  const int P = p.pitch;
-  const size_t off = (size_t)t * P + L.i0;
-  L.H[2] = ld_row_a(a.h, t + 2, L.i0, P); L.U[2] = ld_row_a(a.u, t + 2, L.i0, P); L.V[2] = ld_row_a(a.v, t + 2, L.i0, P);
+  const size_t off = (size_t)t * p.pitch + L.i0;
+  L.H[2] = ca_ld_row<IN_RING>(a, L, a.h, ring, CA_RH, t + 2);
+  L.U[2] = ca_ld_row<IN_RING>(a, L, a.u, ring, CA_RU, t + 2);
+  L.V[2] = ca_ld_row<IN_RING>(a, L, a.v, ring, CA_RV, t + 2);
   if (!p.first_step) {
-    L.du4 = ld4(a.du, off); L.dv4 = ld4(a.dv, off);
-    if (out) L.dh4 = ld4(a.dh, off);                 // (rows above / below the segment: h' is not stored)
+    L.du4 = ca_ld4<IN_RING>(L, a.du, off, ring, CA_RDU, t); L.dv4 = ca_ld4<IN_RING>(L, a.dv, off, ring, CA_RDV, t);
+    if (out)                                         // (rows above / below the segment: h' is not stored)
+      L.dh4 = ca_ld4<IN_RING>(L, a.dh_src != nullptr ? a.dh_src : a.dh, off, ring, CA_RDH, t);
   }
   CAFluxRow Fp;
   ca_bulk_fluxes(p, p.coriolis[t + 1], L.H[1], L.U[1], L.V[1], L.H[2], L.U[2], L.V[0], Fp);
@@ -153,11 +240,11 @@ __device__ __forceinline__ void ca_bulk_tend(const CABulkArgs& a, CABulkLane& L,
     Hn[k] = o.h; L.upn[k] = o.u; L.vpn[k] = o.v;
     DH[k] = o.dh; DU[k] = o.du; DV[k] = o.dv;
   }
-  if (out && L.store) {
-    st4(a.h_o, off, make_float4(Hn[0], Hn[1], Hn[2], Hn[3]));
-    st4(a.dh, off, make_float4(DH[0], DH[1], DH[2], DH[3]));
-    st4(a.du_o, off, make_float4(DU[0], DU[1], DU[2], DU[3]));
-    st4(a.dv_o, off, make_float4(DV[0], DV[1], DV[2], DV[3]));
+  if (out) {
+    ca_st4<OUT_RING>(L, a.h_o, off, ring, CA_RH, t, hbm, make_float4(Hn[0], Hn[1], Hn[2], Hn[3]));
+    ca_st4<OUT_RING>(L, a.dh, off, ring, CA_RDH, t, hbm, make_float4(DH[0], DH[1], DH[2], DH[3]));
+    ca_st4<OUT_RING>(L, a.du_o, off, ring, CA_RDU, t, hbm, make_float4(DU[0], DU[1], DU[2], DU[3]));
+    ca_st4<OUT_RING>(L, a.dv_o, off, ring, CA_RDV, t, hbm, make_float4(DV[0], DV[1], DV[2], DV[3]));
   }
   L.H[0] = L.H[1]; L.U[0] = L.U[1]; L.V[0] = L.V[1];
   L.H[1] = L.H[2]; L.U[1] = L.U[2]; L.V[1] = L.V[2];
@@ -167,9 +254,11 @@ __device__ __forceinline__ void ca_bulk_tend(const CABulkArgs& a, CABulkLane& L,
 // phase 2 of row t: friction of row r = t-1 (swe_k34_body's u update and fluxes, swe_k5_body's v update)
 // given the west lane's u' of row t at columns i0-2, i0-1 and the east lane's u', v' at i0+4.
 // `upp_only`: row r lies above the segment, only its u'' is needed (the south flux of the next row);
-// `out`: row r is one of the segment's rows, u'' and v'' are stored.
+// `out`: row r is one of the segment's rows, u'' and v'' are stored (ring and `hbm` as in ca_bulk_tend).
+template <bool OUT_RING = false>
 __device__ __forceinline__ void ca_bulk_fric(const CABulkArgs& a, CABulkLane& L, int t, float uw2, float uw3,
-                                             float ue, float ve, bool upp_only, bool out) {
+                                             float ue, float ve, bool upp_only, bool out, float* ring = nullptr,
+                                             bool hbm = true) {
   const B2SweParams& p = a.p;
   const float up2[7] = {uw2, uw3, L.upn[0], L.upn[1], L.upn[2], L.upn[3], ue};
   const float vp2[5] = {L.vpn[0], L.vpn[1], L.vpn[2], L.vpn[3], ve};
@@ -181,7 +270,7 @@ __device__ __forceinline__ void ca_bulk_fric(const CABulkArgs& a, CABulkLane& L,
       UPP[d] = swe_friction_u(p, L.up1[x], L.up1[x + 1], L.up1[x - 1], up2[x], L.up0[x], false, false);
       FE2[d] = swe_visc_flux(p.c_nux, L.vp1[d], UPP[d]);
     }
-    if (out && L.store) {
+    if (out && (OUT_RING || L.store)) {
       float Vn[4];
 #pragma unroll
       for (int k = 0; k < 4; ++k) {
@@ -190,8 +279,8 @@ __device__ __forceinline__ void ca_bulk_fric(const CABulkArgs& a, CABulkLane& L,
         Vn[k] = swe_apply_div(p, L.vp1[k], FE2[k + 1], FE2[k], fn2_c, fn2_s);
       }
       const size_t off = (size_t)(t - 1) * p.pitch + L.i0;
-      st4(a.u_o, off, make_float4(UPP[1], UPP[2], UPP[3], UPP[4]));
-      st4(a.v_o, off, make_float4(Vn[0], Vn[1], Vn[2], Vn[3]));
+      ca_st4<OUT_RING>(L, a.u_o, off, ring, CA_RU, t - 1, hbm, make_float4(UPP[1], UPP[2], UPP[3], UPP[4]));
+      ca_st4<OUT_RING>(L, a.v_o, off, ring, CA_RV, t - 1, hbm, make_float4(Vn[0], Vn[1], Vn[2], Vn[3]));
     }
 #pragma unroll
     for (int k = 0; k < 4; ++k) L.upp1[k] = UPP[k + 1];

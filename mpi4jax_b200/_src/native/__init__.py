@@ -101,7 +101,8 @@ class B2SweParams(Structure):
 
 class B2SweState(Structure):
     _fields_ = [(name, c_void_p) for name in
-                ("h0", "h1", "u", "v", "dh", "du", "dv", "fe", "fn", "q", "ke", "fe2", "fn2", "u1", "v1", "du1", "dv1")]
+                ("h0", "h1", "u", "v", "dh", "du", "dv", "fe", "fn", "q", "ke", "fe2", "fn2", "u1", "v1", "du1", "dv1",
+                 "h2", "u2", "v2", "dh1", "dh2", "du2", "dv2")]
 
 
 class B2SweCA(Structure):
@@ -234,7 +235,7 @@ _SIGNATURES = {
 
 
 #: must equal B2_ABI_VERSION in csrc/b2_common.h
-ABI_VERSION = 19
+ABI_VERSION = 20
 #: must equal B2_MAX_RANKS in csrc/b2_common.h (ranks per communicator; sizes the alltoallv count header)
 MAX_RANKS = 16
 _ABI_FIELDS = ("abi_version", "sizeof_status_record", "sizeof_halo_desc", "sizeof_swe_params",

@@ -179,6 +179,9 @@ class ShallowWaterModel:
         self._u1 = z()      # ping-pong partner of u for the friction update
         self._v1 = z()      # ping-pong partner of v
         self._du1, self._dv1 = z(), z()      # ping-pong partners of du, dv (communication-avoiding step)
+        # the communication-avoiding step's second and third buffer sets (it rotates three)
+        self._h2, self._u2, self._v2 = z(), z(), z()
+        self._dh1, self._dh2, self._du2, self._dv2 = z(), z(), z(), z()
         self.fe, self.fn, self.q, self.ke, self.fe2, self.fn2 = z(), z(), z(), z(), z(), z()
         y_global = (np.arange(-1, self.ny_global - 1) * self.cfg.dy)
         cor = self.cfg.coriolis_f + y_global[self.local_slice[0]] * self.cfg.coriolis_beta
@@ -201,6 +204,8 @@ class ShallowWaterModel:
             st.u1 = self._u1.data_ptr()
             st.v1 = self._v1.data_ptr()
             st.du1, st.dv1 = self._du1.data_ptr(), self._dv1.data_ptr()
+            for name in ("h2", "u2", "v2", "dh1", "dh2", "du2", "dv2"):
+                setattr(st, name, getattr(self, "_" + name).data_ptr())
             for name in ("u", "v", "dh", "du", "dv", "fe", "fn", "q", "ke", "fe2", "fn2"):
                 setattr(st, name, getattr(self, name).data_ptr())
             t = self._topo = native.B2HaloDesc()
@@ -266,6 +271,9 @@ class ShallowWaterModel:
         self._v1.copy_(self.v)
         self._du1.copy_(self.du)
         self._dv1.copy_(self.dv)
+        for dst, src in ((self._h2, self.h), (self._u2, self.u), (self._v2, self.v), (self._dh1, self.dh),
+                         (self._dh2, self.dh), (self._du2, self.du), (self._dv2, self.dv)):
+            dst.copy_(src)
         if self.backend == "native" and self.pipeline == "ca":
             nc = self.comm._native_comm()
             rc = native.lib.b2_swe_ca_init(

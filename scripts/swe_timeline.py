@@ -1,6 +1,7 @@
 """Device-side timeline of the communication-avoiding shallow-water step INSIDE a CUDA-graph replay:
 first-CTA-start / last-CTA-end (%globaltimer) of the four kernels of each step, relative to the
-step's first event.  A = frame tendencies, S = bulk (whole step, one pass), X = halo exchange,
+step's first event.  A = frame tendencies, S = bulk (one step; of a pair of steps, S2 in the first and
+the ring launch in the second), X = halo exchange,
 D = frame friction.  Works at any world size (every rank prints its own table to its log).
 
     python -m mpi4jax_b200.run -n 8 scripts/swe_timeline.py [grid] [steps]
