@@ -123,16 +123,23 @@ __global__ void __launch_bounds__(CA_THREADS) swe_ca_init_ext(const B2SweParams 
 }
 
 // ---- S: the bulk, one pass per step (b2_swe_ca_bulk.cuh) ----------------------------------------
-// Also the ring launch of the pair schedule: the same kernel over narrower store windows.
+// Also the ring launch of the pair schedule: the same kernel over the four narrower store windows in one
+// launch.  blockIdx.y picks the window of `win` (the whole bulk: a table of one); `a`'s own window is not
+// used.
+#define CA_MAX_WINDOWS 4
+struct CAWindows {
+  CAWin w[CA_MAX_WINDOWS];
+};
 __global__ void __launch_bounds__(CA_BULK_WARPS * 32)
-swe_ca_bulk_step(const CABulkArgs a, const CAStamp ts) {
+swe_ca_bulk_step(const CABulkArgs a, const __grid_constant__ CAWindows win, const CAStamp ts) {
   ca_stamp_begin(ts);
+  const CAWin& g = win.w[blockIdx.y];
   const int w = (int)blockIdx.x * CA_BULK_WARPS + (int)(threadIdx.x >> 5), lane = threadIdx.x & 31;
-  if (w < ca_bulk_warps(a)) {                          // (whole warps: the lane exchange needs all 32)
+  if (w < ca_bulk_warps(g)) {                          // (whole warps: the lane exchange needs all 32)
     int s, e;
-    ca_bulk_rows(a, w / a.wcols, s, e);
+    ca_bulk_rows(g, w / g.wcols, s, e);
     CABulkLane L;
-    L.store = ca_bulk_lane(a, w % a.wcols, lane, L.i0);
+    L.store = ca_bulk_lane(g, w % g.wcols, lane, L.i0);
     ca_bulk_begin(a, L, s);
     for (int t = s - 2; t <= e; ++t) {
       ca_bulk_tend(a, L, t, t >= s && t < e);
@@ -389,9 +396,9 @@ int b2_swe_ca_init(B2Comm* c, const B2SweParams* p0, const B2SweState* st, const
 //   s2:  A X D (t) ----------------------------------------------> A X D (t+1) ------------> next
 //                                   (ring waits for D (t), A X D (t+1) for S2)
 //
-// The ring launches are swe_ca_bulk_step on the four windows around the inner bulk: rows [4, 8) and
-// [ny-7, ny-4), groups 0 and ng-1 between them; they are the only part of step t+1 that needs the frame's
-// state t+1.  An odd step left over runs the one-step schedule.  h, u, v, du and dv rotate through three
+// The ring launch is swe_ca_bulk_step on the four windows around the inner bulk, one window per
+// blockIdx.y: rows [4, 8) and [ny-7, ny-4), groups 0 and ng-1 between them; it is the only part of step t+1
+// that needs the frame's state t+1.  An odd step left over runs the one-step schedule.  h, u, v, du and dv rotate through three
 // buffer sets: a step reads one and writes another; S2 reads set c (state t), stores the band of state
 // t+1 into set n, where A X D (t) write the frame's, and state t+2 into set m (a segment's step 1 reads
 // rows that a neighbouring segment's step 2 overwrites, so ping-pong is not enough).  dh stays in place
@@ -432,18 +439,24 @@ int b2_swe_multistep_ca(B2Comm* c, const B2SweParams* p0, const B2SweState* st, 
   ca_bulk_geometry(p, x.cb1, 1, sa);
   ca_bulk_geometry(p, x.cb1, ca_rows_per_segment(slot_warps, sa.wcols, ny - 8), sa);
   // pairs: S2's inner bulk (step 1 walks its segments), the ring's four windows; two rows per segment
-  // there: the ring launches are exposed and move little data, so a warp's walk (its rows + 3 tendency
+  // there: the ring launch is exposed and moves little data, so a warp's walk (its rows + 3 tendency
   // rows, each a round trip to HBM) is kept short
   const bool pairs = ny - 7 > 8 && ng >= 3;
-  CABulkArgs pa = {}, pb = {}, ring[4] = {};
+  CAWindows whole = {}, ring = {};
+  whole.w[0] = sa;
+  const unsigned whole_blocks = ca_blocks(ca_bulk_warps(sa), CA_BULK_WARPS);
+  CABulkArgs pa = {}, pb = {}, ra = {};
+  unsigned ring_blocks = 0;
   if (pairs) {
     ca_bulk_window(x.cb1, 8, ny - 7, 1, ng - 1, 3, 1, pb);
     ca_bulk_window(x.cb1, 8, ny - 7, 1, ng - 1, 3, ca_rows_per_segment(slot_pairs, pb.wcols, ny - 15), pb);
     pa.ng = pb.ng;
-    ca_bulk_window(x.cb1, 4, 8, 0, ng, 1, 2, ring[0]);
-    ca_bulk_window(x.cb1, ny - 7, ny - 4, 0, ng, 1, 2, ring[1]);
-    ca_bulk_window(x.cb1, 8, ny - 7, 0, 1, 1, 2, ring[2]);
-    ca_bulk_window(x.cb1, 8, ny - 7, ng - 1, ng, 1, 2, ring[3]);
+    ca_bulk_window(x.cb1, 4, 8, 0, ng, 1, 2, ring.w[0]);
+    ca_bulk_window(x.cb1, ny - 7, ny - 4, 0, ng, 1, 2, ring.w[1]);
+    ca_bulk_window(x.cb1, 8, ny - 7, 0, 1, 1, 2, ring.w[2]);
+    ca_bulk_window(x.cb1, 8, ny - 7, ng - 1, ng, 1, 2, ring.w[3]);
+    for (const CAWin& g : ring.w)
+      if (ca_blocks(ca_bulk_warps(g), CA_BULK_WARPS) > ring_blocks) ring_blocks = ca_blocks(ca_bulk_warps(g), CA_BULK_WARPS);
   }
   const CAFrame fa = ca_frame(p, 5, x.cb1 - 2), fd = ca_frame(p, 3, x.cb1);
   const unsigned tend_blocks = ca_blocks(fa.total, CA_CELLS);
@@ -500,7 +513,7 @@ int b2_swe_multistep_ca(B2Comm* c, const B2SweParams* p0, const B2SweState* st, 
     if (rc) break;
     if (!pair) {
       io(sa, cur, nxt, nullptr, DH[dc]);
-      swe_ca_bulk_step<<<ca_blocks(ca_bulk_warps(sa), CA_BULK_WARPS), CA_BULK_WARPS * 32, 0, s>>>(sa, ca_slot(it, 1));
+      swe_ca_bulk_step<<<whole_blocks, CA_BULK_WARPS * 32, 0, s>>>(sa, whole, ca_slot(it, 1));
       if ((rc = b2_launched(c, "swe_ca_bulk_step"))) break;
       CA_RT(cudaEventRecord(eS, s));
       if (rc || (rc = frame(it, cur, nxt, nullptr, DH[dc]))) break;
@@ -519,13 +532,11 @@ int b2_swe_multistep_ca(B2Comm* c, const B2SweParams* p0, const B2SweState* st, 
     // ring (t+1): needs D (t); A X D (t+1): needs S2 (eS, recorded before the ring re-records it)
     CA_RT(cudaStreamWaitEvent(s, eD, 0));
     CA_RT(cudaStreamWaitEvent(s2, eS, 0));
-    for (int k = 0; k < 4 && rc == 0; ++k) {
-      io(ring[k], nxt, third, DH[dn], DH[dm]);
-      swe_ca_bulk_step<<<ca_blocks(ca_bulk_warps(ring[k]), CA_BULK_WARPS), CA_BULK_WARPS * 32, 0, s>>>(
-          ring[k], ca_slot(it + 1, 1));
-      rc = b2_launched(c, "swe_ca_bulk_step");
-    }
-    if (rc || (rc = frame(it + 1, nxt, third, DH[dn], DH[dm]))) break;
+    if (rc) break;
+    io(ra, nxt, third, DH[dn], DH[dm]);
+    swe_ca_bulk_step<<<dim3(ring_blocks, CA_MAX_WINDOWS), CA_BULK_WARPS * 32, 0, s>>>(ra, ring, ca_slot(it + 1, 1));
+    if ((rc = b2_launched(c, "swe_ca_bulk_step"))) break;
+    if ((rc = frame(it + 1, nxt, third, DH[dn], DH[dm]))) break;
     CA_RT(cudaEventRecord(eS, s));
     cur = third;
     dc = dm;

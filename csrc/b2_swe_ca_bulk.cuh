@@ -53,14 +53,17 @@ __device__ __forceinline__ Row6A ld_row_a(const float* __restrict__ x, int j, in
 #define CA_RING_FLOATS (6 * CA_RING_FIELD)
 enum { CA_RH = 0, CA_RU, CA_RV, CA_RDH, CA_RDU, CA_RDV };
 
-struct CABulkArgs {
-  B2SweParams p;
+// where a launch's warps go: its store window and how its warps tile it
+struct CAWin {
   int ng;                                            // bulk groups per row: columns [4, 4 + 4 ng)
   int r0, r1, g0, g1;                                // store window: rows [r0, r1) x groups [g0, g1)
   int halo;                                          // lanes on each side of a strip that do not store
   int rows;                                          // rows per segment
   int wcols;                                         // warp strips per row of segments
   int nseg;                                          // segments: window rows [r0, r1)
+};
+struct CABulkArgs : CAWin {
+  B2SweParams p;
   const float *h, *u, *v, *du, *dv;                  // this step
   float *h_o, *u_o, *v_o, *du_o, *dv_o;              // the next step
   float* dh;                                         // the next step's dh (own cells only)
@@ -70,21 +73,21 @@ struct CABulkArgs {
 // geometry of a launch over the window [r0, r1) x [g0, g1): a warp's (segment, strip), a lane's group.
 // The one-step kernel over the whole bulk is the window [4, ny - 4) x [0, ng) with halo 1.
 __host__ __device__ inline void ca_bulk_window(int cb1, int r0, int r1, int g0, int g1, int halo, int rows,
-                                               CABulkArgs& a) {
+                                               CAWin& a) {
   a.ng = (cb1 >> 2) - 1;
   a.r0 = r0; a.r1 = r1; a.g0 = g0; a.g1 = g1; a.halo = halo;
   a.rows = rows;
   a.wcols = (g1 - g0 + 32 - 2 * halo - 1) / (32 - 2 * halo);
   a.nseg = (r1 - r0 + rows - 1) / rows;
 }
-__host__ __device__ inline void ca_bulk_geometry(const B2SweParams& p, int cb1, int rows, CABulkArgs& a) {
+__host__ __device__ inline void ca_bulk_geometry(const B2SweParams& p, int cb1, int rows, CAWin& a) {
   ca_bulk_window(cb1, 4, p.ny - 4, 0, (cb1 >> 2) - 1, 1, rows, a);
 }
-__host__ __device__ inline long long ca_bulk_warps(const CABulkArgs& a) { return (long long)a.wcols * a.nseg; }
+__host__ __device__ inline long long ca_bulk_warps(const CAWin& a) { return (long long)a.wcols * a.nseg; }
 // group index of `lane` in strip `wc`; lanes beyond the groups the window's stored lanes need repeat the
 // last of them (at most ng, the group east of the bulk), so a narrow window loads few distinct columns;
 // the lane stores when it returns true
-__host__ __device__ inline bool ca_bulk_lane(const CABulkArgs& a, int wc, int lane, int& i0) {
+__host__ __device__ inline bool ca_bulk_lane(const CAWin& a, int wc, int lane, int& i0) {
   int g = a.g0 + wc * (32 - 2 * a.halo) + lane - a.halo;
   const int ghi = a.g1 + a.halo - 1 < a.ng ? a.g1 + a.halo - 1 : a.ng;
   if (g > ghi) g = ghi;
@@ -127,7 +130,7 @@ struct CABulkLane {
 
 // rows [s, e) of segment `seg`; its tendency rows are s-2 .. e (rows s-2, s-1 and e only feed the
 // friction of rows s .. e-1)
-__host__ __device__ inline void ca_bulk_rows(const CABulkArgs& a, int seg, int& s, int& e) {
+__host__ __device__ inline void ca_bulk_rows(const CAWin& a, int seg, int& s, int& e) {
   s = a.r0 + seg * a.rows;
   e = s + a.rows < a.r1 ? s + a.rows : a.r1;
 }
