@@ -28,7 +28,6 @@
 
 #include "b2_device.cuh"
 #include "b2_halo_ll.cuh"
-#include "b2_launch.cuh"
 #include "b2_runtime.h"
 
 #define HALO_THREADS 256
@@ -36,7 +35,6 @@
 
 __global__ void __launch_bounds__(HALO_THREADS) b2_k_halo_ll(const B2DevComm c, const B2HaloDesc d,
                                                              const int fs) {
-  b2_pdl_enter();
   __shared__ unsigned s_rx[FS_NSIDES], s_tx[FS_NSIDES];
   const int gt = blockIdx.x * blockDim.x + threadIdx.x, gn = gridDim.x * blockDim.x;
   const int ny = d.ny, nx = d.nx, F = d.nfields;
@@ -193,6 +191,6 @@ extern "C" int b2_halo_exchange(B2Comm* c, const B2HaloDesc* d, cudaStream_t str
   int ctas = (d->nfields * mx + HALO_THREADS - 1) / HALO_THREADS;
   if (ctas < HALO_LL_CTAS) ctas = HALO_LL_CTAS;
   if (ctas > 96) ctas = 96;
-  b2_launch(b2_k_halo_ll, ctas, HALO_THREADS, 0, stream, c->dev, *d, fs);
+  b2_k_halo_ll<<<ctas, HALO_THREADS, 0, stream>>>(c->dev, *d, fs);
   return b2_launched(c, "halo_exchange");
 }

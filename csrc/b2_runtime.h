@@ -75,8 +75,6 @@ int b2_get_logging(void);
 typedef void (*b2_print_fn)(const char*);
 void b2_set_print_callback(b2_print_fn fn);
 int b2_launch_count(void);
-int b2_pdl_enabled(void);      // programmatic dependent launch of the stencil/halo chain
-void b2_set_pdl(int enable);
 
 // --- device / driver ---------------------------------------------------------
 int b2_init(int device);

@@ -26,13 +26,11 @@
 // These kernels are pure streaming stencils (1 FLOP per ~2 bytes): the roofline
 // is HBM bandwidth, there is no tensor-core work in this workload.
 #include "b2_swe_body.cuh"
-#include "b2_launch.cuh"
 
 __global__ void __launch_bounds__(SWE_THREADS)
 swe_k1_fluxes(B2SweParams p, const float* __restrict__ h, const float* __restrict__ u,
               const float* __restrict__ v, float* __restrict__ fe, float* __restrict__ fn,
               float* __restrict__ q, float* __restrict__ ke) {
-  b2_pdl_enter();
   int j, i0;
   bool m[4];
   if (!swe_map(p, j, i0, m)) return;
@@ -45,7 +43,6 @@ swe_k2_tendencies(B2SweParams p, const float* __restrict__ h, float* __restrict_
                   float* __restrict__ du, float* __restrict__ dv, const float* __restrict__ fe,
                   const float* __restrict__ fn, const float* __restrict__ q,
                   const float* __restrict__ ke) {
-  b2_pdl_enter();
   int j, i0;
   bool m[4];
   if (!swe_map(p, j, i0, m)) return;
@@ -56,7 +53,6 @@ __global__ void __launch_bounds__(SWE_THREADS)
 swe_k34_friction_u(B2SweParams p, const float* __restrict__ u, float* __restrict__ u_new,
                    const float* __restrict__ v, float* __restrict__ fe2, float* __restrict__ fn2,
                    int has_south) {
-  b2_pdl_enter();
   int j, i0 = -1;
   bool m[4];
   // also the group that holds only the east halo column (nx % 4 == 1): u_new's halo cells are copies
@@ -68,60 +64,10 @@ swe_k34_friction_u(B2SweParams p, const float* __restrict__ u, float* __restrict
 __global__ void __launch_bounds__(SWE_THREADS)
 swe_k5_friction_v(B2SweParams p, float* __restrict__ v, const float* __restrict__ fe2,
                   const float* __restrict__ fn2) {
-  b2_pdl_enter();
   int j, i0;
   bool m[4];
   if (!swe_map(p, j, i0, m)) return;
   swe_k5_body(p, v, fe2, fn2, j, i0, m);
-}
-
-static unsigned swe_blocks(const B2SweParams* p) {
-  const long long n = (long long)(p->ny - 2) * (p->pitch / 4);
-  return (unsigned)((n + SWE_THREADS - 1) / SWE_THREADS);
-}
-
-static int swe_check(const B2SweParams* p) {
-  if (p->pitch % 4 != 0 || p->pitch < p->nx || p->ny < 3 || p->nx < 3) {
-    b2_set_error("swe: need ny,nx >= 3 and a row pitch that is a multiple of 4 floats and >= nx "
-                 "(got ny=%d nx=%d pitch=%d)", p->ny, p->nx, p->pitch);
-    return B2_ERR_BAD_ARG;
-  }
-  return 0;
-}
-
-static int b2_swe_fluxes(B2Comm* c, const B2SweParams* p, const float* h, const float* u, const float* v,
-                  float* fe, float* fn, float* q, float* ke, cudaStream_t s) {
-  if (int rc = swe_check(p)) return rc;
-  b2_launch(swe_k1_fluxes, swe_blocks(p), SWE_THREADS, 0, s, *p, h, u, v, fe, fn, q, ke);
-  return b2_launched(c, "swe_fluxes");
-}
-
-static int b2_swe_tendencies(B2Comm* c, const B2SweParams* p, const float* h, float* h_new, float* u,
-                      float* v, float* dh, float* du, float* dv, const float* fe, const float* fn,
-                      const float* q, const float* ke, cudaStream_t s) {
-  if (int rc = swe_check(p)) return rc;
-  b2_launch(swe_k2_tendencies, swe_blocks(p), SWE_THREADS, 0, s, *p, h, h_new, u, v, dh, du, dv, fe, fn, q, ke);
-  return b2_launched(c, "swe_tendencies");
-}
-
-// friction-u flux + apply + friction-v flux in one kernel (no fe/fn round trip through HBM)
-// (u -> u_new: out of place, u_new must not alias u)
-static int b2_swe_friction_u_fused(B2Comm* c, const B2SweParams* p, const float* u, float* u_new,
-                            const float* v, float* fe2, float* fn2, int has_south, cudaStream_t s) {
-  if (int rc = swe_check(p)) return rc;
-  if (u == u_new) {
-    b2_set_error("swe_friction_u_fused: u_new must not alias u (the update reads u's neighbours)");
-    return B2_ERR_BAD_ARG;
-  }
-  b2_launch(swe_k34_friction_u, swe_blocks(p), SWE_THREADS, 0, s, *p, u, u_new, v, fe2, fn2, has_south);
-  return b2_launched(c, "swe_friction_u_fused");
-}
-
-static int b2_swe_friction_v(B2Comm* c, const B2SweParams* p, float* v, const float* fe2, const float* fn2,
-                      cudaStream_t s) {
-  if (int rc = swe_check(p)) return rc;
-  b2_launch(swe_k5_friction_v, swe_blocks(p), SWE_THREADS, 0, s, *p, v, fe2, fn2);
-  return b2_launched(c, "swe_friction_v");
 }
 
 extern "C" {
@@ -135,6 +81,17 @@ extern "C" {
 int b2_swe_multistep(B2Comm* c, const B2SweParams* p0, const B2SweState* st, const B2HaloDesc* topo,
                      int nsteps, int first_step, cudaStream_t s) {
   B2SweParams p = *p0;
+  if (p.pitch % 4 != 0 || p.pitch < p.nx || p.ny < 3 || p.nx < 3) {
+    b2_set_error("swe: need ny,nx >= 3 and a row pitch that is a multiple of 4 floats and >= nx "
+                 "(got ny=%d nx=%d pitch=%d)", p.ny, p.nx, p.pitch);
+    return B2_ERR_BAD_ARG;
+  }
+  // friction-u is out of place: u and u1 ping-pong
+  if (p.viscosity > 0.f && st->u == st->u1) {
+    b2_set_error("swe_friction_u_fused: u_new must not alias u (the update reads u's neighbours)");
+    return B2_ERR_BAD_ARG;
+  }
+  const unsigned blocks = (unsigned)(((long long)(p.ny - 2) * (p.pitch / 4) + SWE_THREADS - 1) / SWE_THREADS);
   float* h = st->h0;
   float* hn = st->h1;
   float* u = st->u;
@@ -146,15 +103,17 @@ int b2_swe_multistep(B2Comm* c, const B2SweParams* p0, const B2SweState* st, con
   int rc = 0;
   for (int it = 0; it < nsteps && rc == 0; ++it) {
     p.first_step = (first_step && it == 0) ? 1 : 0;
-    if ((rc = b2_swe_fluxes(c, &p, h, u, st->v, st->fe, st->fn, st->q, st->ke, s))) break;
+    swe_k1_fluxes<<<blocks, SWE_THREADS, 0, s>>>(p, h, u, st->v, st->fe, st->fn, st->q, st->ke);
+    if ((rc = b2_launched(c, "swe_fluxes"))) break;
     d.nfields = 4;
     d.field[0] = st->fe; d.kind[0] = 1;
     d.field[1] = st->fn; d.kind[1] = 2;
     d.field[2] = st->q;  d.kind[2] = 0;
     d.field[3] = st->ke; d.kind[3] = 0;
     if ((rc = b2_halo_exchange(c, &d, s))) break;
-    if ((rc = b2_swe_tendencies(c, &p, h, hn, u, st->v, st->dh, st->du, st->dv, st->fe, st->fn,
-                                st->q, st->ke, s))) break;
+    swe_k2_tendencies<<<blocks, SWE_THREADS, 0, s>>>(p, h, hn, u, st->v, st->dh, st->du, st->dv,
+                                                     st->fe, st->fn, st->q, st->ke);
+    if ((rc = b2_launched(c, "swe_tendencies"))) break;
     d.nfields = 3;
     d.field[0] = hn;    d.kind[0] = 0;
     d.field[1] = u;     d.kind[1] = 1;
@@ -163,13 +122,15 @@ int b2_swe_multistep(B2Comm* c, const B2SweParams* p0, const B2SweState* st, con
     if (p.viscosity > 0.f) {
       // friction-u fluxes are evaluated inline from u (incl. their halo, from u's fresh halo):
       // no K3 launch, no (fe, fn) exchange, no HBM round trip of the fluxes
-      if ((rc = b2_swe_friction_u_fused(c, &p, u, un, st->v, st->fe2, st->fn2, topo->south >= 0, s))) break;
+      swe_k34_friction_u<<<blocks, SWE_THREADS, 0, s>>>(p, u, un, st->v, st->fe2, st->fn2, topo->south >= 0);
+      if ((rc = b2_launched(c, "swe_friction_u_fused"))) break;
       { float* t = u; u = un; un = t; }
       d.nfields = 2;
       d.field[0] = st->fe2; d.kind[0] = 1;
       d.field[1] = st->fn2; d.kind[1] = 2;
       if ((rc = b2_halo_exchange(c, &d, s))) break;
-      if ((rc = b2_swe_friction_v(c, &p, st->v, st->fe2, st->fn2, s))) break;
+      swe_k5_friction_v<<<blocks, SWE_THREADS, 0, s>>>(p, st->v, st->fe2, st->fn2);
+      if ((rc = b2_launched(c, "swe_friction_v"))) break;
     }
     float* t = h; h = hn; hn = t;
   }
