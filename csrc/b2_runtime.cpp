@@ -482,6 +482,7 @@ extern "C" long long b2_comm_get_option(B2Comm* c, const char* key) {
   if (const size_t* t = threshold(c, key)) return (long long)*t;
   if (strcmp(key, "max_blocks") == 0) return c->max_blocks;
   if (strcmp(key, "sm_count") == 0) return c->sm_count;
+  if (strcmp(key, "p2p_slot_bytes") == 0) return (long long)c->dev.lay.p2p_slot_bytes;
   if (strcmp(key, "bcast_mc_min") == 0) return (long long)c->bcast_mc_min;
   if (strcmp(key, "nvls_pipeline") == 0) return c->nvls_pipeline ? 1 : 0;
   if (strcmp(key, "gemm_raster") == 0) return c->gemm_raster < 0 ? 0 : c->gemm_raster;

@@ -108,7 +108,8 @@ B2Comm* b2_comm_create(int device, int rank, int nranks, B2Seg* ctl, size_t slot
 int b2_comm_set_stage(B2Comm* c, B2Seg* stage, B2Mc* mc);
 size_t b2_comm_stage_half(B2Comm* c);
 // keys: "ll_max", "oneshot_max", "nvls_min" (bytes), "max_blocks", "bcast_mc_min", "nvls_pipeline",
-// "gemm_raster", "p2p_anysource_scan", "trace_ptr", "trace_cap"; get_option also reads "sm_count"
+// "gemm_raster", "p2p_anysource_scan", "trace_ptr", "trace_cap"; get_option also reads "sm_count" and
+// "p2p_slot_bytes" (the p2p ring's slot size, as rounded up at creation)
 int b2_comm_set_option(B2Comm* c, const char* key, long long value);
 long long b2_comm_get_option(B2Comm* c, const char* key);
 int b2_comm_check_error(B2Comm* c, char* buf, int buflen);     // 0 = ok

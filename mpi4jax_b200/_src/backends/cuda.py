@@ -378,7 +378,9 @@ class NativeComm:
         self._check(_lib().b2_comm_set_option(self.handle, key.encode(), int(value)), "Comm_set_option")
 
     def get_option(self, key: str) -> int:
-        """Current value of a launch parameter: any key of :meth:`set_option` but the trace buffer, or ``sm_count``."""
+        """Current value of a launch parameter: any key of :meth:`set_option` but the trace buffer, ``sm_count``,
+        or ``p2p_slot_bytes`` (the p2p ring's slot size in bytes: ``MPI4JAX_B200_P2P_SLOT_BYTES`` rounded up to
+        4 KiB when the communicator was created; a message longer than that travels in several fragments)."""
         value = int(_lib().b2_comm_get_option(self.handle, key.encode()))
         if value < 0:
             raise ValueError(f"unknown communicator option {key!r}")

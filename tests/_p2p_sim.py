@@ -159,3 +159,68 @@ class Inbox:
             assert pair.try_recv(recv_tag, nb)
             return src, tag, nb
         return None
+
+
+# ---- schedules: the MPI oracle, the model run and the reachability rule of a tagged receive ----
+def _oracle(messages, recv_tags):
+    """MPI matching: each receive takes the earliest not-yet-received message with its tag."""
+    taken, order = set(), []
+    for t in recv_tags:
+        for k, (tag, _) in enumerate(messages):
+            if k not in taken and (t == ANY_TAG or tag == t):
+                taken.add(k)
+                order.append(k)
+                break
+        else:
+            raise AssertionError("test generator produced an unmatched receive")
+    return order
+
+
+def _run(messages, recv_order, slot_bytes=4):
+    """messages: [(tag, nbytes)] sent in order; recv_order: indices in the order they are received
+    (each receive uses the message's tag, or ANY_TAG when flagged)."""
+    pair = Pair(slot_bytes)
+    for tag, nb in messages:
+        pair.post_send(tag, nb)
+    starts, s = [], 0
+    for tag, nb in messages:
+        starts.append(s)
+        s += pair.nfrag(nb)
+    pending = list(recv_order)
+    guard = 0
+    while pending:
+        pair.pump_sender()
+        k, use_any = pending[0]
+        tag, nb = messages[k]
+        if pair.try_recv(ANY_TAG if use_any else tag, nb):
+            pending.pop(0)
+            guard = 0
+        else:
+            guard += 1
+            assert guard < 4, "deadlock in the model: nothing can progress"
+    pair.pump_sender()
+    assert not pair.sendq, "sender still blocked after every message was received"
+    assert pair.head == s and pair.ooo == 0, (pair.head, s, bin(pair.ooo))
+    return [starts.index(seq0) for seq0, _, _ in pair.log]
+
+
+def _reachable(msgs, nfr, received, k):
+    """Can a tagged receive for message k see it?  Replays the scan of p2p_match on the send order:
+    holes (already received, single-fragment) cost one slot, older unreceived messages are hopped
+    over, a message whose fragments fill the rest of the window ends the scan."""
+    first = min(j for j in range(len(msgs)) if j not in received)
+    i = 0
+    for j in range(first, len(msgs)):
+        if i >= NSLOT:
+            return False
+        if j in received:
+            i += 1
+            continue
+        if j == k:
+            return i == 0 or nfr[k] == 1
+        if msgs[j][0] == msgs[k][0]:
+            return False                 # an older message with the same tag would be matched instead
+        if nfr[j] >= NSLOT - i:
+            return False
+        i += nfr[j]
+    return False

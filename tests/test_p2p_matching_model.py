@@ -1,54 +1,22 @@
 """Property tests of the p2p matching protocol against an MPI-semantics oracle, on the executable
-model in tests/_p2p_sim.py (the CUDA implementation it mirrors is exercised by
-tests/collective_ops/test_send_and_recv.py on GPUs)."""
+model in tests/_p2p_sim.py.  The CUDA implementation it mirrors runs schedules that this model
+completes, against the same oracle, in tests/collective_ops/test_p2p_kernels.py
+(test_p2p_schedules_checked_by_the_model)."""
 
 import random
 
 import pytest
 
-from ._p2p_sim import ANY_TAG, NSLOT, Fatal, Inbox, Pair
+from ._p2p_sim import ANY_TAG, NSLOT, Fatal, Inbox, Pair, _oracle, _reachable, _run
 
 
-def _oracle(messages, recv_tags):
-    """MPI matching: each receive takes the earliest not-yet-received message with its tag."""
-    taken, order = set(), []
-    for t in recv_tags:
-        for k, (tag, _) in enumerate(messages):
-            if k not in taken and (t == ANY_TAG or tag == t):
-                taken.add(k)
-                order.append(k)
-                break
-        else:
-            raise AssertionError("test generator produced an unmatched receive")
-    return order
+def test_the_model_has_the_kernels_ring_depth():
+    """NSLOT of the model is B2_P2P_NSLOT of the library the kernels were built with."""
+    from mpi4jax_b200._src import native
 
-
-def _run(messages, recv_order, slot_bytes=4):
-    """messages: [(tag, nbytes)] sent in order; recv_order: indices in the order they are received
-    (each receive uses the message's tag, or ANY_TAG when flagged)."""
-    pair = Pair(slot_bytes)
-    for tag, nb in messages:
-        pair.post_send(tag, nb)
-    starts, s = [], 0
-    for tag, nb in messages:
-        starts.append(s)
-        s += pair.nfrag(nb)
-    pending = list(recv_order)
-    guard = 0
-    while pending:
-        pair.pump_sender()
-        k, use_any = pending[0]
-        tag, nb = messages[k]
-        if pair.try_recv(ANY_TAG if use_any else tag, nb):
-            pending.pop(0)
-            guard = 0
-        else:
-            guard += 1
-            assert guard < 4, "deadlock in the model: nothing can progress"
-    pair.pump_sender()
-    assert not pair.sendq, "sender still blocked after every message was received"
-    assert pair.head == s and pair.ooo == 0, (pair.head, s, bin(pair.ooo))
-    return [starts.index(seq0) for seq0, _, _ in pair.log]
+    if not native.HAS_CUDA_EXT:
+        pytest.skip(f"the native library is not built: {native.CUDA_EXT_ERROR}")
+    assert native._abi_native(native.lib)["p2p_nslot"] == NSLOT
 
 
 def test_in_order_streaming_of_large_messages():
@@ -77,28 +45,6 @@ def test_streamed_message_cannot_overtake():
     msgs = [(3, 4), (5, 12)]
     with pytest.raises(Fatal, match="cannot overtake"):
         _run(msgs, [(1, False), (0, False)])
-
-
-def _reachable(msgs, nfr, received, k):
-    """Can a tagged receive for message k see it?  Replays the scan of p2p_match on the send order:
-    holes (already received, single-fragment) cost one slot, older unreceived messages are hopped
-    over, a message whose fragments fill the rest of the window ends the scan."""
-    first = min(j for j in range(len(msgs)) if j not in received)
-    i = 0
-    for j in range(first, len(msgs)):
-        if i >= NSLOT:
-            return False
-        if j in received:
-            i += 1
-            continue
-        if j == k:
-            return i == 0 or nfr[k] == 1
-        if msgs[j][0] == msgs[k][0]:
-            return False                 # an older message with the same tag would be matched instead
-        if nfr[j] >= NSLOT - i:
-            return False
-        i += nfr[j]
-    return False
 
 
 def test_random_schedules_match_the_mpi_oracle():
