@@ -1,7 +1,10 @@
 // mpi4jax_b200 -- device-side building blocks shared by every kernel:
 //   * system-scope acquire/release accessors for flags that live in peer HBM
-//   * spin-wait with a %globaltimer watchdog (deadlock -> diagnostics + trap,
-//     the analogue of the reference's abort_on_error, mpi_ops_common.h:60-78)
+//   * the %globaltimer watchdog of every spin wait (deadlock -> diagnostics + trap,
+//     the analogue of the reference's abort_on_error, mpi_ops_common.h:60-78) and
+//     the spin-waits on one flag word
+//   * the flag-in-data word ({value, flag} as one 8-byte store) and its poll
+//   * the last-arrival counter (the last CTA of a launch to finish does the epilogue)
 //   * the block-paired cross-GPU barrier (CTA b on every rank <-> CTA b)
 //   * the per-kernel ticket (staging parity + unique flag values, advanced on
 //     the device so CUDA-graph replays stay correct)
@@ -99,21 +102,35 @@ static __device__ __noinline__ void b2_fatal(const B2DevComm& c, int code, int o
   __trap();
 }
 
+// The watchdog of one spin wait: every PERIOD + 1 polls it reads %globaltimer; the first reading
+// starts the wait.  The caller reports with its own b2_fatal arguments:
+//   B2Watchdog<> wd;  while (!ready()) if (wd.expired(c)) b2_fatal(c, B2_ERR_TIMEOUT, ...);
+// (Keep the counter test, the clock read and the timeout test nested as written: a form that
+// returns early, or that computes the result into a flag, adds instructions to every kernel that spins.)
+template <unsigned PERIOD = 0xfffu>
+struct B2Watchdog {
+  unsigned long long t0 = 0;
+  unsigned spins = 0;
+  __device__ __forceinline__ bool expired(const B2DevComm& c) {
+    if ((++spins & PERIOD) == 0) {
+      const unsigned long long now = b2_gtime();
+      if (t0 == 0) t0 = now;
+      else if (now - t0 > c.timeout_ns) return true;
+    }
+    return false;
+  }
+};
+
 // Spin until `(int)(load(p) - want) >= 0` (monotone epochs, wrap-safe).
 __device__ __forceinline__ void b2_wait_ge(const B2DevComm& c, const unsigned* p, unsigned want,
                                            int opcode, int peer) {
   unsigned v = b2_ld_acquire_sys(p);
   if ((int)(v - want) >= 0) return;
-  unsigned long long t0 = 0;
-  unsigned spins = 0;
+  B2Watchdog<> wd;
   while (true) {
     v = b2_ld_acquire_sys(p);
     if ((int)(v - want) >= 0) return;
-    if ((++spins & 0xfffu) == 0) {
-      unsigned long long now = b2_gtime();
-      if (t0 == 0) t0 = now;
-      else if (now - t0 > c.timeout_ns) b2_fatal(c, B2_ERR_TIMEOUT, opcode, peer, want, v, 0);
-    }
+    if (wd.expired(c)) b2_fatal(c, B2_ERR_TIMEOUT, opcode, peer, want, v, 0);
   }
 }
 
@@ -122,16 +139,33 @@ __device__ __forceinline__ void b2_wait_eq(const B2DevComm& c, const unsigned* p
                                            int opcode, int peer) {
   unsigned v = b2_ld_acquire_sys(p);
   if (v == want) return;
-  unsigned long long t0 = 0;
-  unsigned spins = 0;
+  B2Watchdog<> wd;
   while (true) {
     v = b2_ld_acquire_sys(p);
     if (v == want) return;
-    if ((++spins & 0xfffu) == 0) {
-      unsigned long long now = b2_gtime();
-      if (t0 == 0) t0 = now;
-      else if (now - t0 > c.timeout_ns) b2_fatal(c, B2_ERR_TIMEOUT, opcode, peer, want, v, 1);
-    }
+    if (wd.expired(c)) b2_fatal(c, B2_ERR_TIMEOUT, opcode, peer, want, v, 1);
+  }
+}
+
+// ---------------------------------------------------------------------------
+// flag-in-data ("LL") words: {value, flag} travels as ONE 8-byte store; 8-byte stores are single
+// transactions, so a reader that sees the flag sees the value: no fence, no separate signal, one
+// NVLink one-way latency.  Used by the halo exchanges (b2_halo_ll.cuh) and small p2p messages.
+// ---------------------------------------------------------------------------
+__device__ __forceinline__ void b2_ll_put(uint2* p, unsigned v, unsigned flag) {
+  // no "memory" clobber: the value comes from registers and nothing in the kernel reads the
+  // (remote) target, so the compiler stays free to overlap other loads with the push
+  asm volatile("st.relaxed.sys.global.v2.u32 [%0], {%1, %2};" ::"l"(p), "r"(v), "r"(flag));
+}
+// Spin until the word at `p` carries `flag`; return its value.  opcode, peer, aux: the diagnostics.
+__device__ __forceinline__ unsigned b2_ll_poll(const B2DevComm& c, const uint2* p, unsigned flag,
+                                               int opcode, int peer, int aux) {
+  unsigned v, f;
+  B2Watchdog<> wd;
+  while (true) {
+    asm volatile("ld.volatile.global.v2.u32 {%0, %1}, [%2];" : "=r"(v), "=r"(f) : "l"(p) : "memory");
+    if (f == flag) return v;
+    if (wd.expired(c)) b2_fatal(c, B2_ERR_TIMEOUT, opcode, peer, flag, f, aux);
   }
 }
 
@@ -192,18 +226,22 @@ __device__ __forceinline__ unsigned b2_ticket_read(const unsigned* ticket) {
   return s_ticket;
 }
 
+// Thread 0 of each of `nblocks` CTAs calls once its CTA is done: fences the CTA's writes and counts
+// its arrival in *ctr.  True in the last CTA to arrive, which has reset the counter for the next use.
+__device__ __forceinline__ bool b2_last_arrival(unsigned* ctr, unsigned nblocks) {
+  __threadfence();
+  const bool last = atomicAdd(ctr, 1u) == nblocks - 1;
+  if (last) b2_st_volatile(ctr, 0u);
+  return last;
+}
+
 // All threads call; adds `delta` to *target once every one of `nblocks` CTAs is done.
 __device__ __forceinline__ void b2_finish_bump(unsigned* target, unsigned* ctr, unsigned delta,
                                                unsigned nblocks) {
   __syncthreads();
-  if (threadIdx.x == 0) {
+  if (threadIdx.x == 0 && b2_last_arrival(ctr, nblocks)) {
+    b2_st_volatile(target, b2_ld_volatile(target) + delta);
     __threadfence();
-    unsigned old = atomicAdd(ctr, 1u);
-    if (old == nblocks - 1) {
-      b2_st_volatile(ctr, 0u);
-      b2_st_volatile(target, b2_ld_volatile(target) + delta);
-      __threadfence();
-    }
   }
 }
 

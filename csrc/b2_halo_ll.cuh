@@ -1,8 +1,8 @@
 // mpi4jax_b200 -- flag-in-data ("LL") halo transport shared by the stand-alone exchange kernel
 // (b2_halo.cu) and the deep exchange of the communication-avoiding shallow-water step (b2_swe_ca.cu).
 //
-// A halo element travels as ONE 8-byte store {value, flag}; 8-byte stores are atomic, so a reader
-// that sees the flag sees the value: no fence, no separate signal, one NVLink one-way latency.
+// A halo element travels as one flag-in-data word {value, flag} (fz_put / fz_get over b2_ll_put /
+// b2_ll_poll in b2_device.cuh): no fence, no separate signal, one NVLink one-way latency.
 // flag = (messages sent on this side so far) + 1, buffer parity = that count & 1; both ends of
 // a channel count the same messages in device memory (c.ticket[TK_RX + side] / [TK_TX + side]), so
 // kernels using this transport can be mixed freely and replayed from CUDA graphs.
@@ -16,30 +16,12 @@ __device__ __forceinline__ uint2* fz_buf(const B2DevComm& c, int rank, unsigned 
   return (uint2*)(c.heap[rank] + c.lay.halo_ll_off +
                   ((size_t)parity * FS_NSIDES + side) * c.lay.halo_ll_cap);
 }
+// one halo element: a float as a flag-in-data word; a poll that times out reports the side (aux 5)
 __device__ __forceinline__ void fz_put(uint2* p, float v, unsigned flag) {
-  // no "memory" clobber: the value comes from registers and nothing in the kernel reads the
-  // (remote) target, so the compiler stays free to overlap other loads with the push
-  asm volatile("st.relaxed.sys.global.v2.u32 [%0], {%1, %2};" ::"l"(p), "r"(__float_as_uint(v)),
-               "r"(flag));
-}
-__device__ __forceinline__ void fz_put2(uint2* p, float v0, float v1, unsigned flag) {
-  asm volatile("st.relaxed.sys.global.v4.u32 [%0], {%1, %2, %3, %4};" ::"l"(p),
-               "r"(__float_as_uint(v0)), "r"(flag), "r"(__float_as_uint(v1)), "r"(flag));
+  b2_ll_put(p, __float_as_uint(v), flag);
 }
 __device__ __forceinline__ float fz_get(const B2DevComm& c, const uint2* p, unsigned flag, int side) {
-  unsigned v, f;
-  unsigned long long t0 = 0;
-  unsigned spins = 0;
-  while (true) {
-    asm volatile("ld.volatile.global.v2.u32 {%0, %1}, [%2];" : "=r"(v), "=r"(f) : "l"(p) : "memory");
-    if (f == flag) break;
-    if ((++spins & 0xfffu) == 0) {
-      unsigned long long now = b2_gtime();
-      if (t0 == 0) t0 = now;
-      else if (now - t0 > c.timeout_ns) b2_fatal(c, B2_ERR_TIMEOUT, B2_OPC_HALO, side, flag, f, 5);
-    }
-  }
-  return __uint_as_float(v);
+  return __uint_as_float(b2_ll_poll(c, p, flag, B2_OPC_HALO, side, 5));
 }
 
 // End of an exchange kernel: after every thread of the CTA is done, the last CTA to finish advances
@@ -47,17 +29,12 @@ __device__ __forceinline__ float fz_get(const B2DevComm& c, const uint2* p, unsi
 __device__ __forceinline__ void fz_finish(const B2DevComm& c, const int (&nb)[FS_NSIDES],
                                           const unsigned* s_rx, const unsigned* s_tx) {
   __syncthreads();
-  if (threadIdx.x == 0) {
+  if (threadIdx.x == 0 && b2_last_arrival(c.ticket + TK_FIN, gridDim.x)) {
+    for (int k = 0; k < FS_NSIDES; ++k)
+      if (nb[k] >= 0) {
+        b2_st_volatile(c.ticket + TK_RX + k, s_rx[k] + 1u);
+        b2_st_volatile(c.ticket + TK_TX + k, s_tx[k] + 1u);
+      }
     __threadfence();
-    const unsigned old = atomicAdd(c.ticket + TK_FIN, 1u);
-    if (old == gridDim.x - 1) {
-      b2_st_volatile(c.ticket + TK_FIN, 0u);
-      for (int k = 0; k < FS_NSIDES; ++k)
-        if (nb[k] >= 0) {
-          b2_st_volatile(c.ticket + TK_RX + k, s_rx[k] + 1u);
-          b2_st_volatile(c.ticket + TK_TX + k, s_tx[k] + 1u);
-        }
-      __threadfence();
-    }
   }
 }

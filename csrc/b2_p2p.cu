@@ -36,8 +36,9 @@
 // Small messages (<= B2_P2P_LL_MAX bytes) travel flag-in-data: every 4-byte word is pushed as one
 // 8-byte {word, seq + 1} store into the slot's LL area and the receiver polls the words themselves,
 // so the header needs no release fence over the payload and the message costs ONE NVLink one-way
-// latency (the halo kernels' transport, b2_halo_ll.cuh).  Matching, tags, Status and credits are
-// unchanged: the header is still written, its size field tells the receiver which format to read.
+// latency (b2_ll_put / b2_ll_poll, the halo kernels' transport too).  Matching, tags, Status and
+// credits are unchanged: the header is still written, its size field tells the receiver which format
+// to read.
 #include <cstring>
 
 #include "b2_device.cuh"
@@ -64,7 +65,7 @@ struct B2P2PArgs {
   int recv_lanes;      // 0 = no recv role
   B2StatusRecord* status;
   int opcode;
-  int anysource_scan;  // communicator option "p2p_anysource_scan" (see p2p_scan)
+  int anysource_scan;  // communicator option "p2p_anysource_scan" (see the election in p2p_recv_role)
 };
 
 // ---- flag-in-data transport of small messages ---------------------------------------------------
@@ -81,24 +82,6 @@ __device__ __forceinline__ void p2p_store_word(char* dst, size_t w, size_t nbyte
   if (b + 4 <= nbytes && (((uintptr_t)dst) & 3) == 0) { *reinterpret_cast<unsigned*>(dst + b) = v; return; }
   for (size_t k = 0; k < 4 && b + k < nbytes; ++k) dst[b + k] = (char)(v >> (8 * k));
 }
-__device__ __forceinline__ void p2p_ll_put(uint2* p, unsigned v, unsigned flag) {
-  asm volatile("st.relaxed.sys.global.v2.u32 [%0], {%1, %2};" ::"l"(p), "r"(v), "r"(flag));
-}
-__device__ __forceinline__ unsigned p2p_ll_get(const B2DevComm& c, const uint2* p, unsigned flag, int opcode, int src) {
-  unsigned v, f;
-  unsigned long long t0 = 0;
-  unsigned spins = 0;
-  while (true) {
-    asm volatile("ld.volatile.global.v2.u32 {%0, %1}, [%2];" : "=r"(v), "=r"(f) : "l"(p) : "memory");
-    if (f == flag) return v;
-    if ((++spins & 0xfffu) == 0) {
-      unsigned long long now = b2_gtime();
-      if (t0 == 0) t0 = now;
-      else if (now - t0 > c.timeout_ns) b2_fatal(c, B2_ERR_TIMEOUT, opcode, src, flag, f, 7);
-    }
-  }
-}
-
 // The 16-byte header {seq + 1, tag, bytes lo, bytes hi} travels as ONE vector store / load: a
 // receiver that sees the sequence word sees tag and size of the same store (16-byte aligned vector
 // accesses are single transactions on NVLink and in L2 -- what NCCL's LL128 protocol builds on).
@@ -113,6 +96,9 @@ __device__ __forceinline__ void p2p_hdr_put(unsigned* hdr, unsigned seq1, int ta
     asm volatile("st.relaxed.sys.global.v4.u32 [%0], {%1, %2, %3, %4};" ::"l"(hdr), "r"(seq1), "r"((unsigned)tag),
                  "r"(lo), "r"(hi) : "memory");
 }
+// Matching reads headers with this plain volatile load, not an acquire: it orders nothing read later.
+// Every lane matches for itself, a lane reads slot payload only after its own b2_wait_eq (acquire) on
+// its header, flag-in-data words carry their own flags, and the elected source is published after a fence.
 struct P2PHdr { unsigned seq1; int tag; unsigned long long nbytes; };
 __device__ __forceinline__ P2PHdr p2p_hdr_get(const unsigned* hdr) {
   unsigned a, b, c2, d;
@@ -122,16 +108,41 @@ __device__ __forceinline__ P2PHdr p2p_hdr_get(const unsigned* hdr) {
   return h;
 }
 
-__device__ __forceinline__ void stripe_of(size_t fraglen, int lanes, int lane, size_t* lo,
-                                          size_t* hi) {
-  size_t stripe = (fraglen + lanes - 1) / lanes;
+// ---- the ring of pair (s -> d): headers, slots and flag-in-data areas in d's heap (`dheap`), indexed by
+// s; acks in s's heap (`sheap`), indexed by d ----
+__device__ __forceinline__ unsigned* p2p_hdr(const B2DevComm& c, char* dheap, int s, unsigned slot, int lane) {
+  return (unsigned*)(dheap + c.lay.p2p_hdr_off) + (((size_t)s * B2_P2P_NSLOT + slot) * B2_P2P_MAX_LANES + lane) * 4;
+}
+__device__ __forceinline__ char* p2p_slot(const B2DevComm& c, char* dheap, int s, unsigned slot) {
+  return dheap + c.lay.p2p_slot_off + ((size_t)s * B2_P2P_NSLOT + slot) * c.lay.p2p_slot_bytes;
+}
+__device__ __forceinline__ uint2* p2p_ll(const B2DevComm& c, char* dheap, int s, unsigned slot) {
+  return (uint2*)(dheap + c.lay.p2p_ll_off + ((size_t)s * B2_P2P_NSLOT + slot) * (2 * B2_P2P_LL_MAX));
+}
+__device__ __forceinline__ unsigned* p2p_ack(const B2DevComm& c, char* sheap, int d, unsigned slot) {
+  return (unsigned*)(sheap + c.lay.p2p_ack_off) + (size_t)d * B2_P2P_NSLOT + slot;
+}
+
+__device__ __forceinline__ size_t p2p_nfrag(size_t nbytes, size_t slot_bytes) {
+  return nbytes == 0 ? 1 : (nbytes + slot_bytes - 1) / slot_bytes;
+}
+// Fragment f of a message whose first fragment is number seq0: its number, slot, offset in the
+// message and length, and the stripe [lo, hi) of it that lane `lane` of `lanes` moves.
+struct P2PFrag { unsigned fs, slot; size_t off, len, lo, hi; };
+__device__ __forceinline__ P2PFrag p2p_frag(size_t slot_bytes, size_t nbytes, unsigned seq0, size_t f, int lanes,
+                                            int lane) {
+  P2PFrag g;
+  g.fs = seq0 + (unsigned)f;
+  g.slot = g.fs % B2_P2P_NSLOT;
+  g.off = f * slot_bytes;
+  g.len = b2_chunk_len(nbytes, slot_bytes, f);
+  size_t stripe = (g.len + lanes - 1) / lanes;
   stripe = (stripe + 15) & ~(size_t)15;
-  size_t a = stripe * (size_t)lane;
-  if (a > fraglen) a = fraglen;
-  size_t b = a + stripe;
-  if (b > fraglen) b = fraglen;
-  *lo = a;
-  *hi = b;
+  g.lo = stripe * (size_t)lane;
+  if (g.lo > g.len) g.lo = g.len;
+  g.hi = g.lo + stripe;
+  if (g.hi > g.len) g.hi = g.len;
+  return g;
 }
 
 #define P2P_LL_WORDS_PER_THREAD ((B2_P2P_LL_MAX / 4 + B2_THREADS - 1) / B2_THREADS)
@@ -153,38 +164,26 @@ __device__ void p2p_send_role(const B2DevComm& c, const B2P2PArgs& a, int lane) 
     }
   }
   const unsigned seq0 = b2_ticket_read(c.p2p_send_seq + a.dest);
-  const size_t nfrag = a.send_bytes == 0 ? 1 : (a.send_bytes + slot_bytes - 1) / slot_bytes;
+  const size_t nfrag = p2p_nfrag(a.send_bytes, slot_bytes);
   for (size_t f = 0; f < nfrag; ++f) {
-    const unsigned fs = seq0 + (unsigned)f;
-    const unsigned slot = fs % B2_P2P_NSLOT;
-    const size_t fragoff = f * slot_bytes;
-    const size_t fraglen = (a.send_bytes - fragoff < slot_bytes) ? (a.send_bytes - fragoff) : slot_bytes;
-    size_t lo, hi;
-    stripe_of(fraglen, a.send_lanes, lane, &lo, &hi);
+    const P2PFrag g = p2p_frag(slot_bytes, a.send_bytes, seq0, f, a.send_lanes, lane);
     // credit: the previous occupant of this slot (fragment fs - NSLOT) has been consumed
-    if (threadIdx.x == 0) {
-      const unsigned* ack =
-          (const unsigned*)(c.heap[c.rank] + c.lay.p2p_ack_off) + (size_t)a.dest * B2_P2P_NSLOT + slot;
-      b2_wait_ge(c, ack, fs + 1u - B2_P2P_NSLOT, a.opcode, a.dest);
-    }
+    if (threadIdx.x == 0)
+      b2_wait_ge(c, p2p_ack(c, c.heap[c.rank], a.dest, g.slot), g.fs + 1u - B2_P2P_NSLOT, a.opcode, a.dest);
     __syncthreads();
     if (ll) {
-      uint2* area = (uint2*)(dheap + c.lay.p2p_ll_off + ((size_t)c.rank * B2_P2P_NSLOT + slot) * (2 * B2_P2P_LL_MAX));
+      uint2* area = p2p_ll(c, dheap, c.rank, g.slot);
 #pragma unroll
       for (int k = 0; k < P2P_LL_WORDS_PER_THREAD; ++k) {
         const size_t w = (size_t)k * B2_THREADS + threadIdx.x;
-        if (w < nw) p2p_ll_put(area + w, word[k], fs + 1u);
+        if (w < nw) b2_ll_put(area + w, word[k], g.fs + 1u);
       }
     } else {
-      char* dslot = dheap + c.lay.p2p_slot_off + ((size_t)c.rank * B2_P2P_NSLOT + slot) * slot_bytes;
-      b2_copy_bytes<false>(dslot + lo, src + fragoff + lo, hi - lo);
+      b2_copy_bytes<false>(p2p_slot(c, dheap, c.rank, g.slot) + g.lo, src + g.off + g.lo, g.hi - g.lo);
       __syncthreads();
     }
-    if (threadIdx.x == 0) {
-      unsigned* hdr = (unsigned*)(dheap + c.lay.p2p_hdr_off) +
-                      (((size_t)c.rank * B2_P2P_NSLOT + slot) * B2_P2P_MAX_LANES + lane) * 4;
-      p2p_hdr_put(hdr, fs + 1u, a.send_tag, a.send_bytes, !ll);
-    }
+    if (threadIdx.x == 0)
+      p2p_hdr_put(p2p_hdr(c, dheap, c.rank, g.slot, lane), g.fs + 1u, a.send_tag, a.send_bytes, !ll);
   }
   if (a.send_lanes == 1) {
     // the only CTA of the role knows the new value: no counter, no reload (kernel boundaries order it)
@@ -194,82 +193,57 @@ __device__ void p2p_send_role(const B2DevComm& c, const B2P2PArgs& a, int lane) 
   }
 }
 
-// Sequence number of the first fragment of the message a receive (src, tag) consumes.  Executed by
-// thread 0 of EVERY receiving lane on the lane-0 headers (every message has one): the pair state
-// (head, bitmap) only changes when a receive kernel finishes, headers arrive in sequence order and
-// the scan stops at the first fragment that has not arrived, so all lanes pick the same message.
-__device__ unsigned p2p_match(const B2DevComm& c, const B2P2PArgs& a, int src, unsigned head, unsigned ooo,
-                              P2PHdr* found) {
-  const size_t slot_bytes = c.lay.p2p_slot_bytes;
-  const unsigned* hdr_base = (const unsigned*)(c.heap[c.rank] + c.lay.p2p_hdr_off);
-  unsigned long long t0 = 0;
-  unsigned spins = 0;
-  while (true) {
-    unsigned i = 0;
-    while (i < B2_P2P_NSLOT) {
-      if ((ooo >> i) & 1u) { ++i; continue; }            // already consumed out of order
-      const unsigned sq = head + i;
-      const unsigned* h = hdr_base + (((size_t)src * B2_P2P_NSLOT + sq % B2_P2P_NSLOT) * B2_P2P_MAX_LANES) * 4;
-      const P2PHdr hd = p2p_hdr_get(h);
-      if (hd.seq1 != sq + 1u) break;                     // not here yet (nor anything behind it)
-      const unsigned long long nf = hd.nbytes == 0 ? 1 : (hd.nbytes + slot_bytes - 1) / slot_bytes;
-      if (a.recv_tag < 0 || hd.tag == a.recv_tag) {      // ANY_TAG: always the head of the queue
-        if (i != 0 && nf != 1)       // a streamed message cannot overtake (see the file header)
-          b2_fatal(c, B2_ERR_TAG_MISMATCH, a.opcode, src, (unsigned)a.recv_tag, (unsigned)hd.tag, 5);
-        *found = hd;
-        return sq;
-      }
-      if (nf >= B2_P2P_NSLOT - i) break;                  // its fragments fill the rest of the window
-      i += (unsigned)nf;
-    }
-    if ((++spins & 0x3ffu) == 0) {
-      unsigned long long now = b2_gtime();
-      if (t0 == 0) t0 = now;
-      else if (now - t0 > c.timeout_ns)
-        b2_fatal(c, B2_ERR_TIMEOUT, a.opcode, src, (unsigned)a.recv_tag, head, 6);
-    }
-  }
-}
-
-// Communicator option "p2p_anysource_scan" = 1: an ANY_SOURCE receive with a tag looks as deep into
-// every source's window as a receive from a named source does (p2p_scan), instead of at the oldest
-// pending message of each source only (the default).  The scanning variant is mirrored by the model
-// in tests/_p2p_sim.py (Inbox).
-//
-// Non-blocking single pass of the scan in p2p_match: does source `src` hold a message that a
-// receive with tag a.recv_tag may take right now?  (A streamed message that is not at the head is
-// "not available" here -- another source may match -- whereas p2p_match treats it as an error.)
-__device__ bool p2p_scan(const B2DevComm& c, const B2P2PArgs& a, int src) {
-  const unsigned head = b2_ld_volatile(c.p2p_recv_seq + src);
-  const unsigned* hdr_base = (const unsigned*)(c.heap[c.rank] + c.lay.p2p_hdr_off);
-  if (a.recv_tag < 0) {
-    const unsigned* h = hdr_base + (((size_t)src * B2_P2P_NSLOT + head % B2_P2P_NSLOT) * B2_P2P_MAX_LANES) * 4;
-    return b2_ld_acquire_sys(h) == head + 1u;
-  }
-  const unsigned ooo = b2_ld_volatile(c.p2p_ctl + CTL_OOO + src);
-  const size_t slot_bytes = c.lay.p2p_slot_bytes;
+// One pass over the window of source `src`: the `window` fragments from `head`, minus those consumed
+// out of order (bitmap `ooo`), read through the lane-0 headers (every message has one).  It stops
+// at the first fragment that has not arrived, and at the first message with the tag (ANY_TAG: the
+// head of the queue).  The pair state (head, bitmap) only changes when a receive kernel finishes
+// and headers arrive in sequence order, so every lane that walks the window finds the same message.
+enum { P2P_FOUND, P2P_NOT_YET, P2P_STREAMED_BEHIND };
+struct P2PFound { int res; unsigned seq; P2PHdr hd; };   // seq, hd: the message with the tag, if any
+__device__ P2PFound p2p_walk(const B2DevComm& c, int src, int tag, unsigned head, unsigned ooo, unsigned window) {
+  P2PFound m;
+  m.res = P2P_NOT_YET;
   unsigned i = 0;
-  while (i < B2_P2P_NSLOT) {
-    if ((ooo >> i) & 1u) { ++i; continue; }
+  while (i < window) {
+    if ((ooo >> i) & 1u) { ++i; continue; }            // already consumed out of order
     const unsigned sq = head + i;
-    const unsigned* h = hdr_base + (((size_t)src * B2_P2P_NSLOT + sq % B2_P2P_NSLOT) * B2_P2P_MAX_LANES) * 4;
-    if (b2_ld_acquire_sys(h) != sq + 1u) return false;
-    const int tag = (int)b2_ld_volatile(h + 1);
-    const unsigned long long nb =
-        (unsigned long long)b2_ld_volatile(h + 2) | ((unsigned long long)b2_ld_volatile(h + 3) << 32);
-    const unsigned long long nf = nb == 0 ? 1 : (nb + slot_bytes - 1) / slot_bytes;
-    if (tag == a.recv_tag) return i == 0 || nf == 1;
-    if (nf >= B2_P2P_NSLOT - i) return false;
+    const P2PHdr hd = p2p_hdr_get(p2p_hdr(c, c.heap[c.rank], src, sq % B2_P2P_NSLOT, 0));
+    if (hd.seq1 != sq + 1u) break;                     // not here yet (nor anything behind it)
+    const size_t nf = p2p_nfrag(hd.nbytes, c.lay.p2p_slot_bytes);
+    if (tag < 0 || hd.tag == tag) {
+      // a streamed message cannot overtake (see the file header)
+      m.res = i == 0 || nf == 1 ? P2P_FOUND : P2P_STREAMED_BEHIND;
+      m.seq = sq;
+      m.hd = hd;
+      break;
+    }
+    if (nf >= window - i) break;                       // its fragments fill the rest of the window
     i += (unsigned)nf;
   }
-  return false;
+  return m;
+}
+
+// Sequence number of the first fragment of the message a receive (src, tag) consumes.  Executed by
+// thread 0 of EVERY receiving lane.
+__device__ unsigned p2p_match(const B2DevComm& c, const B2P2PArgs& a, int src, unsigned head, unsigned ooo,
+                              P2PHdr* found) {
+  B2Watchdog<0x3ffu> wd;
+  while (true) {
+    const P2PFound m = p2p_walk(c, src, a.recv_tag, head, ooo, B2_P2P_NSLOT);
+    if (m.res == P2P_STREAMED_BEHIND)
+      b2_fatal(c, B2_ERR_TAG_MISMATCH, a.opcode, src, (unsigned)a.recv_tag, (unsigned)m.hd.tag, 5);
+    if (m.res == P2P_FOUND) {
+      *found = m.hd;
+      return m.seq;
+    }
+    if (wd.expired(c)) b2_fatal(c, B2_ERR_TIMEOUT, a.opcode, src, (unsigned)a.recv_tag, head, 6);
+  }
 }
 
 __device__ void p2p_recv_role(const B2DevComm& c, const B2P2PArgs& a, int lane) {
   __shared__ int s_src, s_tag;
   __shared__ unsigned s_seq0, s_head, s_ooo, s_gen;
   const size_t slot_bytes = c.lay.p2p_slot_bytes;
-  const unsigned* hdr_base = (const unsigned*)(c.heap[c.rank] + c.lay.p2p_hdr_off);
 
   // ---- resolve the source (ANY_SOURCE: lane 0 elects, the others follow) ----
   if (threadIdx.x == 0) {
@@ -277,45 +251,33 @@ __device__ void p2p_recv_role(const B2DevComm& c, const B2P2PArgs& a, int lane) 
     if (src < 0) {
       const unsigned gen = b2_ld_volatile(c.p2p_ctl + CTL_GEN) & 0xffffffu;
       if (lane == 0) {
-        unsigned long long t0 = 0;
-        unsigned spins = 0;
+        // The election probes the sources in turn for a message this receive may take now.  By default
+        // it looks at each source's oldest pending message only (a window of one fragment: bit 0 of the
+        // bitmap is never set at the head).  Communicator option "p2p_anysource_scan" = 1 looks as deep
+        // into every source's window as a receive from a named source does; a streamed message behind
+        // the head is "not here" then, since another source may match.  Both are mirrored by the model
+        // in tests/_p2p_sim.py (Inbox).
+        B2Watchdog<> wd;
         int probe = 0;
         while (src < 0) {
-          if (a.anysource_scan) {
-            if (p2p_scan(c, a, probe)) {
-              src = probe;
-              break;
-            }
-          } else {
-            const unsigned want = b2_ld_volatile(c.p2p_recv_seq + probe);
-            const unsigned* h =
-                hdr_base + (((size_t)probe * B2_P2P_NSLOT + want % B2_P2P_NSLOT) * B2_P2P_MAX_LANES) * 4;
-            if (b2_ld_acquire_sys(h) == want + 1u &&
-                (a.recv_tag < 0 || (int)b2_ld_volatile(h + 1) == a.recv_tag)) {
-              src = probe;
-              break;
-            }
+          const unsigned head = b2_ld_volatile(c.p2p_recv_seq + probe);
+          const unsigned ooo = a.anysource_scan ? b2_ld_volatile(c.p2p_ctl + CTL_OOO + probe) : 0u;
+          const unsigned window = a.anysource_scan ? B2_P2P_NSLOT : 1u;
+          if (p2p_walk(c, probe, a.recv_tag, head, ooo, window).res == P2P_FOUND) {
+            src = probe;
+            break;
           }
           probe = (probe + 1) % c.size;
-          if ((++spins & 0xfffu) == 0) {
-            unsigned long long now = b2_gtime();
-            if (t0 == 0) t0 = now;
-            else if (now - t0 > c.timeout_ns) b2_fatal(c, B2_ERR_TIMEOUT, a.opcode, -1, 0, 0, 3);
-          }
+          if (wd.expired(c)) b2_fatal(c, B2_ERR_TIMEOUT, a.opcode, -1, 0, 0, 3);
         }
         __threadfence();
         b2_st_volatile(c.p2p_ctl + CTL_ELECT, (gen << 8) | (unsigned)src);
       } else {
-        unsigned long long t0 = 0;
-        unsigned spins = 0;
+        B2Watchdog<> wd;
         while (true) {
           const unsigned w = b2_ld_volatile(c.p2p_ctl + CTL_ELECT);
           if ((w >> 8) == gen) { src = (int)(w & 0xffu); break; }
-          if ((++spins & 0xfffu) == 0) {
-            unsigned long long now = b2_gtime();
-            if (t0 == 0) t0 = now;
-            else if (now - t0 > c.timeout_ns) b2_fatal(c, B2_ERR_TIMEOUT, a.opcode, -1, gen, w, 4);
-          }
+          if (wd.expired(c)) b2_fatal(c, B2_ERR_TIMEOUT, a.opcode, -1, gen, w, 4);
         }
       }
     }
@@ -338,46 +300,33 @@ __device__ void p2p_recv_role(const B2DevComm& c, const B2P2PArgs& a, int lane) 
   const unsigned seq0 = s_seq0;
   const bool ll = p2p_is_ll(a.recv_bytes);
 
-  const size_t nfrag = a.recv_bytes == 0 ? 1 : (a.recv_bytes + slot_bytes - 1) / slot_bytes;
+  const size_t nfrag = p2p_nfrag(a.recv_bytes, slot_bytes);
   char* dst = (char*)a.recvbuf;
-  const char* myheap = c.heap[c.rank];
+  char* myheap = c.heap[c.rank];
   for (size_t f = 0; f < nfrag; ++f) {
-    const unsigned fs = seq0 + (unsigned)f;
-    const unsigned slot = fs % B2_P2P_NSLOT;
-    const size_t fragoff = f * slot_bytes;
-    const size_t fraglen = (a.recv_bytes - fragoff < slot_bytes) ? (a.recv_bytes - fragoff) : slot_bytes;
-    size_t lo, hi;
-    stripe_of(fraglen, a.recv_lanes, lane, &lo, &hi);
+    const P2PFrag g = p2p_frag(slot_bytes, a.recv_bytes, seq0, f, a.recv_lanes, lane);
     if (ll) {
       // flag-in-data: the words are polled themselves; nothing to wait for, nothing to fence
-      const uint2* area = (const uint2*)(myheap + c.lay.p2p_ll_off + ((size_t)src * B2_P2P_NSLOT + slot) * (2 * B2_P2P_LL_MAX));
+      const uint2* area = p2p_ll(c, myheap, src, g.slot);
       const size_t nw = (a.recv_bytes + 3) >> 2;
       for (size_t w = threadIdx.x; w < nw; w += blockDim.x)
-        p2p_store_word(dst, w, a.recv_bytes, p2p_ll_get(c, area + w, fs + 1u, a.opcode, src));
+        p2p_store_word(dst, w, a.recv_bytes, b2_ll_poll(c, area + w, g.fs + 1u, a.opcode, src, 7));
     } else {
       // this lane's stripe of the slot was written by the sender's lane of the same index: its header
       // (acquire) orders the payload loads
-      const unsigned* hdr = hdr_base + (((size_t)src * B2_P2P_NSLOT + slot) * B2_P2P_MAX_LANES + lane) * 4;
-      if (threadIdx.x == 0) b2_wait_eq(c, hdr, fs + 1u, a.opcode, src);
+      if (threadIdx.x == 0) b2_wait_eq(c, p2p_hdr(c, myheap, src, g.slot, lane), g.fs + 1u, a.opcode, src);
       __syncthreads();
-      const char* sslot = myheap + c.lay.p2p_slot_off + ((size_t)src * B2_P2P_NSLOT + slot) * slot_bytes;
-      b2_copy_bytes<true>(dst + fragoff + lo, sslot + lo, hi - lo);
+      b2_copy_bytes<true>(dst + g.off + g.lo, p2p_slot(c, myheap, src, g.slot) + g.lo, g.hi - g.lo);
     }
     __syncthreads();
     // credit back to the sender: every load of the slot has returned (their values were stored)
     if (threadIdx.x == 0) {
-      unsigned* ack = (unsigned*)(c.heap[src] + c.lay.p2p_ack_off) + (size_t)c.rank * B2_P2P_NSLOT + slot;
+      unsigned* ack = p2p_ack(c, c.heap[src], c.rank, g.slot);
       if (a.recv_lanes == 1) {
-        if (ll) b2_st_relaxed_sys(ack, fs + 1u);      // (the polled words were consumed: nothing left to order)
-        else b2_st_release_sys(ack, fs + 1u);
-      } else {
-        __threadfence();
-        unsigned* done = c.p2p_ctl + CTL_SLOT_DONE + slot;
-        const unsigned old = atomicAdd(done, 1u);
-        if (old == (unsigned)a.recv_lanes - 1u) {
-          b2_st_volatile(done, 0u);
-          b2_st_release_sys(ack, fs + 1u);
-        }
+        if (ll) b2_st_relaxed_sys(ack, g.fs + 1u);    // (the polled words were consumed: nothing left to order)
+        else b2_st_release_sys(ack, g.fs + 1u);
+      } else if (b2_last_arrival(c.p2p_ctl + CTL_SLOT_DONE + g.slot, (unsigned)a.recv_lanes)) {
+        b2_st_release_sys(ack, g.fs + 1u);
       }
     }
   }
@@ -393,12 +342,7 @@ __device__ void p2p_recv_role(const B2DevComm& c, const B2P2PArgs& a, int lane) 
   bool last = a.recv_lanes == 1;
   if (!last) {
     __syncthreads();
-    if (threadIdx.x == 0) {
-      __threadfence();
-      const unsigned old = atomicAdd(c.p2p_ctl + CTL_RECV_FIN, 1u);
-      last = old == (unsigned)a.recv_lanes - 1u;
-      if (last) b2_st_volatile(c.p2p_ctl + CTL_RECV_FIN, 0u);
-    }
+    if (threadIdx.x == 0) last = b2_last_arrival(c.p2p_ctl + CTL_RECV_FIN, (unsigned)a.recv_lanes);
   }
   if (threadIdx.x == 0 && last) {
     // (head, ooo, gen as read at entry: the pair state only changes here, at the end of a receive)

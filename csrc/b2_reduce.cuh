@@ -192,8 +192,7 @@ b2_k_allreduce_ll(const B2DevComm c, const B2LLArgs a) {
     }
     // gather + reduce in rank order (bitwise identical result on every rank)
     B2Vec<T> acc;
-    unsigned long long t0 = 0;
-    unsigned spins = 0;
+    B2Watchdog<> wd;
     for (int q = 0; q < c.size; ++q) {
       uint4 v;
       if (q == c.rank) {
@@ -205,12 +204,7 @@ b2_k_allreduce_ll(const B2DevComm c, const B2LLArgs a) {
           l = b2_ld_peer16(src);
           h = b2_ld_peer16(src + 16);
           if (l.y == flag && l.w == flag && h.y == flag && h.w == flag) break;
-          if ((++spins & 0xfffu) == 0) {
-            unsigned long long now = b2_gtime();
-            if (t0 == 0) t0 = now;
-            else if (now - t0 > c.timeout_ns)
-              b2_fatal(c, B2_ERR_TIMEOUT, a.opcode, q, flag, l.y, 2);
-          }
+          if (wd.expired(c)) b2_fatal(c, B2_ERR_TIMEOUT, a.opcode, q, flag, l.y, 2);
         }
         v = make_uint4(l.x, l.z, h.x, h.z);
       }

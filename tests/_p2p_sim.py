@@ -1,11 +1,12 @@
 """Executable model of the device-side point-to-point matching protocol (csrc/b2_p2p.cu):
 a ring of NSLOT slots per directed pair, fragments numbered consecutively, sender credits from
 per-slot acks, receiver state = (head, bitmap of slots consumed out of order).  Mirrors
-``p2p_send_role`` / ``p2p_match`` / the end-of-kernel update of ``p2p_recv_role`` line by line so
+``p2p_send_role`` / ``p2p_walk`` / the end-of-kernel update of ``p2p_recv_role`` line by line so
 that the algorithm can be property-tested on a machine without GPUs."""
 
 NSLOT = 8
 ANY_TAG = -1
+FOUND, NOT_YET, STREAMED_BEHIND = range(3)      # the three results of one pass over a window
 
 
 class Fatal(Exception):
@@ -50,13 +51,14 @@ class Pair:
         return progressed
 
     # ---- receiver -------------------------------------------------------------------------
-    def match(self, recv_tag):
-        """p2p_match: sequence number of the message to consume, or None (keep spinning)."""
+    def match(self, recv_tag, window=NSLOT):
+        """p2p_walk: one pass over the `window` fragments from the head.  Returns (FOUND, seq) of
+        the message to consume, (NOT_YET, None), or (STREAMED_BEHIND, seq) for a streamed message
+        with the tag that is not at the head.  With a window of one only bit 0 of the bitmap is
+        read, and it is never set at the head: the kernel's default election passes an empty one."""
         head, ooo = self.head, self.ooo
-        if recv_tag < 0:
-            return head
         i = 0
-        while i < NSLOT:
+        while i < window:
             if (ooo >> i) & 1:
                 i += 1
                 continue
@@ -65,19 +67,19 @@ class Pair:
             if seq1 != sq + 1:
                 break
             nf = self.nfrag(nb)
-            if tag == recv_tag:
-                if i != 0 and nf != 1:
-                    raise Fatal("a streamed message cannot overtake")
-                return sq
-            if nf >= NSLOT - i:
+            if recv_tag < 0 or tag == recv_tag:
+                return (FOUND if i == 0 or nf == 1 else STREAMED_BEHIND), sq
+            if nf >= window - i:
                 break
             i += nf
-        return None
+        return NOT_YET, None
 
     def try_recv(self, recv_tag, recv_bytes):
         """One receive kernel; returns False if it cannot complete yet (would spin)."""
-        seq0 = self.match(recv_tag)
-        if seq0 is None:
+        res, seq0 = self.match(recv_tag)
+        if res == STREAMED_BEHIND:
+            raise Fatal("a streamed message cannot overtake")
+        if res == NOT_YET:
             return False
         nfrag = self.nfrag(recv_bytes)
         for f in range(nfrag):
@@ -109,37 +111,15 @@ class Pair:
         return True
 
 
-    # ---- ANY_SOURCE support (communicator option p2p_anysource_scan) -----------------------
-    def scan(self, recv_tag):
-        """Non-blocking variant of match() used by the ANY_SOURCE election: sequence number of the
-        message a receive with this tag would take from this source right now, or None.  A streamed
-        message that is not at the head is simply 'not available' here (another source may match)."""
-        head, ooo = self.head, self.ooo
-        if recv_tag < 0:
-            return head if self.hdr[head % NSLOT][0] == head + 1 else None
-        i = 0
-        while i < NSLOT:
-            if (ooo >> i) & 1:
-                i += 1
-                continue
-            sq = head + i
-            seq1, tag, nb = self.hdr[sq % NSLOT]
-            if seq1 != sq + 1:
-                return None
-            nf = self.nfrag(nb)
-            if tag == recv_tag:
-                return sq if (i == 0 or nf == 1) else None
-            if nf >= NSLOT - i:
-                return None
-            i += nf
-        return None
-
-
 class Inbox:
-    """All directed pairs that end at one receiver: ANY_SOURCE receives (device-side election)."""
+    """All directed pairs that end at one receiver: ANY_SOURCE receives (device-side election).
+    `scan`: the communicator option p2p_anysource_scan; the election looks into every source's
+    window if set, at the oldest pending message of each source (a window of one) if not.  A
+    streamed message behind the head is 'not here' for the election: another source may match."""
 
-    def __init__(self, nsources, slot_bytes=4):
+    def __init__(self, nsources, scan, slot_bytes=4):
         self.pairs = [Pair(slot_bytes) for _ in range(nsources)]
+        self.window = NSLOT if scan else 1
         self.probe = 0
 
     def try_recv_any(self, recv_tag):
@@ -150,12 +130,12 @@ class Inbox:
             self.probe = (self.probe + 1) % n
             pair = self.pairs[src]
             pair.pump_sender()
-            sq = pair.scan(recv_tag)
-            if sq is None:
+            res, sq = pair.match(recv_tag, self.window)
+            if res != FOUND:
                 continue
             _, tag, nb = pair.hdr[sq % NSLOT]
             # the followers (and lane 0 itself) now run the blocking match on the elected source
-            assert pair.match(recv_tag) == sq
+            assert pair.match(recv_tag) == (FOUND, sq)
             assert pair.try_recv(recv_tag, nb)
             return src, tag, nb
         return None
@@ -205,7 +185,7 @@ def _run(messages, recv_order, slot_bytes=4):
 
 
 def _reachable(msgs, nfr, received, k):
-    """Can a tagged receive for message k see it?  Replays the scan of p2p_match on the send order:
+    """Can a tagged receive for message k see it?  Replays the walk of p2p_match on the send order:
     holes (already received, single-fragment) cost one slot, older unreceived messages are hopped
     over, a message whose fragments fill the rest of the window ends the scan."""
     first = min(j for j in range(len(msgs)) if j not in received)

@@ -7,7 +7,7 @@ import random
 
 import pytest
 
-from ._p2p_sim import ANY_TAG, NSLOT, Fatal, Inbox, Pair, _oracle, _reachable, _run
+from ._p2p_sim import ANY_TAG, FOUND, NOT_YET, NSLOT, Fatal, Inbox, Pair, _oracle, _reachable, _run
 
 
 def test_the_model_has_the_kernels_ring_depth():
@@ -77,52 +77,62 @@ def test_unreachable_message_is_a_deadlock_not_a_wrong_match():
     for tag, nb in msgs:
         pair.post_send(tag, nb)
     pair.pump_sender()
-    assert pair.match(9) is None
+    assert pair.match(9) == (NOT_YET, None)
     assert pair.try_recv(0, 4)           # consuming the head opens the window
     pair.pump_sender()
-    assert pair.match(9) == NSLOT
+    assert pair.match(9) == (FOUND, NSLOT)
 
 
 def test_any_source_receives_respect_per_source_order():
-    """ANY_SOURCE with a tag (election scans every source's window): whatever source is picked, the
-    message is that source's earliest pending one with the tag; every message is received once."""
-    rng = random.Random(99)
-    for _ in range(1500):
-        nsrc = rng.randint(1, 5)
-        inbox = Inbox(nsrc)
-        pending = [[] for _ in range(nsrc)]           # per source: (tag, nbytes) still to be received
-        for s in range(nsrc):
-            for _ in range(rng.randint(0, 6)):        # <= 6 single-fragment messages: all inside the window
-                tag, nb = rng.randint(0, 3), rng.choice([0, 1, 4])
-                inbox.pairs[s].post_send(tag, nb)
-                pending[s].append((tag, nb))
-        total = sum(len(q) for q in pending)
-        for _ in range(total):
-            tags = sorted({t for q in pending for t, _ in q})
-            want = ANY_TAG if rng.random() < 0.25 else rng.choice(tags)
-            got = inbox.try_recv_any(want)
-            assert got is not None, (pending, want)
-            src, tag, nb = got
-            assert want == ANY_TAG or tag == want
-            if want == ANY_TAG:
-                assert pending[src][0] == (tag, nb)            # the head of that source's queue
-                pending[src].pop(0)
-            else:
-                k = next(i for i, (t, _) in enumerate(pending[src]) if t == want)
-                assert pending[src][k] == (tag, nb)            # earliest with that tag from that source
-                pending[src].pop(k)
-        assert all(not q for q in pending)
-        assert all(p.ooo == 0 and not p.sendq for p in inbox.pairs)
+    """ANY_SOURCE with a tag, in both election modes (the election looks at every source's window, or
+    at each source's oldest pending message): whatever source is picked, the message is that source's
+    earliest pending one with the tag; every message is received once."""
+    for scan in (False, True):
+        rng = random.Random(99)
+        for _ in range(1500):
+            nsrc = rng.randint(1, 5)
+            inbox = Inbox(nsrc, scan)
+            pending = [[] for _ in range(nsrc)]           # per source: (tag, nbytes) still to be received
+            for s in range(nsrc):
+                for _ in range(rng.randint(0, 6)):        # <= 6 single-fragment messages: all inside the window
+                    tag, nb = rng.randint(0, 3), rng.choice([0, 1, 4])
+                    inbox.pairs[s].post_send(tag, nb)
+                    pending[s].append((tag, nb))
+            total = sum(len(q) for q in pending)
+            for _ in range(total):
+                # tags the election can find: anywhere in a window when it scans, at a head when it does not
+                tags = sorted({t for q in pending for t, _ in (q if scan else q[:1])})
+                want = ANY_TAG if rng.random() < 0.25 else rng.choice(tags)
+                got = inbox.try_recv_any(want)
+                assert got is not None, (scan, pending, want)
+                src, tag, nb = got
+                assert want == ANY_TAG or tag == want
+                if want == ANY_TAG:
+                    assert pending[src][0] == (tag, nb)            # the head of that source's queue
+                    pending[src].pop(0)
+                else:
+                    k = next(i for i, (t, _) in enumerate(pending[src]) if t == want)
+                    assert pending[src][k] == (tag, nb)            # earliest with that tag from that source
+                    pending[src].pop(k)
+            assert all(not q for q in pending)
+            assert all(p.ooo == 0 and not p.sendq for p in inbox.pairs)
 
 
 def test_any_source_skips_sources_without_a_match():
-    inbox = Inbox(3)
-    inbox.pairs[0].post_send(1, 4)
-    inbox.pairs[1].post_send(2, 4)
-    inbox.pairs[1].post_send(7, 4)
-    inbox.pairs[2].post_send(3, 40)                    # streamed message at the head of source 2
-    inbox.pairs[2].post_send(7, 40)                    # streamed, not at the head: not available yet
-    assert inbox.try_recv_any(7) == (1, 7, 4)          # taken out of order from source 1
-    assert inbox.try_recv_any(7) is None               # source 2's tag-7 message is behind a streamed one
-    assert inbox.try_recv_any(3) == (2, 3, 40)
-    assert inbox.try_recv_any(7) == (2, 7, 40)
+    """Both election modes skip sources that hold nothing this receive may take."""
+    for scan in (False, True):
+        inbox = Inbox(3, scan)
+        inbox.pairs[0].post_send(1, 4)
+        inbox.pairs[1].post_send(2, 4)
+        inbox.pairs[1].post_send(7, 4)
+        inbox.pairs[2].post_send(3, 40)                    # streamed message at the head of source 2
+        inbox.pairs[2].post_send(7, 40)                    # streamed, not at the head: not available yet
+        if scan:
+            assert inbox.try_recv_any(7) == (1, 7, 4)      # taken out of order from source 1
+        else:
+            assert inbox.try_recv_any(7) is None           # no source has tag 7 at its head
+            assert inbox.try_recv_any(2) == (1, 2, 4)
+            assert inbox.try_recv_any(7) == (1, 7, 4)      # now at the head of source 1
+        assert inbox.try_recv_any(7) is None               # source 2's tag-7 message is behind a streamed one
+        assert inbox.try_recv_any(3) == (2, 3, 40)
+        assert inbox.try_recv_any(7) == (2, 7, 40)
