@@ -359,9 +359,8 @@ static B2Layout make_layout(int nranks, size_t slot_bytes, size_t ll_cap, size_t
   L.p2p_slot_bytes = round_up(slot_bytes, 4096);
   L.p2p_slot_off = take((size_t)nranks * B2_P2P_NSLOT * L.p2p_slot_bytes);
   L.p2p_ll_off = take((size_t)nranks * B2_P2P_NSLOT * 2 * B2_P2P_LL_MAX);
-  // 8 B per element: room for halo_cap payload bytes per side, plus the padding of every field's
-  // stride to a multiple of 4 elements (b2_halo_exchange): up to 3 x 8 B per field
-  L.halo_ll_cap = 2 * round_up(halo_cap, 4096) + 3 * 8 * B2_HALO_MAX_FIELDS;
+  // 8 B per element: room for halo_cap payload bytes per side
+  L.halo_ll_cap = 2 * round_up(halo_cap, 4096);
   L.halo_ll_off = take(2 * 8 * L.halo_ll_cap);
   L.total = off;
   return L;

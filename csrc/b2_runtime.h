@@ -278,6 +278,9 @@ void b2_set_error(const char* fmt, ...) __attribute__((format(printf, 1, 2)));
 int b2_cuda_check(cudaError_t e, const char* fmt, ...) __attribute__((format(printf, 2, 3)));
 // after a kernel launch: counts it (b2_launch_count), then b2_cuda_check(cudaGetLastError(), "<name>: kernel launch failed")
 int b2_launched(B2Comm* c, const char* name);
+// argument checks shared by the halo exchanges (b2_halo.cu): 0, or B2_ERR_BAD_ARG with the error "<what>: ..."
+int b2_halo_check_ranks(B2Comm* c, const B2HaloDesc* d, const char* what);
+int b2_halo_check_cap(B2Comm* c, int nfields, int depth, int ny, int nx, const char* what);
 // per-call debug log (b2_logging.cpp): `fmt` (may be null) formats the details only when logging is on
 struct B2DebugScope;
 B2DebugScope* b2_debug_begin(B2Comm* c, const char* opname, cudaStream_t stream, const char* fmt, ...)

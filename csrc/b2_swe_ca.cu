@@ -227,46 +227,12 @@ struct CAExt3 { float* a[CA_NF]; };
 __global__ void __launch_bounds__(CA_THREADS) b2_k_halo_ca(const B2DevComm c, const B2HaloDesc d,
                                                            const CAExt3 ext, const int epitch, const CAStamp ts) {
   ca_stamp_begin(ts);
-  __shared__ unsigned s_rx[FS_NSIDES], s_tx[FS_NSIDES];
-  __shared__ int s_cnt[FS_NSIDES + 1];
-  const int gt = blockIdx.x * blockDim.x + threadIdx.x, gn = gridDim.x * blockDim.x;
-  const int ny = d.ny, nx = d.nx;
-  const size_t pitch = (size_t)d.pitch;
-  const int nb[FS_NSIDES] = {d.west, d.east, d.south, d.north, d.sw, d.se, d.nw, d.ne};
-  const int opp[FS_NSIDES] = {CA_E, CA_W, CA_N, CA_S, CA_NE, CA_NW, CA_SE, CA_SW};
-  if (threadIdx.x < FS_NSIDES) {
-    s_rx[threadIdx.x] = b2_ld_volatile(c.ticket + TK_RX + threadIdx.x);
-    s_tx[threadIdx.x] = b2_ld_volatile(c.ticket + TK_TX + threadIdx.x);
-  }
-  if (threadIdx.x == 0) {
-    int acc = 0;
-    for (int k = 0; k < FS_NSIDES; ++k) {
-      s_cnt[k] = acc;
-      if (nb[k] >= 0) acc += ca_msg_count(ny, nx, k);     // |message towards k| == |message landing on k|
-    }
-    s_cnt[FS_NSIDES] = acc;
-  }
-  __syncthreads();
-  const int total = s_cnt[FS_NSIDES];
-  // ---------------- push ----------------
-  for (int k = gt; k < total; k += gn) {
-    int s = 0;
-    while (k >= s_cnt[s + 1]) ++s;
-    const int e = k - s_cnt[s], land = opp[s];
-    int f, js, is, jr, ir, layer;
-    ca_msg_elem(ny, nx, land, e, f, js, is, jr, ir, layer);
-    fz_put(fz_buf(c, nb[s], s_tx[s] & 1u, land) + e, d.field[f][(size_t)js * pitch + is], s_tx[s] + 1u);
-  }
-  // ---------------- poll + scatter ----------------
-  const int jlo = (d.south >= 0) ? 1 : 0, jhi = (d.north >= 0) ? ny - 1 : ny;
-  for (int k = gt; k < total; k += gn) {
-    int s = 0;
-    while (k >= s_cnt[s + 1]) ++s;
-    const int e = k - s_cnt[s];
-    const float val = fz_get(c, fz_buf(c, c.rank, s_rx[s] & 1u, s) + e, s_rx[s] + 1u, s);
-    ca_scatter(ny, nx, pitch, epitch, s, e, jlo, jhi, val, d.field, ext.a);
-  }
-  fz_finish(c, nb, s_rx, s_tx);
+  // (jlo, jhi computed inside the rule: hoisted into the kernel they change its register allocation,
+  // and the exchange, which is on the step's critical path, measured about 1.5 us per step slower)
+  fz_exchange<CA_L>(c, d, CA_NF, [&](int side, int e, float val) {
+    const int jlo = (d.south >= 0) ? 1 : 0, jhi = (d.north >= 0) ? d.ny - 1 : d.ny;
+    ca_scatter(d.ny, d.nx, (size_t)d.pitch, epitch, side, e, jlo, jhi, val, d.field, ext.a);
+  });
   ca_stamp_end(ts);
 }
 
@@ -304,13 +270,7 @@ static int ca_check(B2Comm* c, const B2SweParams& p, const B2SweCA& x) {
     b2_set_error("swe_ca: ext arrays missing or too narrow (epitch %d < nx + 4)", x.epitch);
     return B2_ERR_BAD_ARG;
   }
-  const size_t need = (size_t)CA_NF * CA_L * (size_t)(p.ny > p.nx ? p.ny : p.nx) * sizeof(uint2);
-  if (need > c->dev.lay.halo_ll_cap) {
-    b2_set_error("swe_ca: halo buffers too small (%zu > %zu); raise MPI4JAX_B200_HALO_BYTES", need,
-                 c->dev.lay.halo_ll_cap);
-    return B2_ERR_BAD_ARG;
-  }
-  return 0;
+  return b2_halo_check_cap(c, CA_NF, CA_L, p.ny, p.nx, "swe_ca");
 }
 
 // timeline buffer: [step][kernel 0 = A, 1 = S, 2 = X, 3 = D][start, end]
@@ -348,15 +308,11 @@ static int ca_exchange(B2Comm* c, const B2HaloDesc& topo, const B2SweParams& p, 
   d.field[2] = f2; d.kind[2] = 2;
   CAExt3 ext;
   ext.a[0] = x.hx; ext.a[1] = x.upx; ext.a[2] = x.vpx;
+  if (int rc = b2_halo_check_ranks(c, &d, "swe_ca")) return rc;
+  const int nb[HALO_NSIDES] = {d.west, d.east, d.south, d.north, d.sw, d.se, d.nw, d.ne};
   long long total = 0;
-  const int nb[8] = {d.west, d.east, d.south, d.north, d.sw, d.se, d.nw, d.ne};
-  for (int k = 0; k < 8; ++k) {
-    if (nb[k] < -1 || nb[k] >= c->dev.size) {
-      b2_set_error("swe_ca: invalid neighbour rank %d", nb[k]);
-      return B2_ERR_BAD_ARG;
-    }
+  for (int k = 0; k < HALO_NSIDES; ++k)
     if (nb[k] >= 0) total += ca_msg_count(p.ny, p.nx, k);
-  }
   unsigned ctas = ca_blocks(total, CA_THREADS);          // pure latency: about one element per thread
   if (ctas < 8) ctas = 8;
   if (ctas > 120) ctas = 120;                            // all co-resident next to the bulk kernel's CTAs

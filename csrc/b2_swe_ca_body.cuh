@@ -37,6 +37,7 @@
 // neighbours' cells, layers 1..2 / 1).  Only their outer cells are ever touched.
 #pragma once
 
+#include "b2_halo_geom.h"
 #include "b2_swe_body.cuh"
 
 #ifndef __CUDACC__
@@ -396,56 +397,15 @@ __device__ __forceinline__ void swe_ca_fric_task(const CACtx& c, const CAFrame& 
   else swe_ca_fric_finish(c, ua_out, va_out, j, i, upp);
 }
 
-// ---- exchange geometry -----------------------------------------------------------------------------
-// Element e of the message that LANDS on receiver side `side` (FS_W = it comes from the west
-// neighbour, ...): field f, the sender's cell (js, is), the receiver's cell (jr, ir) and the layer
-// (0 = the main arrays' halo cell).  W / E messages are full height (rows 0 .. ny-1; at a y wall
-// the wall-row values ride along, as in b2_halo.cu), S / N messages cover the interior columns,
-// corner messages are CA_L x CA_L blocks.
-enum { CA_W = 0, CA_E, CA_S, CA_N, CA_SW, CA_SE, CA_NW, CA_NE };
+// ---- exchange geometry: the eight-side messages of b2_halo_geom.h at CA_NF fields, CA_L layers deep -----
 __host__ __device__ inline int ca_msg_count(int ny, int nx, int side) {
-  if (side <= CA_E) return CA_NF * CA_L * ny;
-  if (side <= CA_N) return CA_NF * CA_L * (nx - 2);
-  return CA_NF * CA_L * CA_L;
+  return halo_msg_count(CA_NF, CA_L, ny, nx, side);
 }
 __host__ __device__ inline void ca_msg_elem(int ny, int nx, int side, int e, int& f, int& js, int& is, int& jr,
                                             int& ir, int& layer) {
-  if (side <= CA_E) {
-    f = e / (CA_L * ny);
-    const int l = (e / ny) % CA_L, j = e % ny;
-    layer = l; js = jr = j;
-    if (side == CA_W) { is = nx - 2 - l; ir = -l; }
-    else              { is = 1 + l;      ir = nx - 1 + l; }
-  } else if (side <= CA_N) {
-    const int n = nx - 2;
-    f = e / (CA_L * n);
-    const int l = (e / n) % CA_L, i = 1 + e % n;
-    layer = l; is = ir = i;
-    if (side == CA_S) { js = ny - 2 - l; jr = -l; }
-    else              { js = 1 + l;      jr = ny - 1 + l; }
-  } else {
-    f = e / (CA_L * CA_L);
-    const int lj = (e / CA_L) % CA_L, li = e % CA_L;
-    layer = lj > li ? lj : li;
-    if (side == CA_SW)      { js = ny - 2 - lj; is = nx - 2 - li; jr = -lj;         ir = -li; }
-    else if (side == CA_SE) { js = ny - 2 - lj; is = 1 + li;      jr = -lj;         ir = nx - 1 + li; }
-    else if (side == CA_NW) { js = 1 + lj;      is = nx - 2 - li; jr = ny - 1 + lj; ir = -li; }
-    else                    { js = 1 + lj;      is = 1 + li;      jr = ny - 1 + lj; ir = nx - 1 + li; }
-  }
+  halo_msg_elem(CA_L, ny, nx, side, e, f, js, is, jr, ir, layer);
 }
-// where element e of the message landing on `side` goes on the receiver: every layer into the ext
-// arrays (W / E messages: interior rows only, the corner rows come from the diagonal neighbours),
-// layer 1 also into the main arrays' halo ([jlo, jhi) = the rows of the halo columns b2_halo.cu fills)
 __host__ __device__ inline void ca_scatter(int ny, int nx, size_t pitch, int epitch, int side, int e, int jlo,
                                            int jhi, float val, float* const* field, float* const* ext) {
-  int f, js, is, jr, ir, layer;
-  ca_msg_elem(ny, nx, side, e, f, js, is, jr, ir, layer);
-  const size_t eoff = (size_t)(jr + 2) * epitch + (ir + 2);
-  if (side <= CA_E) {
-    if (jr >= 1 && jr <= ny - 2) ext[f][eoff] = val;
-    if (layer == 0 && jr >= jlo && jr < jhi) field[f][(size_t)jr * pitch + ir] = val;
-  } else {
-    ext[f][eoff] = val;
-    if (layer == 0) field[f][(size_t)jr * pitch + ir] = val;
-  }
+  halo_scatter_deep(CA_L, ny, nx, pitch, epitch, side, e, jlo, jhi, val, field, ext);
 }

@@ -5,7 +5,8 @@
 // bulk kernel with its 32 lanes in lockstep, frame kernels with owner views, deep halo exchange
 // geometry, bulk / frame partition, ping-pong storage) against the stand-alone K1 -> K2 -> K34 -> K5
 // pipeline, bit for bit (every rounding in the bodies is explicit, so host and device agree on the
-// arithmetic).
+// arithmetic).  The halo exchanges' message geometry and receive rules (csrc/b2_halo_geom.h) are
+// compiled here as well.
 // Build: g++ -O1 -ffp-contract=off -shared -fPIC -I csrc -I $CUDA/include tests/native/swe_host_emu.cpp
 #include <cmath>
 #include <cstring>
@@ -178,7 +179,8 @@ void emu_ca_marks(const B2SweParams* p, int rows, int* marks) {
 }
 
 // the message that lands on `side` of the receiver: read from the sender's arrays exactly as the push
-// loop of b2_k_halo_ca does, scattered exactly as its poll loop does (no transport in between)
+// loop of fz_exchange (b2_halo_ll.cuh) does, received exactly as its poll loop hands it to the receive
+// rule of b2_k_halo_ca (emu_ca_deliver) or of b2_k_halo_ll (emu_halo_deliver); no transport in between
 void emu_ca_deliver(int ny, int nx, int pitch, int epitch, int side, int recv_has_south, int recv_has_north,
                     float* const* send_field, float* const* recv_field, float* const* recv_ext) {
   const int jlo = recv_has_south ? 1 : 0, jhi = recv_has_north ? ny - 1 : ny;
@@ -188,6 +190,22 @@ void emu_ca_deliver(int ny, int nx, int pitch, int epitch, int side, int recv_ha
     ca_scatter(ny, nx, (size_t)pitch, epitch, side, e, jlo, jhi, send_field[f][(size_t)js * pitch + is], recv_field,
                recv_ext);
   }
+}
+void emu_halo_deliver(int ny, int nx, int pitch, int nf, const int* kind, int side, int recv_has_south,
+                      int recv_has_north, int uwall, int vwall, float* const* send_field, float* const* recv_field) {
+  const int jlo = recv_has_south ? 1 : 0, jhi = recv_has_north ? ny - 1 : ny;
+  for (int e = 0; e < halo_msg_count(nf, 1, ny, nx, side); ++e) {
+    int f, js, is, jr, ir, layer;
+    halo_msg_elem(1, ny, nx, side, e, f, js, is, jr, ir, layer);
+    halo_recv_walls(ny, nx, (size_t)pitch, side, e, jlo, jhi, uwall != 0, vwall != 0,
+                    send_field[f][(size_t)js * pitch + is], recv_field, kind);
+  }
+}
+// b2_k_halo_ll's closing wall pass, one thread
+void emu_halo_wall_pass(int ny, int nx, int pitch, int nf, const int* kind, int has_west, int has_east, int has_south,
+                        int has_north, int uwall, int vwall, float* const* field) {
+  halo_wall_pass(ny, nx, (size_t)pitch, nf, has_south ? 1 : 0, has_north ? ny - 1 : ny, has_west ? 1 : 0,
+                 has_east ? nx - 1 : nx, uwall != 0, vwall != 0, field, kind, 0, 1);
 }
 
 // swe_ca_init_ext

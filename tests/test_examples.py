@@ -185,9 +185,9 @@ def test_ca_pipeline_under_a_cuda_graph_and_after_load_state():
 @pytest.mark.gpu
 def test_halo_exchange_at_the_halo_buffer_limit(monkeypatch):
     """ops.halo_exchange on three float32 fields whose longer side (341) is not a multiple of 4, on a
-    communicator with 4 KiB halo buffers: 3 * 341 * 4 bytes fit the payload capacity, the padded
-    flag-in-data stride (3 * 344 * 8 bytes) needs the slack the buffers are sized with.  The result
-    must match the numpy model of the 8-neighbour exchange."""
+    communicator with 4 KiB halo buffers: the longest message, 3 * 341 flag-in-data words of 8 bytes
+    (8184 bytes), just fits the 8192-byte buffer of a side.  The result must match the numpy model of
+    the 8-neighbour exchange."""
     import numpy as np
 
     from mpi4jax_b200.ops import halo_exchange

@@ -48,7 +48,7 @@ def test_emulated_native_step_matches_the_ops_backend(emu):
 
 
 # ---- communication-avoiding step (csrc/b2_swe_ca_body.cuh, b2_swe_ca_bulk.cuh, b2_swe_ca.cu) ------------
-_SIDES = ("w", "e", "s", "n", "sw", "se", "nw", "ne")        # CA_W .. CA_NE: where a message lands
+_SIDES = ("w", "e", "s", "n", "sw", "se", "nw", "ne")        # HALO_W .. HALO_NE: where a message lands
 
 
 def _neighbours(r, PY, PX):

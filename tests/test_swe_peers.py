@@ -251,7 +251,8 @@ def test_halo_exchange_with_peers(device):
 
 def _halo_buffer_limit(device, chk, grid, periodic_x):
     """Three fields whose longer side (341) is not a multiple of 4 on a communicator with 4 KiB halo
-    buffers, as test_examples.py::test_halo_exchange_at_the_halo_buffer_limit, with peers."""
+    buffers: the longest message (3 * 341 words of 8 bytes) just fits a side's 8192-byte buffer, as in
+    test_examples.py::test_halo_exchange_at_the_halo_buffer_limit, with peers."""
     old = os.environ.get("MPI4JAX_B200_HALO_BYTES")
     os.environ["MPI4JAX_B200_HALO_BYTES"] = "4096"
     try:
