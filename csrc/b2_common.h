@@ -26,6 +26,11 @@
 #define B2_P2P_MAX_LANES 64      // CTAs cooperating on one p2p message
 #define B2_P2P_LL_MAX 8192       // payload bytes up to which a p2p message travels flag-in-data
 #define B2_HALO_MAX_FIELDS 8
+// arrival words of the fused allgather + GEMM (b2_gemm_ag.cu): B2_AG_CHUNKS u32 per source rank, right
+// after the barrier flags in the control segment, at this fixed distance from flags_off (so that neither
+// B2Layout nor B2DevComm, which every kernel takes by value, changes layout)
+#define B2_AG_CHUNKS 128
+#define B2_AG_FLAGS_REL ((size_t)B2_MAX_BLOCKS * B2_MAX_RANKS * 4)
 
 // ---- dtype / op codes (must match mpi4jax_b200/_src/native/codes.py) -------
 enum B2DType : int {
@@ -111,6 +116,7 @@ static inline size_t round_up(size_t x, size_t m) { return (x + m - 1) / m * m; 
 // Symmetric-heap layout (identical offsets on every rank).
 //
 //   [flags]      B2_MAX_BLOCKS x B2_MAX_RANKS u32   block-paired barrier flags
+//                B2_MAX_RANKS x B2_AG_CHUNKS u32    allgather + GEMM arrival words (at B2_AG_FLAGS_REL)
 //   [p2p hdr]    P x NSLOT x LANES x 16 B           inbox headers (written by the sender)
 //   [p2p ack]    P x NSLOT x 4 B                    slot credits  (written by the receiver)
 //   [ll]         2 parities x P x ll_cap            flag-in-data allreduce buffers

@@ -1,7 +1,7 @@
-// mpi4jax_b200 -- the persistent wgmma GEMM that the row-parallel linear kernels share: TMA producer,
+// mpi4jax_b200 -- the persistent wgmma GEMM that the linear-layer kernels share: TMA producer,
 // 6-stage mbarrier ring, wgmma mainloop, tile order and the per-group epilogues.  Each kernel lives in its
-// own translation unit (b2_gemm.cu: GEMM + allreduce, b2_gemm_rs.cu: GEMM + reduce-scatter); in one unit
-// together ptxas schedules the allreduce kernel differently.
+// own translation unit (b2_gemm.cu: GEMM + allreduce, b2_gemm_rs.cu: GEMM + reduce-scatter, b2_gemm_ag.cu:
+// allgather + GEMM); in one unit together ptxas schedules the allreduce kernel differently.
 #pragma once
 
 #include <cstring>
@@ -25,6 +25,16 @@ struct GemmArgs {
   __nv_bfloat16* out;
   int fused;           // > 1 rank: per-tile NVLS allreduce through the staging segment
   int raster;          // tile order: 0 = row-major, G > 0 = bands of G tile rows (b2_gemm_raster.h)
+};
+
+// allgather + GEMM: A is the (M = P m, K) gathered matrix in the staging, built while the GEMM runs.  Its
+// kernel passes these, and gemm_body reaches them by a downcast of `g`: a larger GemmArgs, or a gemm_body
+// with more parameters, changes the register allocation of the other two kernels.
+struct GemmArgsAg : GemmArgs {
+  CUtensorMap tma_a1;             // A in staging half 1 (the kernel's tma_a: half 0)
+  const __nv_bfloat16* x_local;   // this rank's (m, K) shard
+  int m;                          // rows per rank
+  int chunk_rows;                 // rows per pushed chunk; ceil(m / chunk_rows) <= B2_AG_CHUNKS
 };
 
 __device__ __forceinline__ void mbar_init(uint32_t bar, uint32_t cnt) {
@@ -107,9 +117,64 @@ __device__ __forceinline__ void epi_barrier_all(const B2DevComm& c, unsigned e, 
   asm volatile("bar.sync 1, 256;" ::: "memory");
 }
 
-// The persistent GEMM both kernels share: producer, wgmma mainloop, 6-stage ring and tile order.  EPI
-// picks what the consumers do with a group of finished tiles when the call is fused (> 1 rank).
-enum GemmEpilogue { EPI_ALLREDUCE, EPI_REDUCE_SCATTER };
+// ---------------------------------------------------------------------------
+// allgather + GEMM (EPI_ALLGATHER): every rank pushes its (m, K) shard, chunk by chunk, into rows
+// [rank m, (rank + 1) m) of the gathered matrix in every rank's staging half, and publishes each chunk in an
+// arrival word of the destination (B2_AG_FLAGS_REL); the producer waits for the chunks under a tile's rows.
+// ---------------------------------------------------------------------------
+__device__ __forceinline__ unsigned* ag_arrivals(const B2DevComm& c, int r) {
+  return (unsigned*)(c.heap[r] + c.lay.flags_off + B2_AG_FLAGS_REL);
+}
+
+// Warps 1-3 of warpgroup 0 (96 threads): chunk j goes from CTA j % gridDim.x, to this rank first, then to
+// rank - 1, rank - 2, ..., so rank r receives shard r + 1 first.  After each (chunk, destination) the pushing
+// warps synchronise and one thread publishes the chunk with `val`.  Never waits on anything.
+__device__ __forceinline__ void ag_push(const B2DevComm& c, const GemmArgsAg& a, size_t par, unsigned val) {
+  const int t = threadIdx.x - 32;
+  const size_t row_bytes = (size_t)a.K * sizeof(__nv_bfloat16);
+  const int nch = (a.m + a.chunk_rows - 1) / a.chunk_rows;
+  for (int j = blockIdx.x; j < nch; j += gridDim.x) {
+    const int r0 = j * a.chunk_rows, r1 = r0 + a.chunk_rows < a.m ? r0 + a.chunk_rows : a.m;
+    const size_t nvec = (size_t)(r1 - r0) * row_bytes / 16;
+    const char* src = (const char*)a.x_local + (size_t)r0 * row_bytes;
+    const size_t off = par + ((size_t)c.rank * a.m + r0) * row_bytes;
+    for (int s = 0; s < c.size; ++s) {
+      const int d = (c.rank - s + c.size) % c.size;
+      char* dst = c.stage[d] + off;
+      for (size_t i = t; i < nvec; i += 96 * 4) {
+        uint4 v[4];
+#pragma unroll
+        for (int u = 0; u < 4; ++u)
+          if (i + u * 96 < nvec) v[u] = b2_ld_stream16(src + ((i + u * 96) << 4));
+#pragma unroll
+        for (int u = 0; u < 4; ++u)
+          if (i + u * 96 < nvec) b2_st16(dst + ((i + u * 96) << 4), v[u]);
+      }
+      asm volatile("bar.sync 2, 96;" ::: "memory");
+      if (t == 0) b2_st_release_sys(ag_arrivals(c, d) + (size_t)c.rank * B2_AG_CHUNKS + j, val);
+    }
+  }
+}
+
+// The producer thread: wait until every chunk under gathered rows [lo, lo + BM) has arrived for this launch
+// (arrival word >= val), then order those generic-proxy writes before the TMA's async-proxy reads.
+__device__ __forceinline__ void ag_wait_rows(const B2DevComm& c, const GemmArgsAg& a, int lo, unsigned val) {
+  const unsigned* arr = ag_arrivals(c, c.rank);
+  for (int q = lo / a.m; q < c.size && q * a.m < lo + BM; ++q) {
+    const int r0 = lo > q * a.m ? lo - q * a.m : 0;                 // rows [r0, r1) of shard q
+    const int r1 = lo + BM < (q + 1) * a.m ? lo + BM - q * a.m : a.m;
+    for (int j = r0 / a.chunk_rows; j <= (r1 - 1) / a.chunk_rows; ++j)
+      b2_wait_ge(c, arr + (size_t)q * B2_AG_CHUNKS + j, val, B2_OPC_ALLGATHER, q);
+  }
+  asm volatile("fence.proxy.async.global;" ::: "memory");
+}
+
+// The persistent GEMM all three kernels share: producer, wgmma mainloop, 6-stage ring and tile order.  EPI
+// picks what the consumers do with a group of finished tiles when the call is fused (> 1 rank);
+// EPI_ALLGATHER instead gathers A while the GEMM runs (`g` is a GemmArgsAg: tma_a / g.tma_a1 map the gathered
+// matrix in staging half 0 / 1), walks the tile rows from this rank's own shard on, and stores the tiles like
+// the stand-alone GEMM.
+enum GemmEpilogue { EPI_ALLREDUCE, EPI_REDUCE_SCATTER, EPI_ALLGATHER };
 
 template <int EPI>
 __device__ __forceinline__ void gemm_body(const CUtensorMap& tma_a, const CUtensorMap& tma_b, const B2DevComm& c,
@@ -123,7 +188,7 @@ __device__ __forceinline__ void gemm_body(const CUtensorMap& tma_a, const CUtens
   auto bar = [](uint64_t* p) { return (uint32_t)__cvta_generic_to_shared(p); };
 
   unsigned ticket = 0, e = 0;
-  if (g.fused) {
+  if (EPI == EPI_ALLGATHER || g.fused) {
     ticket = b2_ticket_read(c.ticket);
     e = b2_ld_volatile(c.epoch + blockIdx.x);
   }
@@ -138,22 +203,39 @@ __device__ __forceinline__ void gemm_body(const CUtensorMap& tma_a, const CUtens
 
   const int num_n = g.N / BN, tiles = (g.M / BM) * num_n, num_kb = g.K / BK;
 
+  // allgather + GEMM: tile row m_blk of the tile order is gathered tile row (m_blk + rot) mod (M / BM), so
+  // the first tiles lie in this rank's own shard
+  int rot = 0;
+  if constexpr (EPI == EPI_ALLGATHER)
+    rot = (int)(((long long)c.rank * static_cast<const GemmArgsAg&>(g).m) / BM);
+
   if (wg == 0) {
     if (threadIdx.x == 0) {
       // ===== TMA producer =====
+      const CUtensorMap* ta = &tma_a;
+      if constexpr (EPI == EPI_ALLGATHER)
+        if (ticket & 1u) ta = &static_cast<const GemmArgsAg&>(g).tma_a1;
       uint32_t stage = 0, phase = 0;
+      int waited = -1;                                          // allgather: the tile row already waited for
       for (int tile = blockIdx.x; tile < tiles; tile += gridDim.x) {
         int m_blk, n_blk;
         b2_gemm_tile_coords(tile, g.M / BM, num_n, g.raster, m_blk, n_blk);
+        if constexpr (EPI == EPI_ALLGATHER) {
+          m_blk = (m_blk + rot) % (g.M / BM);
+          if (m_blk != waited) ag_wait_rows(c, static_cast<const GemmArgsAg&>(g), m_blk * BM, ticket + 1u);
+          waited = m_blk;
+        }
         for (int kb = 0; kb < num_kb; ++kb) {
           mbar_wait(bar(&empty_bar[stage]), phase ^ 1u);
           mbar_expect_tx(bar(&full_bar[stage]), A_STAGE_BYTES + B_STAGE_BYTES);
-          tma_load_2d(smem_a + stage * A_STAGE_BYTES, &tma_a, bar(&full_bar[stage]), kb * BK, m_blk * BM);
+          tma_load_2d(smem_a + stage * A_STAGE_BYTES, ta, bar(&full_bar[stage]), kb * BK, m_blk * BM);
           tma_load_2d(smem_b + stage * B_STAGE_BYTES, &tma_b, bar(&full_bar[stage]), kb * BK, n_blk * BN);
           if (++stage == STAGES) { stage = 0; phase ^= 1u; }
         }
       }
     }
+    if constexpr (EPI == EPI_ALLGATHER)
+      if (warp > 0) ag_push(c, static_cast<const GemmArgsAg&>(g), par, ticket + 1u);
   } else {
     // ===== consumers: wgmma -> bf16 -> (staging + per-group collective | output) =====
     const int cw = wg - 1;                                      // rows cw * 64 .. +64 of the tile
@@ -169,6 +251,7 @@ __device__ __forceinline__ void gemm_body(const CUtensorMap& tma_a, const CUtens
     for (int tile = blockIdx.x; tile < tiles; tile += gridDim.x) {
       int m_blk, n_blk;
       b2_gemm_tile_coords(tile, g.M / BM, num_n, g.raster, m_blk, n_blk);
+      if constexpr (EPI == EPI_ALLGATHER) m_blk = (m_blk + rot) % (g.M / BM);
       uint32_t prev = 0;
       for (int kb = 0; kb < num_kb; ++kb) {
         mbar_wait(bar(&full_bar[stage]), phase);                // TMA landed this stage
@@ -318,19 +401,34 @@ __device__ __forceinline__ void gemm_body(const CUtensorMap& tma_a, const CUtens
   }
 
   __syncthreads();
-  if (g.fused) b2_finish_bump(c.ticket, c.ticket + 1, 1u, gridDim.x);
+  if (EPI == EPI_ALLGATHER || g.fused) b2_finish_bump(c.ticket, c.ticket + 1, 1u, gridDim.x);
 }
 
-// Tensor maps, shared-memory reservation and the persistent grid of either kernel; `g` is filled in
-// except for the tile order.
-// `attr_set`: the kernel's own flag that its shared-memory size has been reserved.
+// The tile order, shared-memory reservation and persistent grid of a GEMM kernel; `g` is filled in except
+// for the tile order.  `attr_set`: the kernel's own flag that its shared-memory size has been reserved.
 template <typename Kernel>
-int gemm_launch(Kernel kernel, bool& attr_set, B2Comm* c, const void* A, const void* B, GemmArgs g, const char* what,
-                cudaStream_t stream) {
-  // banded tile order for the stand-alone GEMM; the fused epilogues recompute a tile's coordinates per
+int gemm_geometry(Kernel kernel, bool& attr_set, B2Comm* c, GemmArgs& g, const char* what, size_t& smem, int& grid) {
+  // banded tile order for the stand-alone store; the fused epilogues recompute a tile's coordinates per
   // 16-byte vector (integer divisions in front of every staging load), so they keep the cheaper
   // row-major formula
   g.raster = c->gemm_raster >= 0 ? c->gemm_raster : (g.fused ? 0 : B2_GEMM_RASTER_GROUP);
+  smem = (size_t)STAGES * (A_STAGE_BYTES + B_STAGE_BYTES) + 1024;
+  if (!attr_set) {
+    if (int rc = b2_cuda_check(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem),
+                               "%s: cannot reserve %zu bytes of shared memory", what, smem))
+      return rc;
+    attr_set = true;
+  }
+  const int tiles = (g.M / BM) * (g.N / BN);
+  grid = tiles < c->sm_count ? tiles : c->sm_count;
+  if (grid > B2_MAX_BLOCKS) grid = B2_MAX_BLOCKS;
+  return 0;
+}
+
+// Tensor maps, staging check and launch of the allreduce and reduce-scatter kernels.
+template <typename Kernel>
+int gemm_launch(Kernel kernel, bool& attr_set, B2Comm* c, const void* A, const void* B, GemmArgs g, const char* what,
+                cudaStream_t stream) {
   if (g.fused && (size_t)g.M * g.N * 2 + 4096 > c->dev.stage_half) {
     b2_set_error("%s: staging too small (need %zu bytes, have %zu)", what, (size_t)g.M * g.N * 2 + 4096,
                  c->dev.stage_half);
@@ -340,16 +438,9 @@ int gemm_launch(Kernel kernel, bool& attr_set, B2Comm* c, const void* A, const v
   if (b2_tensor_map_2d_bf16(&ta, A, (unsigned long long)g.M, (unsigned long long)g.K, BM, BK) ||
       b2_tensor_map_2d_bf16(&tb, B, (unsigned long long)g.N, (unsigned long long)g.K, BN, BK))
     return B2_ERR_BAD_ARG;
-  const size_t smem = (size_t)STAGES * (A_STAGE_BYTES + B_STAGE_BYTES) + 1024;
-  if (!attr_set) {
-    if (int rc = b2_cuda_check(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem),
-                               "%s: cannot reserve %zu bytes of shared memory", what, smem))
-      return rc;
-    attr_set = true;
-  }
-  const int tiles = (g.M / BM) * (g.N / BN);
-  int grid = tiles < c->sm_count ? tiles : c->sm_count;
-  if (grid > B2_MAX_BLOCKS) grid = B2_MAX_BLOCKS;
+  size_t smem;
+  int grid;
+  if (int rc = gemm_geometry(kernel, attr_set, c, g, what, smem, grid)) return rc;
   kernel<<<grid, GEMM_THREADS, smem, stream>>>(ta, tb, c->dev, g);
   return b2_launched(c, what);
 }

@@ -351,7 +351,7 @@ static B2Layout make_layout(int nranks, size_t slot_bytes, size_t ll_cap, size_t
   B2Layout L;
   size_t off = 0;
   auto take = [&](size_t bytes) { size_t o = off; off = round_up(off + bytes, 4096); return o; };
-  L.flags_off = take((size_t)B2_MAX_BLOCKS * B2_MAX_RANKS * 4);
+  L.flags_off = take(B2_AG_FLAGS_REL + (size_t)B2_MAX_RANKS * B2_AG_CHUNKS * 4);
   L.p2p_hdr_off = take((size_t)nranks * B2_P2P_NSLOT * B2_P2P_MAX_LANES * 16);
   L.p2p_ack_off = take((size_t)nranks * B2_P2P_NSLOT * 4);
   L.ll_cap = round_up(ll_cap, 4096);

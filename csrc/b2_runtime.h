@@ -216,6 +216,11 @@ int b2_gemm_allreduce(B2Comm* c, const void* A, const void* B, void* out, int M,
 // (M / size) x N shard of the sum; pull-and-fold epilogue, no multicast
 int b2_gemm_reduce_scatter(B2Comm* c, const void* A, const void* B, void* out, int M, int N, int K,
                            cudaStream_t stream);
+// ... and the column-parallel layer before it (b2_gemm_ag.cu): out (size m x N) = the (m x K) x_local of
+// every rank, gathered in rank order, @ w^T (w: N x K); m and K the same on every rank, N may differ.  The
+// shards are pushed into the staging while the GEMM runs; no multicast
+int b2_gemm_allgather(B2Comm* c, const void* x_local, const void* w, void* out, int m, int N, int K,
+                      cudaStream_t stream);
 
 // --- fused halo exchange + shallow-water stencils (see b2_halo.cu, b2_swe.cu) --
 struct B2HaloDesc {

@@ -714,7 +714,7 @@ class NativeComm:
         self._bind_status(status, rec, out.element_size())
         return out
 
-    # -- row-parallel linear: wgmma GEMM + allreduce / reduce-scatter (csrc/b2_gemm*.cu) ------------
+    # -- linear layers: wgmma GEMM + allreduce / reduce-scatter, allgather + GEMM (csrc/b2_gemm*.cu) ---
     def gemm_allreduce(self, x: torch.Tensor, weight: torch.Tensor) -> torch.Tensor:
         """``allreduce_SUM(x @ weight.T)`` for bf16 ``x (M, K)``, ``weight (N, K)`` in ONE kernel."""
         M, K = x.shape
@@ -743,6 +743,20 @@ class NativeComm:
         rc = _lib().b2_gemm_reduce_scatter(self.handle, x.data_ptr(), weight.data_ptr(), out.data_ptr(), M, N, K,
                                            self._stream())
         self._check(rc, "Reduce_scatter_block")
+        return out
+
+    def gemm_allgather(self, x: torch.Tensor, weight: torch.Tensor) -> torch.Tensor:
+        """``allgather(x).reshape(size * m, K) @ weight.T`` for bf16 ``x (m, K)`` (the same m and K on every rank)
+        and this rank's ``weight (N, K)`` in ONE kernel (csrc/b2_gemm_ag.cu); no multicast needed."""
+        m, K = x.shape
+        N = weight.shape[0]
+        P = self.comm.size
+        out = torch.empty((P * m, N), dtype=torch.bfloat16, device=x.device)
+        if P > 1:
+            self.ensure_stage(codes.OPC_ALLGATHER, P * m * K * 2)       # the gathered matrix, per parity
+        rc = _lib().b2_gemm_allgather(self.handle, x.data_ptr(), weight.data_ptr(), out.data_ptr(), m, N, K,
+                                      self._stream())
+        self._check(rc, "Allgather")
         return out
 
     # -- fused halo exchange ---------------------------------------------------------
@@ -786,7 +800,7 @@ def _nvtx_wrap(name: str, fn):
 NVTX_OPS = ("barrier", "allreduce", "reduce", "scan", "allgather", "alltoall", "bcast", "gather", "scatter",
             "send", "recv", "sendrecv", "reduce_scatter", "alltoallv", "allgatherv", "reduce_scatterv", "gatherv",
             "scatterv", "reduce_loc",
-            "gemm_allreduce", "gemm_reduce_scatter",
+            "gemm_allreduce", "gemm_reduce_scatter", "gemm_allgather",
             "halo_exchange")
 if env_flag("MPI4JAX_B200_NVTX", False):
     for _name in NVTX_OPS:

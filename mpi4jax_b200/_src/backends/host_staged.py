@@ -146,5 +146,8 @@ class HostStagedComm:
     def gemm_reduce_scatter(self, *a, **k):
         self._unsupported("the fused GEMM + reduce-scatter kernel")
 
+    def gemm_allgather(self, *a, **k):
+        self._unsupported("the fused allgather + GEMM kernel")
+
     def halo_exchange(self, *a, **k):
         self._unsupported("the fused halo-exchange kernel")

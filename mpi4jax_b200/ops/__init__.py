@@ -6,4 +6,4 @@ from .._src import (  # noqa: F401
     reduce_scatter, reduce_scatterv, scan, scatter, scatterv, send, send_with_grad, sendrecv,
 )
 from .halo import halo_exchange  # noqa: F401
-from .linear import linear_allreduce, linear_reduce_scatter  # noqa: F401
+from .linear import linear_allgather, linear_allreduce, linear_reduce_scatter  # noqa: F401

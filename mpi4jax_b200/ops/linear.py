@@ -21,6 +21,14 @@ Its kernel (csrc/b2_gemm_rs.cu) shares the GEMM and reduces each group of tiles 
 staged partial, with no multicast, so it also runs where NVLS is off or the ranks share a GPU.  The
 adjoint of a reduce-scatter is an allgather: with ``G = allgather(g)``, ``grad_x = G @ weight`` and
 ``grad_weight = G.T @ x``.
+
+``linear_allgather(x, weight)`` is the column-parallel layer in front of it: ``allgather(x) @ weight.T``
+with rank q's rows first gathered at ``[q m, (q+1) m)``, and this rank's own column shard of the weight.
+Its kernel (csrc/b2_gemm_ag.cu) runs the same GEMM on the gathered matrix while the ranks push their
+shards into every rank's staging, so the allgather's NVLink traffic overlaps the tiles already computable.
+The fuse decision depends only on what the ranks share (m, K, the dtype and the transport), never on this
+rank's N, so a rank with no columns at all still pushes its rows.  The adjoint pairs the two layers:
+``grad_x = linear_reduce_scatter(g, weight.T)`` and ``grad_weight = g.T @ allgather(x)``.
 """
 
 from __future__ import annotations
@@ -141,3 +149,59 @@ def linear_reduce_scatter(x: torch.Tensor, weight: torch.Tensor, *, comm: Option
     if not needs_autograd(x, weight):
         return _forward_rs(x, weight, comm)
     return _LinearReduceScatter.apply(x, weight, comm)
+
+
+def _fuse_ag(x: torch.Tensor, w: torch.Tensor, comm: Comm) -> bool:
+    """bf16 CUDA operands, ``P m`` a multiple of the tile height, the native transport: whether to run the
+    allgather kernel.  The same answer on every rank of ``comm``: it never looks at this rank's N."""
+    P, m = comm.Get_size(), x.shape[0]
+    return (x.is_cuda and w.is_cuda and x.dtype == torch.bfloat16 and w.dtype == torch.bfloat16 and m > 0
+            and (P * m) % _BM == 0 and comm.transport == "native")
+
+
+def _forward_ag(x: torch.Tensor, w: torch.Tensor, comm: Comm) -> torch.Tensor:
+    P, (m, K), N = comm.Get_size(), x.shape, w.shape[0]
+    if _fuse_ag(x, w, comm):
+        nc = comm._native_comm()
+        # this rank's N up to a multiple of the tile width (at least one tile, so that a rank without
+        # columns still runs the kernel and pushes its rows) with zero rows of the weight
+        Np = max(_BN, -(-N // _BN) * _BN)
+        xk, wk = _kernel_operands(x, F.pad(w, (0, 0, 0, Np - N)) if Np != N else w)
+        y = nc.gemm_allreduce(xk, wk) if P == 1 else nc.gemm_allgather(xk, wk)
+        return y if Np == N else y[:, :N].contiguous()
+    X = _dispatch.allgather(comm, x.contiguous()).reshape(P * m, K)
+    return X @ w.t()
+
+
+class _LinearAllgather(torch.autograd.Function):
+    @staticmethod
+    def forward(x, w, comm):
+        return _forward_ag(x, w, comm)
+
+    @staticmethod
+    def setup_context(ctx, inputs, output):
+        x, w, ctx.comm = inputs
+        ctx.save_for_backward(x, w)
+
+    @staticmethod
+    def backward(ctx, g):
+        x, w = ctx.saved_tensors
+        P = ctx.comm.Get_size()
+        # rows r of sum_q g_q @ w_q (the N_q may differ), then the gathered x again, on every rank in this order
+        grad_x = _forward_rs(g, w.t(), ctx.comm)
+        X = _dispatch.allgather(ctx.comm, x.contiguous()).reshape(P * x.shape[0], x.shape[1])
+        return grad_x, g.t() @ X, None
+
+
+def linear_allgather(x: torch.Tensor, weight: torch.Tensor, *, comm: Optional[Comm] = None) -> torch.Tensor:
+    """``allgather(x).reshape(P m, K) @ weight.T`` over the P ranks of ``comm``: shape ``(P m, N)``, rank q's
+    rows at ``[q m, (q+1) m)``.  ``x (m, K)`` has the same shape on every rank; ``weight (N, K)`` is this
+    rank's column shard, and N may differ between ranks."""
+    comm = comm or get_default_comm()
+    if x.dim() != 2 or weight.dim() != 2:
+        raise ValueError(f"linear_allgather: x and weight must be 2-D (got {x.dim()}-D and {weight.dim()}-D)")
+    if x.shape[1] != weight.shape[1]:
+        raise ValueError(f"linear_allgather: x has {x.shape[1]} columns, weight {weight.shape[1]}")
+    if not needs_autograd(x, weight):
+        return _forward_ag(x, weight, comm)
+    return _LinearAllgather.apply(x, weight, comm)

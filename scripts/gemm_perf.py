@@ -1,5 +1,5 @@
 """Fused wgmma GEMM+allreduce vs cuBLAS GEMM followed by an allreduce (ours / NCCL), and for M divisible by
-the world size the same for GEMM+reduce-scatter over the rows."""
+the world size the same for GEMM+reduce-scatter over the rows and for allgather (of M / P rows per rank)+GEMM."""
 import os
 import sys
 
@@ -9,7 +9,7 @@ import torch.distributed as dist  # noqa: E402
 
 import mpi4jax_b200 as m  # noqa: E402
 from mpi4jax_b200 import MPI  # noqa: E402
-from mpi4jax_b200.ops import linear_allreduce, linear_reduce_scatter  # noqa: E402
+from mpi4jax_b200.ops import linear_allgather, linear_allreduce, linear_reduce_scatter  # noqa: E402
 from mpi4jax_b200.utils import max_over_ranks  # noqa: E402
 
 comm = MPI.COMM_WORLD
@@ -56,6 +56,15 @@ for (M, N, K) in [(4096, 4096, 4096 // size), (8192, 8192, 8192 // size), (8192,
                 dist.reduce_scatter_tensor(out, y, group=nccl)
                 return out
             rows["cublas + nccl reduce_scatter_tensor"] = timeit(g)
+        xs = x[:M // size].contiguous()           # this rank's rows of the gathered (M, K) operand
+        rows["fused allgather+wgmma (one kernel)"] = timeit(lambda: linear_allgather(xs, w, comm=comm))
+        rows["our allgather + cublas"] = timeit(lambda: m.allgather(xs, comm=comm).reshape(M, K) @ w.t())
+        if nccl is not None:
+            def h():
+                X = torch.empty(M, K, device=dev, dtype=xs.dtype)
+                dist.all_gather_into_tensor(X, xs, group=nccl)
+                return X @ w.t()
+            rows["nccl all_gather_into_tensor + cublas"] = timeit(h)
     rows["cublas gemm only"] = timeit(lambda: x @ w.t())
     if rank == 0:
         print(f"M={M} N={N} K/rank={K} (bf16 out {M * N * 2 / 2**20:.0f} MiB): " +
