@@ -1,13 +1,16 @@
 // mpi4jax_b200 -- the persistent wgmma GEMM that the linear-layer kernels share: TMA producer,
 // 6-stage mbarrier ring, wgmma mainloop, tile order and the per-group epilogues.  Each kernel lives in its
 // own translation unit (b2_gemm.cu: GEMM + allreduce, b2_gemm_rs.cu: GEMM + reduce-scatter, b2_gemm_ag.cu:
-// allgather + GEMM); in one unit together ptxas schedules the allreduce kernel differently.
+// allgather + GEMM; b2_gemm_f8.cu: the three float8 twins); in one unit together ptxas schedules the allreduce
+// kernel differently.
 #pragma once
 
 #include <cstring>
+#include <type_traits>
 
 #include <cuda.h>
 #include <cuda_bf16.h>
+#include <cuda_fp8.h>
 
 #include "b2_device.cuh"
 #include "b2_runtime.h"
@@ -32,10 +35,36 @@ struct GemmArgs {
 // with more parameters, changes the register allocation of the other two kernels.
 struct GemmArgsAg : GemmArgs {
   CUtensorMap tma_a1;             // A in staging half 1 (the kernel's tma_a: half 0)
-  const __nv_bfloat16* x_local;   // this rank's (m, K) shard
+  const __nv_bfloat16* x_local;   // this rank's (m, K) shard (float8 kernel: one byte per element)
   int m;                          // rows per rank
   int chunk_rows;                 // rows per pushed chunk; ceil(m / chunk_rows) <= B2_AG_CHUNKS
 };
+
+// Scaled float8 operands: partial (i, j) = rn_bf16(S[i, j] * (sx[i * sx_inc] * sw[j * sw_inc])).  The scales
+// are read through these pointers at every launch (a graph replay sees scales updated in place); an increment
+// of 0 is one scale for the whole tensor, 1 one per row of A / column of the output.
+struct GemmScales {
+  const float* sx;
+  const float* sw;
+  int sx_inc, sw_inc;
+};
+// The float8 kernels' arguments, reached like GemmArgsAg by a downcast of `g`.  Allgather + GEMM: the push
+// warps copy this rank's row scales (sx, sx_inc) as m floats per shard into a region `sx_off` bytes into the
+// staging half, after the gathered (P m, K) matrix; the epilogue reads them there with an increment of 1.
+struct GemmArgsF8 : GemmArgs {
+  GemmScales s;
+};
+struct GemmArgsAgF8 : GemmArgsAg {
+  GemmScales s;
+  size_t sx_off;
+};
+
+// Operand element types of the mainloop.  A k-block is one 128-byte row of the swizzle atom in either
+// type: BK = 64 bf16 or 128 e4m3 elements, so the stage sizes, the GMMA descriptors and the +32 B per wgmma
+// k-step are the same, and one wgmma takes 16 or 32 elements of K.
+template <typename T> struct GemmElem;
+template <> struct GemmElem<__nv_bfloat16> { static constexpr int BK = 64, WGMMA_K = 16; };
+template <> struct GemmElem<__nv_fp8_e4m3> { static constexpr int BK = 128, WGMMA_K = 32; };
 
 __device__ __forceinline__ void mbar_init(uint32_t bar, uint32_t cnt) {
   asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(bar), "r"(cnt));
@@ -74,6 +103,22 @@ __device__ __forceinline__ void wgmma_bf16(float (&d)[64], uint64_t adesc, uint6
       "{\n.reg .pred p;\nsetp.ne.b32 p, %66, 0;\n"
       "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 "
       "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1, 0, 0;\n}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+        "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
+        "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
+        "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
+        "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
+        "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "l"(adesc), "l"(bdesc), "r"(accum));
+}
+// the same for e4m3 operands, 32 elements of K per instruction (float8 wgmma has no transpose immediates)
+__device__ __forceinline__ void wgmma_e4m3(float (&d)[64], uint64_t adesc, uint64_t bdesc, uint32_t accum) {
+  asm volatile(
+      "{\n.reg .pred p;\nsetp.ne.b32 p, %66, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n128k32.f32.e4m3.e4m3 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1;\n}"
       : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
         "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
         "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
@@ -128,10 +173,13 @@ __device__ __forceinline__ unsigned* ag_arrivals(const B2DevComm& c, int r) {
 
 // Warps 1-3 of warpgroup 0 (96 threads): chunk j goes from CTA j % gridDim.x, to this rank first, then to
 // rank - 1, rank - 2, ..., so rank r receives shard r + 1 first.  After each (chunk, destination) the pushing
-// warps synchronise and one thread publishes the chunk with `val`.  Never waits on anything.
+// warps synchronise and one thread publishes the chunk with `val`.  Never waits on anything.  Float8: the
+// chunk's row scales go with its rows, to gathered rows [rank m + r0, rank m + r1) of the scale region, before
+// the same barrier and arrival word.
+template <typename T>
 __device__ __forceinline__ void ag_push(const B2DevComm& c, const GemmArgsAg& a, size_t par, unsigned val) {
   const int t = threadIdx.x - 32;
-  const size_t row_bytes = (size_t)a.K * sizeof(__nv_bfloat16);
+  const size_t row_bytes = (size_t)a.K * sizeof(T);
   const int nch = (a.m + a.chunk_rows - 1) / a.chunk_rows;
   for (int j = blockIdx.x; j < nch; j += gridDim.x) {
     const int r0 = j * a.chunk_rows, r1 = r0 + a.chunk_rows < a.m ? r0 + a.chunk_rows : a.m;
@@ -149,6 +197,11 @@ __device__ __forceinline__ void ag_push(const B2DevComm& c, const GemmArgsAg& a,
 #pragma unroll
         for (int u = 0; u < 4; ++u)
           if (i + u * 96 < nvec) b2_st16(dst + ((i + u * 96) << 4), v[u]);
+      }
+      if constexpr (!std::is_same_v<T, __nv_bfloat16>) {
+        const GemmArgsAgF8& f = static_cast<const GemmArgsAgF8&>(a);
+        float* sdst = (float*)(c.stage[d] + par + f.sx_off) + (size_t)c.rank * a.m;
+        for (int i = r0 + t; i < r1; i += 96) sdst[i] = f.s.sx[(size_t)i * f.s.sx_inc];
       }
       asm volatile("bar.sync 2, 96;" ::: "memory");
       if (t == 0) b2_st_release_sys(ag_arrivals(c, d) + (size_t)c.rank * B2_AG_CHUNKS + j, val);
@@ -176,7 +229,7 @@ __device__ __forceinline__ void ag_wait_rows(const B2DevComm& c, const GemmArgsA
 // the stand-alone GEMM.
 enum GemmEpilogue { EPI_ALLREDUCE, EPI_REDUCE_SCATTER, EPI_ALLGATHER };
 
-template <int EPI>
+template <int EPI, typename T = __nv_bfloat16>
 __device__ __forceinline__ void gemm_body(const CUtensorMap& tma_a, const CUtensorMap& tma_b, const B2DevComm& c,
                                           const GemmArgs& g) {
   extern __shared__ uint8_t smem_raw[];
@@ -201,7 +254,9 @@ __device__ __forceinline__ void gemm_body(const CUtensorMap& tma_a, const CUtens
   }
   __syncthreads();
 
-  const int num_n = g.N / BN, tiles = (g.M / BM) * num_n, num_kb = g.K / BK;
+  constexpr bool F8 = !std::is_same_v<T, __nv_bfloat16>;
+  constexpr int KB = GemmElem<T>::BK;                           // elements of K per k-block (128 bytes)
+  const int num_n = g.N / BN, tiles = (g.M / BM) * num_n, num_kb = g.K / KB;
 
   // allgather + GEMM: tile row m_blk of the tile order is gathered tile row (m_blk + rot) mod (M / BM), so
   // the first tiles lie in this rank's own shard
@@ -228,14 +283,14 @@ __device__ __forceinline__ void gemm_body(const CUtensorMap& tma_a, const CUtens
         for (int kb = 0; kb < num_kb; ++kb) {
           mbar_wait(bar(&empty_bar[stage]), phase ^ 1u);
           mbar_expect_tx(bar(&full_bar[stage]), A_STAGE_BYTES + B_STAGE_BYTES);
-          tma_load_2d(smem_a + stage * A_STAGE_BYTES, ta, bar(&full_bar[stage]), kb * BK, m_blk * BM);
-          tma_load_2d(smem_b + stage * B_STAGE_BYTES, &tma_b, bar(&full_bar[stage]), kb * BK, n_blk * BN);
+          tma_load_2d(smem_a + stage * A_STAGE_BYTES, ta, bar(&full_bar[stage]), kb * KB, m_blk * BM);
+          tma_load_2d(smem_b + stage * B_STAGE_BYTES, &tma_b, bar(&full_bar[stage]), kb * KB, n_blk * BN);
           if (++stage == STAGES) { stage = 0; phase ^= 1u; }
         }
       }
     }
     if constexpr (EPI == EPI_ALLGATHER)
-      if (warp > 0) ag_push(c, static_cast<const GemmArgsAg&>(g), par, ticket + 1u);
+      if (warp > 0) ag_push<T>(c, static_cast<const GemmArgsAg&>(g), par, ticket + 1u);
   } else {
     // ===== consumers: wgmma -> bf16 -> (staging + per-group collective | output) =====
     const int cw = wg - 1;                                      // rows cw * 64 .. +64 of the tile
@@ -259,8 +314,10 @@ __device__ __forceinline__ void gemm_body(const CUtensorMap& tma_a, const CUtens
         const uint64_t bdesc = gmma_desc(smem_b + stage * B_STAGE_BYTES);
         wgmma_fence();
 #pragma unroll
-        for (int k = 0; k < BK / WGMMA_K; ++k)                  // +32 B per WGMMA_K inside the swizzle atom
-          wgmma_bf16(acc, adesc + (uint64_t)(k * 2), bdesc + (uint64_t)(k * 2), (kb | k) != 0);
+        for (int k = 0; k < KB / GemmElem<T>::WGMMA_K; ++k) {   // +32 B per wgmma k-step inside the swizzle atom
+          if constexpr (F8) wgmma_e4m3(acc, adesc + (uint64_t)(k * 2), bdesc + (uint64_t)(k * 2), (kb | k) != 0);
+          else wgmma_bf16(acc, adesc + (uint64_t)(k * 2), bdesc + (uint64_t)(k * 2), (kb | k) != 0);
+        }
         wgmma_commit();
         wgmma_wait<1>();                                        // the previous stage's MMAs have retired
         if (kb > 0 && leader) mbar_arrive(bar(&empty_bar[prev]));
@@ -273,6 +330,33 @@ __device__ __forceinline__ void gemm_body(const CUtensorMap& tma_a, const CUtens
       // accumulator fragment: acc[4j + {0,1}] = row r, columns 8j + 2(lane % 4) + {0,1}; acc[4j + {2,3}] = row r + 8
       const size_t row = (size_t)m_blk * BM + cw * 64 + wq * 16 + (lane >> 2);
       __nv_bfloat16* dst = (g.fused ? stage_local : g.out) + row * g.N + (size_t)n_blk * BN + 2 * (lane & 3);
+      if constexpr (F8) {
+        // acc * (sx[row] * sw[col]) in fp32, then the one bf16 rounding below.  Allgather: the gathered row
+        // scales in the staging, written by the ranks' push warps; every full_bar wait of this tile came after
+        // the producer's ld.acquire.sys of their arrival words (ag_wait_rows), so they are visible here.  L2
+        // loads (.cg): another tile may have brought the same 128-byte line into L1 before all of it arrived.
+        float x0, x1;
+        const GemmScales* s;
+        if constexpr (EPI == EPI_ALLGATHER) {
+          s = &static_cast<const GemmArgsAgF8&>(g).s;
+          const float* sxg = (const float*)(c.stage[c.rank] + par + static_cast<const GemmArgsAgF8&>(g).sx_off);
+          x0 = __ldcg(sxg + row);
+          x1 = __ldcg(sxg + row + 8);
+        } else {
+          s = &static_cast<const GemmArgsF8&>(g).s;
+          x0 = __ldg(s->sx + row * s->sx_inc);
+          x1 = __ldg(s->sx + (row + 8) * s->sx_inc);
+        }
+        const float* sw = s->sw + ((size_t)n_blk * BN + 2 * (lane & 3)) * s->sw_inc;
+#pragma unroll
+        for (int j = 0; j < BN / 8; ++j) {
+          const float w0 = __ldg(sw + (size_t)(8 * j) * s->sw_inc), w1 = __ldg(sw + (size_t)(8 * j + 1) * s->sw_inc);
+          acc[4 * j] *= x0 * w0;
+          acc[4 * j + 1] *= x0 * w1;
+          acc[4 * j + 2] *= x1 * w0;
+          acc[4 * j + 3] *= x1 * w1;
+        }
+      }
 #pragma unroll
       for (int j = 0; j < BN / 8; ++j) {
         *reinterpret_cast<__nv_bfloat162*>(dst + 8 * j) = __floats2bfloat162_rn(acc[4 * j], acc[4 * j + 1]);
@@ -425,9 +509,19 @@ int gemm_geometry(Kernel kernel, bool& attr_set, B2Comm* c, GemmArgs& g, const c
   return 0;
 }
 
-// Tensor maps, staging check and launch of the allreduce and reduce-scatter kernels.
-template <typename Kernel>
-int gemm_launch(Kernel kernel, bool& attr_set, B2Comm* c, const void* A, const void* B, GemmArgs g, const char* what,
+// TMA map of a row-major (rows x cols) operand of element type T, box BM (= BN) rows x one k-block
+template <typename T>
+int gemm_tensor_map(CUtensorMap* map, const void* p, int rows, int cols) {
+  if constexpr (std::is_same_v<T, __nv_bfloat16>)
+    return b2_tensor_map_2d_bf16(map, p, (unsigned long long)rows, (unsigned long long)cols, BM, BK);
+  else
+    return b2_tensor_map_2d_u8(map, p, (unsigned long long)rows, (unsigned long long)cols, BM, GemmElem<T>::BK);
+}
+
+// Tensor maps, staging check and launch of the allreduce and reduce-scatter kernels.  `Args`: GemmArgs, or
+// GemmArgsF8 for the float8 kernels (element type T).
+template <typename T = __nv_bfloat16, typename Kernel, typename Args>
+int gemm_launch(Kernel kernel, bool& attr_set, B2Comm* c, const void* A, const void* B, Args g, const char* what,
                 cudaStream_t stream) {
   if (g.fused && (size_t)g.M * g.N * 2 + 4096 > c->dev.stage_half) {
     b2_set_error("%s: staging too small (need %zu bytes, have %zu)", what, (size_t)g.M * g.N * 2 + 4096,
@@ -435,9 +529,7 @@ int gemm_launch(Kernel kernel, bool& attr_set, B2Comm* c, const void* A, const v
     return B2_ERR_BAD_ARG;
   }
   CUtensorMap ta, tb;
-  if (b2_tensor_map_2d_bf16(&ta, A, (unsigned long long)g.M, (unsigned long long)g.K, BM, BK) ||
-      b2_tensor_map_2d_bf16(&tb, B, (unsigned long long)g.N, (unsigned long long)g.K, BN, BK))
-    return B2_ERR_BAD_ARG;
+  if (gemm_tensor_map<T>(&ta, A, g.M, g.K) || gemm_tensor_map<T>(&tb, B, g.N, g.K)) return B2_ERR_BAD_ARG;
   size_t smem;
   int grid;
   if (int rc = gemm_geometry(kernel, attr_set, c, g, what, smem, grid)) return rc;
@@ -445,9 +537,10 @@ int gemm_launch(Kernel kernel, bool& attr_set, B2Comm* c, const void* A, const v
   return b2_launched(c, what);
 }
 
-inline bool gemm_shape_ok(const char* what, int M, int N, int K) {
-  if (M <= 0 || N <= 0 || K <= 0 || M % BM || N % BN || K % BK) {
-    b2_set_error("%s: need M %% %d == 0, N %% %d == 0, K %% %d == 0 (got %d, %d, %d)", what, BM, BN, BK, M, N, K);
+// `kb`: the k-block in elements, BK for bf16 and GemmElem<__nv_fp8_e4m3>::BK for float8
+inline bool gemm_shape_ok(const char* what, int M, int N, int K, int kb = BK) {
+  if (M <= 0 || N <= 0 || K <= 0 || M % BM || N % BN || K % kb) {
+    b2_set_error("%s: need M %% %d == 0, N %% %d == 0, K %% %d == 0 (got %d, %d, %d)", what, BM, BN, kb, M, N, K);
     return false;
   }
   return true;

@@ -527,22 +527,22 @@ extern "C" int b2_comm_destroy(B2Comm* c) {
 }
 
 // ---------------------------------------------------------------------------
-// TMA descriptor for a row-major (rows x cols) bf16 matrix, box = box_rows x box_cols,
+// TMA descriptor for a row-major (rows x cols) matrix of `esize`-byte elements, box = box_rows x box_cols,
 // 128-byte swizzle (what the wgmma K-major SWIZZLE_128B shared-memory descriptor expects)
 // ---------------------------------------------------------------------------
-extern "C" int b2_tensor_map_2d_bf16(CUtensorMap* out, const void* ptr, unsigned long long rows,
-                                     unsigned long long cols, unsigned box_rows, unsigned box_cols) {
+static int tensor_map_2d(CUtensorMap* out, CUtensorMapDataType type, unsigned esize, const void* ptr,
+                         unsigned long long rows, unsigned long long cols, unsigned box_rows, unsigned box_cols) {
   if (!load_driver()) return 1;
-  if (((uintptr_t)ptr & 15) != 0 || (cols * 2) % 16 != 0 || box_cols * 2 != 128) {
+  if (((uintptr_t)ptr & 15) != 0 || (cols * esize) % 16 != 0 || box_cols * esize != 128) {
     b2_set_error("tensor map: need a 16-byte aligned base, a row pitch that is a multiple of 16 bytes "
                  "and a 128-byte box row");
     return 1;
   }
   cuuint64_t dims[2] = {(cuuint64_t)cols, (cuuint64_t)rows};
-  cuuint64_t strides[1] = {(cuuint64_t)cols * 2};
+  cuuint64_t strides[1] = {(cuuint64_t)cols * esize};
   cuuint32_t box[2] = {box_cols, box_rows};
   cuuint32_t estr[2] = {1, 1};
-  CUresult r = p_cuTensorMapEncodeTiled(out, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(ptr),
+  CUresult r = p_cuTensorMapEncodeTiled(out, type, 2, const_cast<void*>(ptr),
                                         dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
                                         CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                                         CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
@@ -551,6 +551,15 @@ extern "C" int b2_tensor_map_2d_bf16(CUtensorMap* out, const void* ptr, unsigned
     return 1;
   }
   return 0;
+}
+extern "C" int b2_tensor_map_2d_bf16(CUtensorMap* out, const void* ptr, unsigned long long rows,
+                                     unsigned long long cols, unsigned box_rows, unsigned box_cols) {
+  return tensor_map_2d(out, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, ptr, rows, cols, box_rows, box_cols);
+}
+// one-byte elements (float8): the TMA copies bytes, the wgmma reads them as e4m3
+extern "C" int b2_tensor_map_2d_u8(CUtensorMap* out, const void* ptr, unsigned long long rows,
+                                   unsigned long long cols, unsigned box_rows, unsigned box_cols) {
+  return tensor_map_2d(out, CU_TENSOR_MAP_DATA_TYPE_UINT8, 1, ptr, rows, cols, box_rows, box_cols);
 }
 
 // Layout record for the import-time ABI check (mpi4jax_b200/_src/native/__init__.py): the Python

@@ -221,6 +221,15 @@ int b2_gemm_reduce_scatter(B2Comm* c, const void* A, const void* B, void* out, i
 // shards are pushed into the staging while the GEMM runs; no multicast
 int b2_gemm_allgather(B2Comm* c, const void* x_local, const void* w, void* out, int m, int N, int K,
                       cudaStream_t stream);
+// ... and their scaled float8 twins (b2_gemm_f8.cu): e4m3 operands, K a multiple of 128, bf16 output; each
+// rank's partial (i, j) is rn_bf16(S[i, j] * (sx[i * sx_inc] * sw[j * sw_inc])), fp32 scales read on the device
+// (inc 0: one per tensor, 1: one per row of A / x_local, one per column of the output)
+int b2_gemm_allreduce_f8(B2Comm* c, const void* A, const void* B, void* out, int M, int N, int K, const float* sx,
+                         int sx_inc, const float* sw, int sw_inc, cudaStream_t stream);
+int b2_gemm_reduce_scatter_f8(B2Comm* c, const void* A, const void* B, void* out, int M, int N, int K,
+                              const float* sx, int sx_inc, const float* sw, int sw_inc, cudaStream_t stream);
+int b2_gemm_allgather_f8(B2Comm* c, const void* x_local, const void* w, void* out, int m, int N, int K,
+                         const float* sx, int sx_inc, const float* sw, int sw_inc, cudaStream_t stream);
 
 // --- fused halo exchange + shallow-water stencils (see b2_halo.cu, b2_swe.cu) --
 struct B2HaloDesc {
@@ -293,6 +302,8 @@ B2DebugScope* b2_debug_begin(B2Comm* c, const char* opname, cudaStream_t stream,
 void b2_debug_end(B2DebugScope* s, int code);
 int b2_tensor_map_2d_bf16(CUtensorMap* out, const void* ptr, unsigned long long rows, unsigned long long cols,
                           unsigned box_rows, unsigned box_cols);
+int b2_tensor_map_2d_u8(CUtensorMap* out, const void* ptr, unsigned long long rows, unsigned long long cols,
+                        unsigned box_rows, unsigned box_cols);
 
 #ifdef __cplusplus
 }

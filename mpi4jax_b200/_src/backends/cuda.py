@@ -759,6 +759,55 @@ class NativeComm:
         self._check(rc, "Allgather")
         return out
 
+    # -- scaled float8 twins (csrc/b2_gemm_f8.cu): e4m3 ``x`` and ``weight``, K a multiple of 128, bf16 out;
+    # ``scale_x`` / ``scale_w`` are float32 with one element (per tensor) or one per row of x / row of weight
+    def gemm_allreduce_f8(self, x: torch.Tensor, weight: torch.Tensor, scale_x: torch.Tensor,
+                          scale_w: torch.Tensor) -> torch.Tensor:
+        """``allreduce_SUM(rn_bf16((x @ weight.T) * scale_x[:, None] * scale_w))`` in ONE kernel."""
+        M, K = x.shape
+        N = weight.shape[0]
+        out = torch.empty((M, N), dtype=torch.bfloat16, device=x.device)
+        if self.comm.size > 1:
+            if not self.has_nvls:
+                raise MPIError("gemm_allreduce_f8 needs NVLS multicast support")
+            self.ensure_stage(codes.OPC_ALLREDUCE, M * N * 2)
+        rc = _lib().b2_gemm_allreduce_f8(self.handle, x.data_ptr(), weight.data_ptr(), out.data_ptr(), M, N, K,
+                                         *_scale_args(scale_x, scale_w), self._stream())
+        self._check(rc, "Allreduce")
+        return out
+
+    def gemm_reduce_scatter_f8(self, x: torch.Tensor, weight: torch.Tensor, scale_x: torch.Tensor,
+                               scale_w: torch.Tensor) -> torch.Tensor:
+        """This rank's ``(M / size, N)`` row shard of :meth:`gemm_allreduce_f8`'s sum, in ONE kernel."""
+        M, K = x.shape
+        N = weight.shape[0]
+        P = self.comm.size
+        if M % P:
+            raise ValueError(f"gemm_reduce_scatter_f8: M = {M} is not divisible by the {P} ranks")
+        out = torch.empty((M // P, N), dtype=torch.bfloat16, device=x.device)
+        if P > 1:
+            self.ensure_stage(codes.OPC_REDUCE_SCATTER, M * N * 2 // P)
+        rc = _lib().b2_gemm_reduce_scatter_f8(self.handle, x.data_ptr(), weight.data_ptr(), out.data_ptr(), M, N, K,
+                                              *_scale_args(scale_x, scale_w), self._stream())
+        self._check(rc, "Reduce_scatter_block")
+        return out
+
+    def gemm_allgather_f8(self, x: torch.Tensor, weight: torch.Tensor, scale_x: torch.Tensor,
+                          scale_w: torch.Tensor) -> torch.Tensor:
+        """Row ``q m + i`` = ``rn_bf16((X @ weight.T)[q m + i] * scale_x_q[i] * scale_w)``, X the gathered
+        ``x (m, K)`` of every rank; each rank's row scales are gathered with its rows, in ONE kernel."""
+        m, K = x.shape
+        N = weight.shape[0]
+        P = self.comm.size
+        out = torch.empty((P * m, N), dtype=torch.bfloat16, device=x.device)
+        if P > 1:
+            # the gathered matrix, then its row scales at a 16-byte aligned offset, per parity
+            self.ensure_stage(codes.OPC_ALLGATHER, (P * m * K + 15) // 16 * 16 + P * m * 4)
+        rc = _lib().b2_gemm_allgather_f8(self.handle, x.data_ptr(), weight.data_ptr(), out.data_ptr(), m, N, K,
+                                         *_scale_args(scale_x, scale_w), self._stream())
+        self._check(rc, "Allgather")
+        return out
+
     # -- fused halo exchange ---------------------------------------------------------
     def halo_exchange(self, fields, kinds, west, east, south, north, periodic_x=True,
                       at_east_wall=False, at_north_wall=False, sw=-1, se=-1, nw=-1, ne=-1) -> None:
@@ -801,10 +850,17 @@ NVTX_OPS = ("barrier", "allreduce", "reduce", "scan", "allgather", "alltoall", "
             "send", "recv", "sendrecv", "reduce_scatter", "alltoallv", "allgatherv", "reduce_scatterv", "gatherv",
             "scatterv", "reduce_loc",
             "gemm_allreduce", "gemm_reduce_scatter", "gemm_allgather",
+            "gemm_allreduce_f8", "gemm_reduce_scatter_f8", "gemm_allgather_f8",
             "halo_exchange")
 if env_flag("MPI4JAX_B200_NVTX", False):
     for _name in NVTX_OPS:
         setattr(NativeComm, _name, _nvtx_wrap(_name, getattr(NativeComm, _name)))
+
+
+def _scale_args(scale_x: torch.Tensor, scale_w: torch.Tensor):
+    """(sx, sx_inc, sw, sw_inc) of the float8 GEMM entry points: a contiguous float32 scale tensor is read with
+    an increment of 0 when it has one element, 1 otherwise."""
+    return (scale_x.data_ptr(), int(scale_x.numel() > 1), scale_w.data_ptr(), int(scale_w.numel() > 1))
 
 
 class _NullEvent:

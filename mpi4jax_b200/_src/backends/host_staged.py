@@ -149,5 +149,14 @@ class HostStagedComm:
     def gemm_allgather(self, *a, **k):
         self._unsupported("the fused allgather + GEMM kernel")
 
+    def gemm_allreduce_f8(self, *a, **k):
+        self._unsupported("the fused float8 GEMM + allreduce kernel")
+
+    def gemm_reduce_scatter_f8(self, *a, **k):
+        self._unsupported("the fused float8 GEMM + reduce-scatter kernel")
+
+    def gemm_allgather_f8(self, *a, **k):
+        self._unsupported("the fused float8 allgather + GEMM kernel")
+
     def halo_exchange(self, *a, **k):
         self._unsupported("the fused halo-exchange kernel")

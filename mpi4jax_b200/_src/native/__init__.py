@@ -215,6 +215,15 @@ _SIGNATURES = {
     "b2_gemm_allreduce": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p]),
     "b2_gemm_reduce_scatter": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p]),
     "b2_gemm_allgather": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p]),
+    "b2_gemm_allreduce_f8": (
+        c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_int, c_void_p, c_int, c_void_p],
+    ),
+    "b2_gemm_reduce_scatter_f8": (
+        c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_int, c_void_p, c_int, c_void_p],
+    ),
+    "b2_gemm_allgather_f8": (
+        c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_int, c_void_p, c_int, c_void_p],
+    ),
     "b2_halo_exchange": (c_int, [c_void_p, POINTER(B2HaloDesc), c_void_p]),
     "b2_swe_multistep_ca": (
         c_int,

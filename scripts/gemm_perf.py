@@ -1,5 +1,7 @@
 """Fused wgmma GEMM+allreduce vs cuBLAS GEMM followed by an allreduce (ours / NCCL), and for M divisible by
-the world size the same for GEMM+reduce-scatter over the rows and for allgather (of M / P rows per rank)+GEMM."""
+the world size the same for GEMM+reduce-scatter over the rows and for allgather (of M / P rows per rank)+GEMM.
+Then the same in scaled float8 (e4m3, bf16 out) against torch._scaled_mm with fast accumulation; at world size
+1 the fused rows are the stand-alone float8 GEMM.  The first line names the card and its power limit."""
 import os
 import sys
 
@@ -31,6 +33,15 @@ def timeit(fn, iters=10):
     e.synchronize()
     return max_over_ranks(s.elapsed_time(e) / iters * 1e3, comm)
 
+
+if rank == 0:
+    try:
+        import subprocess
+        q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader", "-i",
+                            str(dev.index or 0)], capture_output=True, text=True, timeout=30).stdout.strip()
+    except (OSError, subprocess.SubprocessError):
+        q = torch.cuda.get_device_name(dev)
+    print(f"device: {q}", flush=True)
 
 for (M, N, K) in [(4096, 4096, 4096 // size), (8192, 8192, 8192 // size), (8192, 4096, 1024), (2048, 4096, 4096)]:
     x = torch.randn(M, K, device=dev).bfloat16()
@@ -66,6 +77,39 @@ for (M, N, K) in [(4096, 4096, 4096 // size), (8192, 8192, 8192 // size), (8192,
                 return X @ w.t()
             rows["nccl all_gather_into_tensor + cublas"] = timeit(h)
     rows["cublas gemm only"] = timeit(lambda: x @ w.t())
+    # scaled float8 (e4m3): the fused kernels, torch._scaled_mm (fast accumulation) + our collective, and + NCCL
+    x8, w8 = x.to(torch.float8_e4m3fn), w.to(torch.float8_e4m3fn)
+    sx, sw = torch.ones(M, 1, device=dev), torch.ones(1, N, device=dev)     # _scaled_mm's row-wise scale shapes
+    sxv, swv = sx.reshape(M), sw.reshape(N)
+
+    def smm(a, sa):
+        return torch._scaled_mm(a, w8.t(), scale_a=sa, scale_b=sw, out_dtype=torch.bfloat16, use_fast_accum=True)
+
+    rows["f8 fused wgmma+NVLS (one kernel)"] = timeit(
+        lambda: linear_allreduce(x8, w8, comm=comm, scale_x=sxv, scale_w=swv))
+    rows["f8 _scaled_mm + our allreduce"] = timeit(lambda: m.allreduce(smm(x8, sx), MPI.SUM, comm=comm))
+    if nccl is not None:
+        def f8():
+            y = smm(x8, sx)
+            dist.all_reduce(y, group=nccl)
+            return y
+        rows["f8 _scaled_mm + nccl allreduce"] = timeit(f8)
+    if M % size == 0 and size > 1:
+        rows["f8 fused wgmma+reduce-scatter (one kernel)"] = timeit(
+            lambda: linear_reduce_scatter(x8, w8, comm=comm, scale_x=sxv, scale_w=swv))
+        x8s, sxs = x8[:M // size].contiguous(), sxv[:M // size]
+        rows["f8 fused allgather+wgmma (one kernel)"] = timeit(
+            lambda: linear_allgather(x8s, w8, comm=comm, scale_x=sxs, scale_w=swv))
+        rows["f8 our allgather + _scaled_mm"] = timeit(
+            lambda: smm(m.allgather(x8s.view(torch.uint8), comm=comm).reshape(M, K).view(torch.float8_e4m3fn),
+                        m.allgather(sxs, comm=comm).reshape(M, 1)))
+        if nccl is not None:
+            def h8():
+                X = torch.empty(M, K, device=dev, dtype=torch.uint8)
+                dist.all_gather_into_tensor(X, x8s.view(torch.uint8), group=nccl)
+                return smm(X.view(torch.float8_e4m3fn), sx)
+            rows["f8 nccl all_gather_into_tensor + _scaled_mm"] = timeit(h8)
+    rows["f8 _scaled_mm only"] = timeit(lambda: smm(x8, sx))
     if rank == 0:
         print(f"M={M} N={N} K/rank={K} (bf16 out {M * N * 2 / 2**20:.0f} MiB): " +
               "; ".join(f"{k} {v:.1f} us ({flops / v / 1e6:.0f} TF/s/GPU)" for k, v in rows.items()), flush=True)
