@@ -746,6 +746,9 @@ extern "C" size_t b2_stage_need(int opcode, int nranks, size_t blk_bytes) {
       return B2_A2AV_HDR + stride + 4096;
     case B2_OPC_REDUCE_SCATTERV:                 // blk_bytes: the output rows N x row bytes, one block per rank
       return B2_A2AV_HDR + stride * (size_t)nranks + 4096;
+    case B2_OPC_MOE_DISPATCH:                    // blk_bytes: the N x k pair rows, behind the E send counts
+      return B2_MOE_HDR + stride + 4096;
+    // B2_OPC_MOE_COMBINE (blk_bytes: the R expert-side rows) takes the default
     default:
       return stride + 4096;
   }
@@ -763,6 +766,12 @@ static int plan_staged(B2Comm* c, int opcode, size_t blk_bytes, const void* kern
   }
   pick_chunks(c, blk_bytes, coresident_blocks(c, kernel), chunk, grid);
   return 0;
+}
+
+// plan_staged for the kernels of other translation units (b2_moe.cu)
+int b2_plan_staged(B2Comm* c, int opcode, size_t blk_bytes, const void* kernel, const char* name, size_t* chunk,
+                   int* grid) {
+  return plan_staged(c, opcode, blk_bytes, kernel, name, chunk, grid);
 }
 
 static int check_root(const B2Comm* c, int root, const char* name) {

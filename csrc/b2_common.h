@@ -16,11 +16,15 @@
 #include <cstddef>
 #include <cstdint>
 
-#define B2_ABI_VERSION 20  // bump whenever a struct shared with Python or a C signature changes
+#define B2_ABI_VERSION 21  // bump whenever a struct shared with Python or a C signature changes
 #define B2_MAX_RANKS 16          // ranks per NVLink domain we support (8 on HGX H100)
 // bytes of the count header in front of the rows the variable-count collectives stage: one int64
 // per possible rank (keeps the rows 16-byte aligned)
 #define B2_A2AV_HDR ((size_t)B2_MAX_RANKS * sizeof(long long))
+// experts of a top-k dispatch (b2_moe.cu): every CTA keeps the P x E send counts of all ranks in shared memory,
+// and the sender's header holds its E counts in front of its rows (2 KiB, keeps the rows 16-byte aligned)
+#define B2_MOE_MAX_EXPERTS 256
+#define B2_MOE_HDR ((size_t)B2_MOE_MAX_EXPERTS * sizeof(long long))
 #define B2_MAX_BLOCKS 1024       // max CTAs per collective launch (flag rows)
 #define B2_P2P_NSLOT 8           // ring slots per directed pair
 #define B2_P2P_MAX_LANES 64      // CTAs cooperating on one p2p message
@@ -96,7 +100,7 @@ enum B2OpCode : int {
   B2_OPC_BARRIER = 0, B2_OPC_ALLREDUCE, B2_OPC_REDUCE, B2_OPC_SCAN, B2_OPC_ALLGATHER,
   B2_OPC_ALLTOALL, B2_OPC_BCAST, B2_OPC_GATHER, B2_OPC_SCATTER, B2_OPC_SEND, B2_OPC_RECV,
   B2_OPC_SENDRECV, B2_OPC_HALO, B2_OPC_REDUCE_SCATTER, B2_OPC_ALLTOALLV, B2_OPC_ALLGATHERV,
-  B2_OPC_REDUCE_SCATTERV, B2_OPC_GATHERV, B2_OPC_SCATTERV, B2_OPC_COUNT
+  B2_OPC_REDUCE_SCATTERV, B2_OPC_GATHERV, B2_OPC_SCATTERV, B2_OPC_MOE_DISPATCH, B2_OPC_MOE_COMBINE, B2_OPC_COUNT
 };
 
 static inline size_t b2_dtype_size(int dt) {
@@ -144,6 +148,7 @@ struct B2Layout {
 enum B2TicketWord : int {
   TK_COLL = 0,        // collective ticket: staging parity and flag values, advanced once per launch
   TK_COLL_FIN = 1,    // finish counter of the collective kernels
+  TK_GRID = 2,        // [2] grid-wide wait of the MoE combine kernel: arrivals, then the launch's release value
   TK_FIN = 6,         // finish counter of the halo kernels
   TK_RX = 32,         // [8] halo messages received per side
   TK_TX = 40,         // [8] halo messages sent per side

@@ -235,6 +235,20 @@ __device__ __forceinline__ bool b2_last_arrival(unsigned* ctr, unsigned nblocks)
   return last;
 }
 
+// Grid-wide wait of a launch whose CTAs are all resident at once (plan_staged's grid): returns in every CTA once
+// all gridDim.x CTAs have called it.  ctr[0] counts the arrivals (zero between launches: the last arrival resets
+// it) and the last arrival publishes `gen` in ctr[1]; `gen` must grow from launch to launch (the staged kernels
+// pass their ticket + 1).  Writes a CTA made before the call, and what it acquired from peers, are visible to
+// every CTA after it.  All threads call.
+__device__ __forceinline__ void b2_grid_wait(const B2DevComm& c, unsigned* ctr, unsigned gen, int opcode) {
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    if (b2_last_arrival(ctr, gridDim.x)) b2_st_release_sys(ctr + 1, gen);
+    else b2_wait_ge(c, ctr + 1, gen, opcode, -1);
+  }
+  __syncthreads();
+}
+
 // All threads call; adds `delta` to *target once every one of `nblocks` CTAs is done.
 __device__ __forceinline__ void b2_finish_bump(unsigned* target, unsigned* ctr, unsigned delta,
                                                unsigned nblocks) {

@@ -494,7 +494,7 @@ static const char* opcode_name(int opc) {
   static const char* names[] = {"Barrier", "Allreduce", "Reduce", "Scan", "Allgather", "Alltoall",
                                 "Bcast", "Gather", "Scatter", "Send", "Recv", "Sendrecv", "Halo",
                                 "Reduce_scatter_block", "Alltoallv", "Allgatherv", "Reduce_scatterv", "Gatherv",
-                                "Scatterv"};
+                                "Scatterv", "Moe_dispatch", "Moe_combine"};
   if (opc < 0 || opc >= B2_OPC_COUNT) return "Unknown";
   return names[opc];
 }

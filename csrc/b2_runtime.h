@@ -197,6 +197,26 @@ int b2_reduce_scatterv(B2Comm* c, const void* in, void* out, size_t row_bytes, s
 // always one of the inputs; reduce writes them on `root` only.  Pairs fold in rank order (see b2_reduce_loc.cu).
 int b2_reduce_loc(B2Comm* c, const void* in_val, const void* in_idx, void* out_val, void* out_idx, size_t count,
                   int val_dtype, int idx_bytes, int op, int opcode, int root, cudaStream_t stream);
+// Top-k expert dispatch (b2_moe.cu).  `order` [n_pairs] int64: the pair (t * k + j) at each position of this
+// rank's pairs sorted by expert; `send_counts` [num_experts] int64: the sorted pairs of each expert, clamped in
+// expert order to n_pairs (the pairs past their sum go nowhere).  Sorted pair s carries row order[s] / k of `in`
+// (k = 1: row order[s], the pair mode).  Expert e lives on rank e / L (L = num_experts / nranks); rank r's
+// out_rows rows hold, for l = 0..L-1 and then q = 0..nranks-1, the pairs rank q sends to expert r L + l, cut
+// at out_rows, then zeros.  recv_counts [L x nranks], pos and dest [n_pairs] (this rank's pairs: the row and
+// rank they landed in, -1 if dropped) are written unless null.  n_pairs, row_bytes, num_experts and out_rows
+// must be the same on every rank.
+int b2_moe_dispatch(B2Comm* c, const void* in, void* out, size_t row_bytes, size_t n_pairs, int k,
+                    const long long* order, const long long* send_counts, int num_experts, size_t out_rows,
+                    long long* recv_counts, long long* pos, long long* dest, cudaStream_t stream);
+// Top-k expert combine (b2_moe.cu): token t of `out` (tokens rows of row_bytes) is the fold over its k pairs,
+// slot order, of weights[t k + j] * (row pos[t k + j] of rank dest[t k + j]'s `in`), pairs with dest -1
+// skipped: fp32 (f64 for f64) products and sums, rounded once, +0 for a token with none.  `weights` null:
+// unit weights.  pairs != 0: out holds the tokens x k pair rows unfolded and unweighted (zeros where dropped).
+// Each rank stages the first sum(recv_counts[0..n_counts)) of its in_rows rows; in_rows, row_bytes, tokens, k
+// and dtype (f32, f64, f16 or bf16) must be the same on every rank.
+int b2_moe_combine(B2Comm* c, const void* in, void* out, size_t row_bytes, size_t in_rows, size_t tokens, int k,
+                   const long long* pos, const long long* dest, const float* weights, const long long* recv_counts,
+                   int n_counts, int dtype, int pairs, cudaStream_t stream);
 
 // --- point to point ----------------------------------------------------------
 // source/tag may be -1 (ANY).  `status` is a host-mapped B2StatusRecord or null.
@@ -292,6 +312,9 @@ void b2_set_error(const char* fmt, ...) __attribute__((format(printf, 1, 2)));
 int b2_cuda_check(cudaError_t e, const char* fmt, ...) __attribute__((format(printf, 2, 3)));
 // after a kernel launch: counts it (b2_launch_count), then b2_cuda_check(cudaGetLastError(), "<name>: kernel launch failed")
 int b2_launched(B2Comm* c, const char* name);
+// the staging check and launch geometry of a staged kernel (b2_collectives.cu)
+int b2_plan_staged(B2Comm* c, int opcode, size_t blk_bytes, const void* kernel, const char* name, size_t* chunk,
+                   int* grid);
 // argument checks shared by the halo exchanges (b2_halo.cu): 0, or B2_ERR_BAD_ARG with the error "<what>: ..."
 int b2_halo_check_ranks(B2Comm* c, const B2HaloDesc* d, const char* what);
 int b2_halo_check_cap(B2Comm* c, int nfields, int depth, int ny, int nx, const char* what);

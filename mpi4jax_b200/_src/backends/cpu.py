@@ -15,6 +15,7 @@ GPU-less CI box.  The image has no MPI, so gloo carries the bytes; semantics fol
 
 from __future__ import annotations
 
+import itertools
 import time
 from collections import deque
 from typing import Optional
@@ -317,6 +318,76 @@ def scatterv(comm: Comm, x: torch.Tensor, send_counts: Optional[torch.Tensor], r
     d = sum(sent[:r])
     out[:k] = rows[d: d + k]
     return out, torch.tensor(k, dtype=torch.int64)
+
+
+def moe_dispatch(comm: Comm, x: torch.Tensor, order: torch.Tensor, send_counts: torch.Tensor, k: int,
+                 num_experts: int, out_rows: int, with_plan: bool = True):
+    """Same rules as the kernel (csrc/b2_moe.cu: b2_k_moe_dispatch): everybody gathers every rank's per-expert
+    counts, clamped in expert order, and its sorted pair rows, then assembles the rows of its own experts and
+    works out where its own pairs landed (correctness path).  ``(rows, recv_counts (L, P), pos, dest)``, the last
+    three None unless ``with_plan``."""
+    P, r = comm.size, comm.rank
+    L = num_experts // P
+    n = order.shape[0]
+    raw = x.view(torch.uint8) if x.dtype in codes.FP8_DTYPE_CODE else x      # index ops do not all take float8
+    counts, stack = _gather_segments(comm, raw[order // k], send_counts.tolist(), n)
+    first = [[0, *itertools.accumulate(row)] for row in counts]              # [q][e]: q's first sorted pair of e
+    tot = [sum(counts[q][e] for q in range(P)) for e in range(num_experts)]
+    land = [0] * num_experts                                                 # [e]: the owner's first row of e
+    for e in range(num_experts):
+        land[e] = 0 if e % L == 0 else land[e - 1] + tot[e - 1]
+    out = torch.zeros((out_rows, *x.shape[1:]), dtype=raw.dtype)
+    recv = torch.zeros((L, P), dtype=torch.int64)
+    for l in range(L):
+        at = land[r * L + l]
+        for q in range(P):
+            c = counts[q][r * L + l]
+            kk = max(0, min(c, out_rows - at))
+            d = first[q][r * L + l]
+            out[at: at + kk] = stack[q, d: d + kk]
+            recv[l, q] = kk
+            at += c
+    out = out.view(x.dtype)
+    if not with_plan:
+        return out, None, None, None
+    pos = torch.full((n,), -1, dtype=torch.int64)
+    dest = torch.full((n,), -1, dtype=torch.int64)
+    for e in range(num_experts):
+        at = land[e] + sum(counts[q][e] for q in range(r))
+        kk = max(0, min(counts[r][e], out_rows - at))
+        pairs = order[first[r][e]: first[r][e] + kk]
+        pos[pairs] = torch.arange(at, at + kk)
+        dest[pairs] = e // L
+    return out, recv, pos, dest
+
+
+def moe_combine(comm: Comm, y: torch.Tensor, pos: torch.Tensor, dest: torch.Tensor, weights: Optional[torch.Tensor],
+                recv_counts: torch.Tensor, pairs: bool = False) -> torch.Tensor:
+    """Same rules as the kernel (csrc/b2_moe.cu: b2_k_moe_combine): everybody gathers every rank's rows; token t
+    folds the rows of its delivered pairs in slot order, products and sums as separate round-to-nearest fp32
+    operations (f64 for f64), starting from the first product, rounded once (correctness path).  ``pairs``: the
+    ``(N, k, ...)`` rows unfolded and unweighted, zeros where dropped."""
+    P, R = comm.size, y.shape[0]
+    N, k = pos.shape
+    stack = _gather_stack(comm, y)                                           # (P, R, *S')
+    ok = (dest >= 0) & (dest < P) & (pos >= 0) & (pos < R)
+    if R == 0:
+        rows = torch.zeros((N, k, *y.shape[1:]), dtype=y.dtype)
+    else:
+        rows = stack[dest.clamp(0, P - 1), pos.clamp(0, R - 1)]             # (N, k, *S')
+    bcast = (N, *[1] * (y.dim() - 1))
+    if pairs:
+        return torch.where(ok.view(N, k, *bcast[1:]), rows, torch.zeros((), dtype=y.dtype))
+    acc_dt = torch.float64 if y.dtype == torch.float64 else torch.float32
+    acc = torch.zeros((N, *y.shape[1:]), dtype=acc_dt)
+    started = torch.zeros(N, dtype=torch.bool)
+    for j in range(k):
+        term = rows[:, j].to(acc_dt)
+        if weights is not None:
+            term = weights[:, j].to(acc_dt).view(bcast) * term
+        acc = torch.where(ok[:, j].view(bcast), torch.where(started.view(bcast), acc + term, term), acc)
+        started |= ok[:, j]
+    return acc.to(y.dtype)
 
 
 def bcast(comm: Comm, x: torch.Tensor, root: int) -> torch.Tensor:

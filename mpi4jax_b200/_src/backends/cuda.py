@@ -66,6 +66,8 @@ def stage_need(opcode: int, nranks: int, blk_bytes: int) -> int:
         return ALLTOALLV_HEADER + stride + 4096
     if opcode == codes.OPC_REDUCE_SCATTERV:                        # the header, then one block per rank
         return ALLTOALLV_HEADER + stride * nranks + 4096
+    if opcode == codes.OPC_MOE_DISPATCH:                           # the E send counts, then the pair rows
+        return codes.MOE_MAX_EXPERTS * 8 + stride + 4096
     mult = nranks if opcode in (codes.OPC_ALLTOALL, codes.OPC_SCATTER, codes.OPC_REDUCE_SCATTER) else 1
     return stride * mult + 4096
 
@@ -657,6 +659,46 @@ class NativeComm:
                 recv_counts.data_ptr(), *extra, self._stream())
         self._check(rc, opname)
         return out, recv_counts
+
+    # -- top-k expert routing (csrc/b2_moe.cu; ops/moe.py states the rules) ----------------------------
+    def moe_dispatch(self, x: torch.Tensor, order: torch.Tensor, send_counts: torch.Tensor, k: int, num_experts: int,
+                     out_rows: int, with_plan: bool = True):
+        """``(rows, recv_counts (L, P), pos, dest)``: sorted pair s of this rank carries row ``order[s] // k`` of
+        ``x`` to the owner of its expert.  ``with_plan`` False: only the rows (a replay of a dispatch whose
+        counts, pos and dest are known)."""
+        x = _prep(x)
+        P = self.comm.size
+        n_pairs = order.shape[0]
+        row_bytes = math.prod(x.shape[1:]) * x.element_size()
+        out = torch.empty((out_rows, *x.shape[1:]), dtype=x.dtype, device=x.device)
+        plan = None
+        if with_plan:
+            plan = (torch.empty((num_experts // P, P), dtype=torch.int64, device=x.device),
+                    torch.empty(n_pairs, dtype=torch.int64, device=x.device),
+                    torch.empty(n_pairs, dtype=torch.int64, device=x.device))
+        self.ensure_stage(codes.OPC_MOE_DISPATCH, n_pairs * row_bytes)
+        rc = _lib().b2_moe_dispatch(self.handle, x.data_ptr(), out.data_ptr(), row_bytes, n_pairs, k,
+                                    order.data_ptr(), send_counts.data_ptr(), num_experts, out_rows,
+                                    *((None, None, None) if plan is None else (t.data_ptr() for t in plan)),
+                                    self._stream())
+        self._check(rc, "Moe_dispatch")
+        return (out, None, None, None) if plan is None else (out, *plan)
+
+    def moe_combine(self, y: torch.Tensor, pos: torch.Tensor, dest: torch.Tensor, weights: Optional[torch.Tensor],
+                    recv_counts: torch.Tensor, pairs: bool = False) -> torch.Tensor:
+        """Token t: its delivered pairs' rows of the owners' ``y``, weighted and folded in slot order; ``pairs``:
+        the ``(N, k, ...)`` rows unfolded (zeros where dropped)."""
+        y = _prep(y)
+        N, k = pos.shape
+        row_bytes = math.prod(y.shape[1:]) * y.element_size()
+        out = torch.empty((N, k, *y.shape[1:]) if pairs else (N, *y.shape[1:]), dtype=y.dtype, device=y.device)
+        self.ensure_stage(codes.OPC_MOE_COMBINE, y.shape[0] * row_bytes)
+        rc = _lib().b2_moe_combine(self.handle, y.data_ptr(), out.data_ptr(), row_bytes, y.shape[0], N, k,
+                                   pos.data_ptr(), dest.data_ptr(), None if weights is None else weights.data_ptr(),
+                                   recv_counts.data_ptr(), recv_counts.numel(), codes.DTYPE_CODE[y.dtype],
+                                   1 if pairs else 0, self._stream())
+        self._check(rc, "Moe_combine")
+        return out
 
     # -- point to point ------------------------------------------------------------
     def _status_record(self, status: Optional[Status], itemsize: int):

@@ -116,6 +116,15 @@ class HostStagedComm:
     def scatterv(self, x, send_counts, root: int, out_rows: int, max_rows: int):
         return self._rowsv(_cpu.scatterv, x, send_counts, root, out_rows, max_rows)
 
+    def moe_dispatch(self, x, order, send_counts, k: int, num_experts: int, out_rows: int, with_plan: bool = True):
+        outs = _cpu.moe_dispatch(self.comm, self._down(x), self._down(order), self._down(send_counts), k, num_experts,
+                                 out_rows, with_plan)
+        return tuple(self._up(o, x) for o in outs)
+
+    def moe_combine(self, y, pos, dest, weights, recv_counts, pairs: bool = False):
+        args = [None if t is None else self._down(t) for t in (y, pos, dest, weights, recv_counts)]
+        return self._up(_cpu.moe_combine(self.comm, *args, pairs), y)
+
     def bcast(self, x, root: int):
         out = _cpu.bcast(self.comm, self._down(x), root)
         return x if self.comm.rank == root else self._up(out, x)

@@ -272,6 +272,26 @@ def scatterv(comm: Comm, x: torch.Tensor, send_counts: Optional[torch.Tensor], r
                    out_rows, max_rows)
 
 
+def moe_dispatch(comm: Comm, x: torch.Tensor, order: torch.Tensor, send_counts: torch.Tensor, k: int,
+                 num_experts: int, out_rows: int, with_plan: bool = True):
+    """``(rows, recv_counts, pos, dest)`` of a top-k dispatch whose pairs are already sorted (ops/moe.py states
+    the rules); ``with_plan`` False: the rows only, the rest None."""
+    _plain(x)
+    if x.is_cuda:
+        return comm._native_comm().moe_dispatch(x, order, send_counts, k, num_experts, out_rows, with_plan)
+    return _on_cpu(comm, "Moe_dispatch", f"with {order.shape[0]} pairs to {num_experts} experts", _cpu.moe_dispatch,
+                   x, order, send_counts, k, num_experts, out_rows, with_plan)
+
+
+def moe_combine(comm: Comm, y: torch.Tensor, pos: torch.Tensor, dest: torch.Tensor, weights: Optional[torch.Tensor],
+                recv_counts: torch.Tensor, pairs: bool = False) -> torch.Tensor:
+    _plain(y)
+    if y.is_cuda:
+        return comm._native_comm().moe_combine(y, pos, dest, weights, recv_counts, pairs)
+    return _on_cpu(comm, "Moe_combine", f"with {pos.shape[0]} tokens x {pos.shape[1]} pairs", _cpu.moe_combine, y,
+                   pos, dest, weights, recv_counts, pairs)
+
+
 def bcast(comm: Comm, x: torch.Tensor, root: int) -> torch.Tensor:
     _plain(x)
     if x.is_cuda:

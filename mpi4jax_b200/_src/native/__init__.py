@@ -202,6 +202,16 @@ _SIGNATURES = {
         c_int,
         [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_size_t, c_int, c_int, c_int, c_int, c_int, c_void_p],
     ),
+    "b2_moe_dispatch": (
+        c_int,
+        [c_void_p, c_void_p, c_void_p, c_size_t, c_size_t, c_int, c_void_p, c_void_p, c_int, c_size_t, c_void_p,
+         c_void_p, c_void_p, c_void_p],
+    ),
+    "b2_moe_combine": (
+        c_int,
+        [c_void_p, c_void_p, c_void_p, c_size_t, c_size_t, c_size_t, c_int, c_void_p, c_void_p, c_void_p, c_void_p,
+         c_int, c_int, c_int, c_void_p],
+    ),
     "b2_status_alloc": (POINTER(B2StatusRecord), []),
     "b2_status_free": (None, [POINTER(B2StatusRecord)]),
     "b2_send": (c_int, [c_void_p, c_void_p, c_size_t, c_int, c_int, c_void_p]),
@@ -243,7 +253,7 @@ _SIGNATURES = {
 
 
 #: must equal B2_ABI_VERSION in csrc/b2_common.h
-ABI_VERSION = 20
+ABI_VERSION = 21
 #: must equal B2_MAX_RANKS in csrc/b2_common.h (ranks per communicator; sizes the alltoallv count header)
 MAX_RANKS = 16
 _ABI_FIELDS = ("abi_version", "sizeof_status_record", "sizeof_halo_desc", "sizeof_swe_params",

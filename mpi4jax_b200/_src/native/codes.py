@@ -59,6 +59,12 @@ OPC_ALLGATHERV = 15
 OPC_REDUCE_SCATTERV = 16
 OPC_GATHERV = 17
 OPC_SCATTERV = 18
+OPC_MOE_DISPATCH = 19
+OPC_MOE_COMBINE = 20
+
+# experts a top-k dispatch may route to (B2_MOE_MAX_EXPERTS: the kernel keeps every rank's per-expert counts in
+# shared memory)
+MOE_MAX_EXPERTS = 256
 
 # MPI names of the reduction collectives (debug log lines, error messages)
 OPC_REDUCTION_NAME = {OPC_ALLREDUCE: "Allreduce", OPC_REDUCE: "Reduce", OPC_SCAN: "Scan",

@@ -1,5 +1,6 @@
 """Functional op namespace: the 15 primitives plus the fused ops that go beyond the
-reference's one-MPI-call-per-op model (fused multi-field halo exchange)."""
+reference's one-MPI-call-per-op model (fused multi-field halo exchange, the fused linear layers and top-k
+expert routing)."""
 
 from .._src import (  # noqa: F401
     allgather, allgatherv, allreduce, alltoall, alltoallv, barrier, bcast, gather, gatherv, recv, reduce,
@@ -7,3 +8,4 @@ from .._src import (  # noqa: F401
 )
 from .halo import halo_exchange  # noqa: F401
 from .linear import linear_allgather, linear_allreduce, linear_reduce_scatter  # noqa: F401
+from .moe import MoePlan, moe_combine, moe_dispatch  # noqa: F401
